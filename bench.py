@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — reprojection residuals/sec and LM iterations/sec of the bundle-adjustment hot path.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--workload cfg4] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--workload cfg4] [--impl ours|reference] [--dump-outputs DIR]
 
 One "step" = one full `bundle_adjust()` (calibration.py:199-212 semantics: ftol=1e-4, max_nfev=100, linear loss) over one
 synthetic scene of the BASELINE.json configuration `--workload`.  Default workload at EVERY N: cfg4 = configs[3] (16 cameras x
@@ -15,9 +15,13 @@ Metric (both arms, same definition):
 `value`  : solves timed on the device with the packed problem already resident in HBM (CUDA events on the solver's stream).
 `e2e`    : the same through the public API `Calibration.bundle_adjust()` from pinned host numpy buffers: packing, H2D, solve, D2H of
            the solved parameters all inside the timed region (wall clock, device synchronised).
-`--impl reference` times the reference's CPU path on the host cores on a bounded frame-subsample of the same workload: the
-unmodified reference (through tests/refshim) where /root/reference exists (the build container), else its numpy + scipy restatement
-oracle/ba_oracle.py (the GPU box: the reference is pure Python and cannot travel); `cpu_baseline.kind` says which.
+`--impl reference` times the reference's CPU path on the host cores on a bounded frame-subsample of the same workload, through its
+numpy + scipy restatement oracle/ba_oracle.py (the identical scipy.optimize.least_squares call).
+`--dump-outputs DIR` writes what the last timed device-resident solve of the main workload computed, as float64 .npy files: the solved
+parameters (cam_rt, board_rt, frame_rt, intrinsics: what Engine.get_params returns) and solve.npy = [cost, initial_cost, optimality,
+nfev, njev, status].  The scene is generated from --seed, so the same arguments give the same inputs on every run.  With --gpus N > 1
+frame_rt holds rank 0's frames.
+The library must have been built by __graft_entry__.build(); the benchmark compiles nothing and writes nothing into the tree.
 """
 import argparse
 import json
@@ -47,51 +51,25 @@ def subsample_frames(scene, frames):
   return s
 
 
-def reference_available():
-  return os.path.isdir("/root/reference/multical") and os.environ.get("MCBA_BENCH_FORCE_PORT") != "1"
-
-
-def cpu_reference_step(scene, use_reference):
-  """One bundle_adjust of the reference's CPU path on the host cores: (residuals/s, seconds, nfev, njev, corners, kind)."""
-  if use_reference:
-    sys.path.insert(0, os.path.join(ROOT, "tests", "refshim"))
-    import loader
-    ref = loader.load()
-    calib = loader.build_calibration(ref, scene).enable(cameras=True)
-    n = int(calib.inliers.sum())
-    count = {"n": 0}
-    import scipy.optimize as so
-    real = so.least_squares
-    res_box = {}
-    def spy(*a, **k):
-      r = real(*a, **k); res_box["r"] = r; return r
-    so.least_squares = spy                    # only to read res.nfev / res.njev: the reference discards the result object
-    try:
-      t = time.perf_counter()
-      calib.bundle_adjust(tolerance=BA_KW["tolerance"], max_iterations=BA_KW["max_iterations"], loss=BA_KW["loss"])      # incl. its sparsity_matrix build
-      dt = time.perf_counter() - t
-    finally:
-      so.least_squares = real
-    r = res_box["r"]
-    return n * (r.nfev + r.njev) / dt, dt, int(r.nfev), int(r.njev), n, "reference"
+def cpu_reference_step(scene):
+  """One bundle_adjust of the reference's CPU path (its numpy + scipy restatement) on the host cores:
+  (residuals/s, seconds, nfev, njev, corners)."""
   from oracle.ba_oracle import Problem
   prob = Problem.from_scene(scene, optimize=dict(cameras=True))
   t = time.perf_counter()
   _, res = prob.bundle_adjust(tolerance=BA_KW["tolerance"], max_iterations=BA_KW["max_iterations"], loss=BA_KW["loss"])
   dt = time.perf_counter() - t
   n = int(prob.inliers.sum())
-  return n * (res.nfev + res.njev) / dt, dt, int(res.nfev), int(res.njev), n, "port"
+  return n * (res.nfev + res.njev) / dt, dt, int(res.nfev), int(res.njev), n
 
 
 def cpu_baseline_block(scene, workload, frames):
   """The CPU baseline on the first `frames` frames of the workload, after a small warm-up call (imports, caches)."""
-  use_ref = reference_available()
   nf = min(scene["F"], frames)
-  cpu_reference_step(subsample_frames(scene, np.arange(min(2, nf))), use_ref)
-  v, dt, nfev, njev, n, kind = cpu_reference_step(subsample_frames(scene, np.arange(nf)), use_ref)
-  what = ("unmodified reference Calibration.bundle_adjust through tests/refshim (incl. its sparsity_matrix build)" if kind == "reference"
-          else "oracle/ba_oracle.py: numpy restatement of evaluate + the identical scipy.optimize.least_squares call (the reference is absent on this box)")
-  return dict(value=v, unit=UNIT, cores=os.cpu_count(), kind=kind,
+  cpu_reference_step(subsample_frames(scene, np.arange(min(2, nf))))
+  v, dt, nfev, njev, n = cpu_reference_step(subsample_frames(scene, np.arange(nf)))
+  what = "oracle/ba_oracle.py: numpy restatement of evaluate + the identical scipy.optimize.least_squares call"
+  return dict(value=v, unit=UNIT, cores=os.cpu_count(), kind="port",
               sample=f"{workload}: first {nf} of {scene['F']} frames ({n} corners), one full bundle_adjust ({nfev} nfev, {njev} njev, {dt:.1f} s); "
                      f"{what}; all {os.cpu_count()} host cores available to numpy / scipy / OpenCV's default thread pools, the Python-level algorithm is serial"), dt, nfev, njev, n
 
@@ -145,18 +123,7 @@ class ClockSampler(threading.Thread):
                 reasons=sorted(self.reasons), samples=len(self.samples), source=self.source)
 
 
-def measured_peak():
-  p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-  if os.path.exists(p):
-    return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-  return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
-def ncu_traffic(workload):
-  p = os.path.join(ROOT, "profiles", "traffic.json")
-  if os.path.exists(p):
-    return json.load(open(p)).get(workload)
-  return None
+HBM_PEAK_GBS = 3350.0      # H100 SXM data sheet: 3.35 TB/s of HBM3 (a peak, not a reached figure)
 
 
 def run_reference(args):
@@ -166,27 +133,26 @@ def run_reference(args):
     return
   scene = synthetic.make_workload(args.workload, seed=args.seed)
   frames = args.ref_frames or REF_FRAMES.get(args.workload, 4)
-  use_ref = reference_available()
   nf = min(scene["F"], frames)
   sample = subsample_frames(scene, np.arange(nf))
   for _ in range(max(1, min(args.warmup, 2))):
-    cpu_reference_step(subsample_frames(scene, np.arange(min(2, nf))), use_ref)
+    cpu_reference_step(subsample_frames(scene, np.arange(min(2, nf))))
   tot_res, tot_t, nfev, njev = 0.0, 0.0, 0, 0
   t_start = time.perf_counter()
   steps_done = 0
   for _ in range(args.steps):
-    v, dt, nf_, nj_, n, kind = cpu_reference_step(sample, use_ref)
+    v, dt, nf_, nj_, n = cpu_reference_step(sample)
     tot_res += n * (nf_ + nj_); tot_t += dt; nfev += nf_; njev += nj_; steps_done += 1
     if time.perf_counter() - t_start > args.ref_budget_s: break          # bounded: the whole run ends within minutes
   value = tot_res / tot_t
-  what = "unmodified reference through tests/refshim" if kind == "reference" else "oracle/ba_oracle.py (numpy + the identical scipy call)"
+  what = "oracle/ba_oracle.py (numpy + the identical scipy call)"
   line = dict(metric=METRIC, value=value, unit=UNIT, n_gpus=args.gpus, steps=steps_done, warmup=args.warmup,
               ms_per_step=1e3 * tot_t / steps_done, higher_is_better=True, scaling="strong", vs_baseline=None, dtype="f64",
               data="synthetic", impl="reference",
               config=dict(workload=args.workload, sample=f"first {nf} of {scene['F']} frames, full bundle_adjust per step", corners=n,
                           steps_requested=args.steps, steps_run=steps_done, budget_s=args.ref_budget_s),
               lm_iters_per_sec=njev / tot_t,
-              cpu_baseline=dict(value=value, unit=UNIT, cores=os.cpu_count(), kind=kind,
+              cpu_baseline=dict(value=value, unit=UNIT, cores=os.cpu_count(), kind="port",
                                 sample=f"{args.workload}: first {nf} of {scene['F']} frames ({n} corners), {what}: scipy TRF + LSMR with 2-point "
                                        f"finite-difference Jacobian; all {os.cpu_count()} host cores available to the default thread pools of numpy / "
                                        f"scipy / OpenCV, the Python-level algorithm is serial"),
@@ -209,8 +175,7 @@ def run_ours(args):
   if world > 1:
     dist.init_process_group("nccl", device_id=torch.device("cuda", local))
   stream = torch.cuda.current_stream()
-  flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")      # > 126 MB L2
-  peak, peak_src = measured_peak()
+  flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")      # > the 50 MB L2 of an H100
   NO_PREPARE = 256
 
   def barrier():
@@ -238,7 +203,7 @@ def run_ours(args):
   if world > 1:
     mdist.init_comm(eng, rank, world)
 
-  def measure(local_scene, steps, warmup, e2e=True, roofline=True):
+  def measure(local_scene, steps, warmup, e2e=True, roofline=True, dump_dir=None):
     """Device-resident solves, end-to-end solves and the linearisation kernel's roofline point for one (sharded) scene."""
     calib = from_scene(local_scene).enable(cameras=True)
     n_total = allsum_int(int(calib.inliers.sum()))
@@ -259,6 +224,12 @@ def run_ours(args):
     for _ in range(steps):
       res, ms = solve_resident()
       t_dev += ms; evals += res.nfev + res.njev; njev += res.njev; launches += res.kernel_launches; last = res
+    if dump_dir and rank == 0:
+      os.makedirs(dump_dir, exist_ok=True)
+      for name, a in zip(("cam_rt", "board_rt", "frame_rt", "intrinsics"), eng.get_params()):
+        np.save(os.path.join(dump_dir, name + ".npy"), np.asarray(a, dtype=np.float64))
+      np.save(os.path.join(dump_dir, "solve.npy"),
+              np.array([last.cost, last.initial_cost, last.optimality, last.nfev, last.njev, last.status], dtype=np.float64))
     barrier()
     t_dev = allmax(t_dev)
     out = dict(corners=n_total, ms_per_step=t_dev / steps, value=n_total * evals / (t_dev * 1e-3), lm_iters_per_sec=njev / (t_dev * 1e-3),
@@ -295,7 +266,7 @@ def run_ours(args):
         times.append(e0.elapsed_time(e1) * 1e-3)
       dur = float(np.mean(times))
       ach = info["bytes_per_launch"] / dur / 1e9
-      out["roofline"] = dict(bound="hbm", achieved=ach, peak=peak, unit="GB/s", frac=ach / peak, bytes_per_launch=info["bytes_per_launch"],
+      out["roofline"] = dict(bound="hbm", achieved=ach, peak=HBM_PEAK_GBS, unit="GB/s", frac=ach / HBM_PEAK_GBS, bytes_per_launch=info["bytes_per_launch"],
                              launch_ms=dur * 1e3, launches_per_step=out["nfev_plus_njev_per_step"] / 2.0)
     return out, calib
 
@@ -304,7 +275,7 @@ def run_ours(args):
   scene = synthetic.make_workload(args.workload, seed=args.seed)
   my = mdist.frame_range(scene["F"], rank, world)
   local_scene = pin(subsample_frames(scene, np.arange(*my)) if world > 1 else scene)
-  main, calib = measure(local_scene, args.steps, args.warmup)
+  main, calib = measure(local_scene, args.steps, args.warmup, dump_dir=args.dump_outputs)
 
   # the same end-to-end call over a float32 table: make_point_table keeps the dtype of the detector's corners (tables.py:15-17; cv2 returns
   # float32), so for real detections THIS is the reference's table.  The scene is the main scene rounded to float32 (8 B per entry over the link).
@@ -336,7 +307,7 @@ def run_ours(args):
   if world == 1 and args.secondary:
     for wl in ("cfg2", "cfg3", "cfg5"):      # cfg5 = BASELINE configs[4] (64 cameras x 2000 frames, 50.8 M corners, n_s = 1030): it fits one GPU as well
       if wl == args.workload: continue
-      o, _ = measure(pin(synthetic.make_workload(wl, seed=args.seed)), max(3, args.steps // 2), args.warmup)
+      o, _ = measure(pin(synthetic.make_workload(wl, seed=args.seed)), args.steps, args.warmup)
       o.pop("cost", None)
       others[wl] = o
   if world > 1:
@@ -360,7 +331,7 @@ def run_ours(args):
       base = dict(synthetic.WORKLOADS["cfg2"])
       wscene = synthetic.make_scene(seed=args.seed, **{**base, "F": base["F"] * world})
       wmy = mdist.frame_range(wscene["F"], rank, world)
-      o, _ = measure(pin(subsample_frames(wscene, np.arange(*wmy))), max(3, args.steps // 2), args.warmup, e2e=False, roofline=False)
+      o, _ = measure(pin(subsample_frames(wscene, np.arange(*wmy))), args.steps, args.warmup, e2e=False, roofline=False)
       o.pop("cost", None)
       others["weak_cfg2_per_gpu"] = dict(o, scaling="weak", frames_per_gpu=base["F"])
   sampler.stop_flag = True; sampler.join(timeout=2)
@@ -369,12 +340,12 @@ def run_ours(args):
     if world > 1: dist.destroy_process_group()
     return
 
-  roofline = dict(main["roofline"], traffic=ncu_traffic(args.workload), peak_source=peak_src,
+  roofline = dict(main["roofline"], peak_source="H100 SXM data sheet (3.35 TB/s HBM3)",
                   kernel="k_linearize (fused: residuals + analytic Jacobian + per-view moment SYRK on the fp64 tensor path + twist-map expansion into "
                          "H_ff / W / shared records; reads every corner once, writes nothing per corner or per view)",
                   algorithmic_bytes="18 B/corner (16 B observation f64x2 + 2 B point index) + 16 B/view, one launch per evaluation",
-                  note="the contract bound is HBM; the pass needs ~160 DFMA + 12 DMMA(m8n8k4) per corner against 18 B (~60 flop/B vs an fp64 ridge of "
-                       "~6 flop/B on B200), so the fp64 pipe bounds it: see profiles/ for sm__inst_executed_pipe_fp64 / pipe_fp64 cycles of the same launch")
+                  note="the bound named is HBM; the pass needs ~160 DFMA + 12 DMMA(m8n8k4) per corner against 18 B (~60 flop/B vs an fp64 ridge of "
+                       "~10 flop/B on an H100 SXM: 34 TFLOP/s fp64 over 3.35 TB/s, data sheet), so the fp64 pipe bounds it")
 
   # ---- CPU baseline: the reference's path on a bounded sample of the same workload ---------------------------------------------
   cpu_baseline, *_ = cpu_baseline_block(scene, args.workload, args.ref_frames or REF_FRAMES.get(args.workload, 4))
@@ -421,12 +392,11 @@ def main():
   ap.add_argument("--ref-frames", type=int, default=0, help="frames in the CPU-baseline sample (0: per-workload default)")
   ap.add_argument("--ref-budget-s", type=float, default=240.0, help="the reference arm stops taking steps after this many seconds")
   ap.add_argument("--no-secondary", dest="secondary", action="store_false", help="skip the secondary workload blocks")
+  ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the main workload's last timed solve as DIR/<name>.npy")
   args = ap.parse_args()
   if args.impl == "reference":
     run_reference(args)
   else:
-    import __graft_entry__ as g
-    g.build()
     run_ours(args)
 
 

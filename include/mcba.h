@@ -1,4 +1,4 @@
-/* mcba.h — C-ABI of the B200 bundle-adjustment engine (libmcba.so).
+/* mcba.h — C-ABI of the H100 bundle-adjustment engine (libmcba.so).
  *
  * Drop-in boundary for ONE numeric seam of the reference (multical):
  *     scipy.optimize.least_squares(evaluate, self.param_vec, jac_sparsity=..., x_scale='jac',
@@ -9,7 +9,7 @@
  *
  * Plain C types only: opaque handle, host pointers + sizes, integer status (0 = ok; message via
  * mcba_last_error).  All host arrays are borrowed for the duration of the call and copied.
- * There is no CPU fallback: every entry point fails with MCBA_ERR_CUDA if no sm_100 device works.
+ * There is no CPU fallback: every entry point fails with MCBA_ERR_CUDA if no sm_90 device works.
  *
  * Index contract (bit-exact with the reference): packed corner k corresponds to row k of
  * np.argwhere(calib.inliers) = (camera, frame, board, point) in row-major order of the dense

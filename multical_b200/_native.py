@@ -1,5 +1,5 @@
-"""ctypes binding of include/mcba.h (libmcba.so).  Fails loudly when the library or a
-B200-class device is missing: there is no CPU fallback on the product path."""
+"""ctypes binding of include/mcba.h (libmcba.so).  Fails loudly when the library or an
+H100 (sm_90) device is missing: there is no CPU fallback on the product path."""
 import ctypes as C
 import os
 

@@ -1,5 +1,5 @@
 """`Calibration` with the reference's public surface (multical/optimization/calibration.py:43-300)
-whose `bundle_adjust()` runs on a B200 through libmcba.so instead of
+whose `bundle_adjust()` runs on an H100 through libmcba.so instead of
 `scipy.optimize.least_squares` over numpy + cv2 (calibration.py:199-212).
 
 Constructor signature, method names, argument meanings, logging and error behaviour follow the

@@ -1,4 +1,4 @@
-// kernels.cuh — sm_100a kernels of the bundle-adjustment hot path.
+// kernels.cuh — sm_90a kernels of the bundle-adjustment hot path.
 //
 // Data layout in HBM (built once by mcba_upload, solver.cu): corners are stored FRAME-MAJOR, sorted by
 // (frame, camera, board, point), so that every "view" (frame,camera,board) is one contiguous run and all
@@ -322,7 +322,7 @@ k_views(DeviceProblem p, ViewKernelArgs a) {
 // ------------------------------------------------------------------------------------------------
 // k_views_mma: the per-view moment accumulation as what it is -- a small fp64 SYRK.  Per 32-corner chunk the warp
 // stages Gt = [G | r] (64 residual rows x NC columns, NC = D+1 padded to a multiple of 8) in shared memory and
-// accumulates M += Gt^T Gt on the fp64 tensor path (mma.sync m8n8k4 "DMMA"; tcgen05 has no fp64 kind).  The 8x8 C
+// accumulates M += Gt^T Gt on the fp64 tensor path (mma.sync m8n8k4 "DMMA"; wgmma has no fp64 kind).  The 8x8 C
 // fragments ARE the per-view accumulators (2 doubles per lane and tile), so one pass produces all D(D+1)/2 + D
 // moments: no register-limited PART split, no cross-lane reduction.  Same outputs as k_views<MODE_MOMENTS>.
 __device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double b) {

@@ -258,8 +258,8 @@ __device__ __forceinline__ void schur_frame(const LmArgs& a, int f, double reg, 
 // Operands: Y is tile-major ([row tile][frame][32][FB], rows beyond n_s zero), so the frames of a step (48 k-columns: 8 frames x 6, or
 // 4 x 12) are ONE contiguous piece per operand: a step is two bulk asynchronous copies (cp.async.bulk + mbarrier) of 12 KB straight into
 // shared memory, SYRK_STAGES steps in flight per CTA.  (Frame-major Y needed a copy per frame and operand, 16 per step, and a step then
-// cost what the copy unit takes to work off 16 requests -- about 1.2 us whatever their size: 1.3 ms of SYRK at n_s = 1030 x 2000 frames;
-// before that, register-prefetched operands: one HBM/L2 round trip per step.)
+// cost what the copy unit takes to work off 16 requests, whatever their size; before that, register-prefetched operands: one HBM/L2
+// round trip per step.)
 // Product on the fp64 tensor path, bound by the fragment loads from shared memory, not by the DMMAs: warp w owns the 16 x 16 block
 // (w & 3) of the tile and every second k-step (w >> 2) -- 4 fragment loads feed 4 DMMAs (8 x 16 blocks over all k-steps: 3 loads per 2)
 // -- and the rows a lane group reads are permuted (group g -> row 2 (g & 3) + (g >> 2)) so that with 6 doubles per row the 16 lanes of a
@@ -366,7 +366,7 @@ __device__ __forceinline__ void syrk_tile(const LmArgs& a, int ti, int tj, int c
 
 // ---- blocked right-looking Cholesky for n_s > CHOL_SMALL_MAX, NB = 32 panels, the grid cooperating between barriers.
 // The diagonal block by ONE warp: lane i keeps row i in registers, a column is one shuffle of the pivot, one rsqrt and a
-// shuffle per trailing column -- no block barrier on the column path (scripts/chol_bench.cu: 9.2 us against 12.9 us for the
+// shuffle per trailing column -- no block barrier on the column path (scripts/chol_bench.cu times it against the
 // 256-thread version, whose column costs two __syncthreads).  The inverse of the factor follows in the same warp, lane j solving
 // for column j with four independent partial sums per row.
 __device__ __noinline__ void chol_diag_warp_body(int n, int kb, double* S, double* Linv_all, int* chol_fail, double* sh) {
@@ -625,9 +625,9 @@ constexpr int SUBST_HALF = 16, SUBST_UN = 8;
 // on (shared memory, double buffered), and the block's panel of L^T -- rows 32 j .. 32 j + 31, each contiguous -- is read with all the
 // loads of a thread in flight at once: forward in axpy form (thread = column i: b_i -= sum_k L^T[k][i] y_k, 32 loads per column, the
 // next block's rows first), backward over the SAME panels in dot form (thread = (rows k, k + 16; column slice): 16 loads in flight, the 16
-// slices of a row reduced by shuffles).  Fixed order everywhere.  History (profiles/r02_k_lm_phases_*): two dependent L2 round trips
-// per block and direction, 8-deep load batches: 70 us at n_s = 286, 540 us at n_s = 1030; the panels through a 4-stage ring of bulk
-// asynchronous copies (16 requests of 2 KB per stage): 41 / 298 us -- a stage cost what the copy unit takes for 16 requests, ~1 us.
+// slices of a row reduced by shuffles).  Fixed order everywhere.  Slower forms this replaced: two dependent L2 round trips
+// per block and direction with 8-deep load batches; the panels through a 4-stage ring of bulk asynchronous copies (16 requests of 2 KB
+// per stage), where a stage cost what the copy unit takes for 16 requests.
 __host__ __device__ inline size_t subst_smem_doubles(int n) {
   return (size_t)((n + CHOL_NB - 1) / CHOL_NB) * CHOL_NB + 2 * CHOL_NB * (CHOL_NB + 1) + 64;
 }

@@ -50,7 +50,7 @@ struct mcba_ctx {
   int rank = 0, world = 1;
   int launches = 0;
   bool solving = false;   // inside mcba_solve (the fp32-Hessian candidate is never used by the parity hooks)
-  int num_sms = 148;
+  int num_sms = 132;
 
   bool uploaded = false;
   DeviceProblem P{};
@@ -728,7 +728,7 @@ int mcba_create(int device, mcba_ctx** out) {
   cudaDeviceProp prop;
   e = cudaGetDeviceProperties(&prop, device);
   if (e != cudaSuccess) { g_create_error = cudaGetErrorString(e); return MCBA_ERR_CUDA; }
-  if (prop.major != 10) { g_create_error = "libmcba is built for sm_100a only (found sm_" + std::to_string(prop.major * 10 + prop.minor) + ")"; return MCBA_ERR_CUDA; }
+  if (prop.major != 9 || prop.minor != 0) { g_create_error = "libmcba is built for sm_90a only (found sm_" + std::to_string(prop.major * 10 + prop.minor) + ")"; return MCBA_ERR_CUDA; }
   mcba_ctx* ctx = new mcba_ctx();
   ctx->device = device;
   ctx->num_sms = prop.multiProcessorCount;

@@ -8,7 +8,7 @@ import this file.
 Pinning status: the reference ships NO tests, golden vectors or fixtures for this path
 (SURVEY.md §4, §8c) — "parity unpinned" by the reference's own tests.  The restatement is
 instead pinned against the *running reference itself* (imported unmodified through
-tests/refshim in the build container) by tests/golden/make_golden.py, whose outputs are
+tests/refshim) by tests/golden/make_golden.py, whose outputs are
 committed under tests/golden/ and re-checked by tests/test_oracle.py on every run.
 
 Each function cites the reference lines it follows.  All arithmetic is float64 like the

@@ -1,4 +1,4 @@
-// Single-CTA Cholesky variants that were measured against the shipping ones and dropped (profiles/r02_chol_bench.txt): kept here, next to
+// Single-CTA Cholesky variants that were measured against the shipping ones and dropped (scripts/chol_bench.cu): kept here, next to
 // the micro-benchmark that times them (scripts/chol_bench.cu), not in the product's headers.
 //   chol_small_body   the round-1 scheme: matrix cyclically distributed in registers, two block barriers per column
 //   chol_diag_body    the 32 x 32 diagonal block by 256 threads (the product uses one warp: chol_diag_warp_body)

@@ -1,4 +1,4 @@
-"""Developer diagnostics on a GPU box: prints parity numbers without asserting (run under gpurun)."""
+"""Developer diagnostics on a GPU box: prints parity numbers without asserting."""
 import sys, time, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np

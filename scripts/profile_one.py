@@ -1,4 +1,4 @@
-"""Launch the hot kernels a few times on one workload (target for ncu; see profiles/README.md)."""
+"""Launch the hot kernels a few times on one workload (target for a profiler; MCBA_PROF=1 prints k_lm phase stamps)."""
 import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np

@@ -13,7 +13,7 @@ GOLDEN_CASES = ["standard_2x6", "fisheye_3x5", "rational_2x5", "cube3_3x6", "pos
 
 
 def pytest_configure(config):
-  config.addinivalue_line("markers", "gpu: needs a B200 (run with -m gpu on the GPU box)")
+  config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a); run with -m gpu on a machine that has one")
 
 
 def load_golden(name):

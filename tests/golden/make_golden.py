@@ -1,7 +1,7 @@
 """Generate golden vectors from the UNMODIFIED reference (imported through tests/refshim).
 
-Run in the build container only (`/root/reference` must exist):
-    python tests/golden/make_golden.py
+Run with MULTICAL_REFERENCE pointing at a checkout of multical:
+    MULTICAL_REFERENCE=<path> python tests/golden/make_golden.py [case ...]
 For each small synthetic scene it stores the inputs (plain arrays) and what the reference computes:
   x0            Calibration.param_vec                          (parameters.py:44-46)
   r0, r1        evaluate(x0), evaluate(x1)                     (calibration.py:204-206)
@@ -34,6 +34,7 @@ CASES = {
   "invalid_poses_3x6": dict(C=3, F=6, vis=0.5, seed=16, model="standard"),
   "thin_prism_2x5": dict(C=2, F=5, vis=0.5, seed=17, model="thin_prism"),
   "tilted_2x5": dict(C=2, F=5, vis=0.5, seed=18, model="tilted"),
+  "cube2_3x5": dict(C=3, F=5, vis=0.6, seed=21, model="standard", boards=("cube", 10, 10, 0.04, 2), rig="dome"),
 }
 
 
@@ -175,12 +176,45 @@ def pnp_cases(ref, only):
     print(name, "views", table.valid.size, "valid", int(table.valid.sum()), "max err", float(np.max(table.reprojection_error)), os.path.getsize(path) // 1024, "KB")
 
 
+def reference_objects_case(ref, name="reference_objects_2x5"):
+  """What the reference's own Calibration computes over its own ParamList / Camera / PoseSet / Table / motion-model objects, for the
+  three motion models (static, rolling, hand_eye), before any solve:
+    <motion>_x0       Calibration.param_vec                                        (parameters.py:44-46)
+    <motion>_ok       reprojected.valid & point_table.valid
+    <motion>_proj     reprojected.points                                           (calibration.py:124-130)
+    <motion>_err      reprojection_error                                           (calibration.py:134-136)
+    <motion>_cost0    0.5 * sum of squared inlier residuals at x0                   (calibration.py:204-206)
+  rolling: end pose = start pose moved by 5 mm; hand_eye: arm poses = the frame estimates, identity hand-eye pair, cameras and
+  camera poses fixed."""
+  scene = synthetic.make_scene(C=2, F=5, vis=0.4, seed=77)
+  src = scene["init"]
+  data = dict(
+    model=scene["model"], points=scene["points"], valid=scene["valid"],
+    cam_valid=scene["cam_valid"], frame_valid=scene["frame_valid"], board_valid=scene["board_valid"],
+    board_points=np.stack(scene["board_points"]), K=src["K"], dist=src["dist"],
+    cam_poses=src["cam_poses"], frame_poses=src["frame_poses"], board_poses=src["board_poses"],
+    image_size=np.array(scene["image_size"]), cameras_enabled=True)
+  end = src["frame_poses"].copy(); end[:, :3, 3] += 0.005
+  data["rolling_frame_poses_end"] = end
+  for motion, spec in (("static", None), ("rolling", ("rolling", end)), ("hand_eye", ("hand_eye", src["frame_poses"], np.eye(4), np.eye(4)))):
+    rc = loader.build_calibration(ref, scene, motion=spec)
+    rc = rc.enable(camera_poses=False, cameras=False) if motion == "hand_eye" else rc.enable(cameras=True)
+    r = (np.asarray(rc.reprojected.points) - np.asarray(rc.point_table.points))[np.asarray(rc.inliers)]
+    data.update({f"{motion}_x0": np.asarray(rc.param_vec), f"{motion}_ok": np.asarray(rc.reprojected.valid) & np.asarray(rc.point_table.valid),
+                 f"{motion}_proj": np.asarray(rc.reprojected.points), f"{motion}_err": np.asarray(rc.reprojection_error),
+                 f"{motion}_cost0": 0.5 * float(np.sum(r ** 2))})
+  path = os.path.join(HERE, name + ".npz")
+  np.savez_compressed(path, **data)
+  print(name, {m: data[f"{m}_cost0"] for m in ("static", "rolling", "hand_eye")}, os.path.getsize(path) // 1024, "KB")
+
+
 def main():
   ref = loader.load()
   only = sys.argv[1:]          # optional: regenerate just the named cases (existing fixtures stay byte-identical)
   if not only or "outliers_3x6" in only: outlier_case(ref)
   if not only or any(n in only for n in ("rolling_2x6", "handeye_2x6")): motion_cases(ref, only)
   if not only or any(n.startswith("pnp_") for n in only): pnp_cases(ref, only)
+  if not only or "reference_objects_2x5" in only: reference_objects_case(ref)
   for name, kw in CASES.items():
     if only and name not in only: continue
     scene = synthetic.make_scene(**kw)

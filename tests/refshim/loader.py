@@ -1,5 +1,6 @@
-"""TEST INFRASTRUCTURE ONLY — import the unmodified reference hot path from
-/root/reference (exists only in the build container, never on the GPU box).
+"""TEST INFRASTRUCTURE ONLY — import the unmodified reference hot path from a checkout of multical whose
+location is given by the MULTICAL_REFERENCE environment variable.  Only tests/golden/make_golden.py uses it:
+the test-suite compares against the golden vectors it stores, never against the reference itself.
 
 Recipe = SURVEY.md Appendix B: stand-in `structs`, `cached_property` alias, empty
 `quaternion`, and stub *packages* for `multical` / `multical.board` whose __path__ points
@@ -10,17 +11,17 @@ import os
 import sys
 import types
 
-REFERENCE_ROOT = "/root/reference"
+REFERENCE_ROOT = os.environ.get("MULTICAL_REFERENCE", "")
 
 
 def available():
-  return os.path.isdir(os.path.join(REFERENCE_ROOT, "multical"))
+  return bool(REFERENCE_ROOT) and os.path.isdir(os.path.join(REFERENCE_ROOT, "multical"))
 
 
 def load():
   """Returns a namespace with the reference classes; raises if the reference is absent."""
   if not available():
-    raise RuntimeError("reference tree not present (expected on the GPU box)")
+    raise RuntimeError("set MULTICAL_REFERENCE to a checkout of multical")
   here = os.path.dirname(os.path.abspath(__file__))
   if here not in sys.path:
     sys.path.insert(0, here)

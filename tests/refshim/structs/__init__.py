@@ -1,8 +1,7 @@
 """TEST INFRASTRUCTURE ONLY.
 
 Stand-in for the third-party `py-structs` package (setup.py:47 of the reference,
-un-vendored and absent from this image) so that the *unmodified* reference hot path
-(/root/reference/multical/optimization/calibration.py etc.) can be imported in the
-build container to validate the oracle and to generate tests/golden/ fixtures.
-Never imported by multical_b200 (the product) and never used on the GPU box.
+not a dependency of this project) so that the *unmodified* reference hot path
+(multical/optimization/calibration.py etc.) can be imported to generate the
+tests/golden/ fixtures.  Never imported by multical_b200 (the product) or by the test-suite.
 """

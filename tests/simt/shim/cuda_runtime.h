@@ -1,6 +1,6 @@
 // cuda_runtime.h -- TEST INFRASTRUCTURE ONLY: host stand-in for the CUDA runtime calls multical_b200/csrc/solver.cu makes, used
 // when tests/simt builds the kernels for the SIMT interpreter (simt.h).  "Device" memory is host memory, streams are
-// synchronous, the one reported device calls itself sm_100 so that mcba_create accepts it.  Peer / IPC calls fail.
+// synchronous, the one reported device calls itself sm_90 so that mcba_create accepts it.  Peer / IPC calls fail.
 #pragma once
 #include <chrono>
 #include <condition_variable>
@@ -42,9 +42,9 @@ static inline cudaError_t cudaSetDevice(int) { return cudaSuccess; }
 static inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp* p, int) {
   memset(p, 0, sizeof(*p));
   snprintf(p->name, sizeof(p->name), "SIMT interpreter (host)");
-  p->major = 10; p->minor = 0;
+  p->major = 9; p->minor = 0;
   const char* e = getenv("SIMT_SMS");
-  p->multiProcessorCount = e ? std::max(1, atoi(e)) : 148;
+  p->multiProcessorCount = e ? std::max(1, atoi(e)) : 132;
   p->sharedMemPerBlockOptin = 227 * 1024;
   p->totalGlobalMem = (size_t)8 << 30;
   return cudaSuccess;

