@@ -8,9 +8,10 @@
 //                                         are stored once; the shared-parameter blocks are accumulated per (CTA, camera) in a record that
 //                                         only this CTA's owning warp ever touches (plain read-modify-write in L2, no atomics).
 //   k_reduce_shared<NP>        sums the per-CTA records in CTA order (fixed -> bit-reproducible run to run) and stores H_ss, g_s, cost.
-//
-// Replaces k_views_mma + k_expand_frames + k_expand_shared of round 1 (1 KB/view moment records written and read back twice:
-// 1.45x the algorithmic bytes at 5.5 M corners, and fp64 atomics into H_ss / g that made two identical solves differ in the 8th digit).
+//   k_fold_hand_eye            hand-eye frames: the 12 hand-eye rows and columns of H_ss, g_s as per-frame folds of H_ff, W_f, g_f
+//                              (the frames are derived poses; their blocks are emitted for the fold only), summed in frame order.
+// Every motion model goes through these kernels, and none of them adds to H or g with atomics: two identical linearisations agree bit for
+// bit (only the board-point blocks of boards=True, k_point_blocks in kernels.cuh, are added with fp64 atomics).
 // Reference semantics: the Jacobian scipy builds by finite differences over calibration.py:173-196's sparsity pattern, here analytic.
 #pragma once
 #include "solver_kernels.cuh"
@@ -249,7 +250,7 @@ __device__ __forceinline__ void lin_flush_wacc(const DeviceProblem& p, const Lin
   const int B = p.B;
   double* tl = w + L::tail(B);
   const int cam = (int)tl[1];
-  if (cam < 0 || !p.motion_on || tl[3] == 0.0) return;
+  if (cam < 0 || !p.frame_blocks || tl[3] == 0.0) return;
   __syncwarp();
   if (lane == 0) tl[3] = 0.0;
   double* wacc = w + L::wacc(B);
@@ -406,9 +407,9 @@ k_linearize(DeviceProblem p, LinArgs a) {
   const int B = p.B, n_s = p.n_s;
   const int split = a.split, slots = nwarps / split, slot = warp / split, sub = warp % split;
   const bool leader = sub == 0;
-  const bool frames_on = p.motion_on != 0;
+  const bool frames_on = p.frame_blocks != 0;
   const size_t wd = lin_warp_doubles(NC, T, D, FB, NIN, B, NP);
-  double* w = lsm + (size_t)warp * wd;          // this warp's slice; w[0 .. NC*MMA_KPAD) is the stage buffer of the chunk loop
+  double* w = lsm + (size_t)warp * wd;          // this warp's slice; w[0 .. NC*LIN_KPAD) is the stage buffer of the chunk loop
   // pose tables staged in shared memory by bulk asynchronous copies: the frame's [NP] (double buffered: the next frame's is in flight
   // while this one is worked on), then the boards' (they do not change during the launch)
   __shared__ __align__(8) unsigned long long tbar[3];
@@ -838,6 +839,67 @@ k_reduce_shared(DeviceProblem p, ReduceArgs a) {
   for (int f = tid; f < a.F; f += RED_THREADS) cs += a.frame_cost[f];
   cs = block_sum(cs, sm);
   if (tid == 0) *a.cost_out = cs;
+}
+
+// ------------------------------------------------------------------------------------------------
+// k_fold_hand_eye: hand-eye frames with free hand-eye parameters he = [W | G].  Every residual of frame f reaches he through the frame's
+// twist, J_he = J_f M_f (hand_eye_frame_map), so with the frame blocks k_linearize emitted (frame_blocks) and k_point_blocks completed
+//     H_he,he = sum_f M_f^T H_ff M_f      H_s,he = sum_f W_f[s, :] M_f   (every shared row s outside he)      g_he = sum_f M_f^T g_f
+// One CTA per row s of H_s,he (he rows: the upper triangle of H_he,he; row n_s: g_he); thread (slice, j) sums column j over the frames
+// f == slice mod FOLD_SLICES in frame order, and the slices' partials are added in slice order: fixed order, no atomics.  The CTA builds
+// the maps of FOLD_FRAMES frames at a time in shared memory.  The he block, both triangles of every coupling and g_he are stored (nothing
+// else writes them); the he rows of W_f are never written or read.
+constexpr int FOLD_SLICES = 16;
+constexpr int FOLD_THREADS = FOLD_SLICES * 16;
+constexpr int FOLD_FRAMES = 64;
+__global__ void __launch_bounds__(FOLD_THREADS)
+k_fold_hand_eye(DeviceProblem p, const double* Hff, const double* W, double* Hss, double* g) {
+  __shared__ double Mf[FOLD_FRAMES][72];
+  __shared__ double part[FOLD_SLICES][16];
+  const int n_s = p.n_s, he = p.off_he;
+  const int r = blockIdx.x, j = threadIdx.x % 16, slice = threadIdx.x / 16;
+  const int q = r - he;
+  const bool hrow = q >= 0 && q < 12;
+  const bool live = j < 12 && !(hrow && j < q);
+  double acc = 0.0;
+  for (int f0 = 0; f0 < p.F; f0 += FOLD_FRAMES) {
+    const int nf = min(FOLD_FRAMES, p.F - f0);
+    __syncthreads();
+    if ((int)threadIdx.x < nf) {
+      const PoseT& pw = p.he_T[0]; const PoseT& pg = p.he_T[1];
+      const int f = f0 + threadIdx.x;
+      hand_eye_frame_map(pg.R, p.arm_T[f].R, pw.JL, pg.JL, pg.t, p.frame_T[f].t, Mf[threadIdx.x]);
+    }
+    __syncthreads();
+    if (!live) continue;
+    for (int i = slice; i < nf; i += FOLD_SLICES) {
+      const double* M = Mf[i];
+      const int f = f0 + i;
+      if (r == n_s) {
+        const double* gf = g + n_s + 6 * f;
+        for (int k = 0; k < 6; k++) acc += M[12 * k + j] * gf[k];
+      } else if (hrow) {
+        const double* H = Hff + 36 * f;
+        for (int k = 0; k < 6; k++) {
+          double t = 0.0;
+          for (int l = 0; l < 6; l++) t += M[12 * l + q] * H[6 * l + k];
+          acc += t * M[12 * k + j];
+        }
+      } else {
+        const double* w = W + ((size_t)f * n_s + r) * 6;
+        for (int k = 0; k < 6; k++) acc += w[k] * M[12 * k + j];
+      }
+    }
+  }
+  part[slice][j] = acc;
+  __syncthreads();
+  if (slice != 0 || !live) return;
+  for (int s = 1; s < FOLD_SLICES; s++) acc += part[s][j];
+  if (r == n_s) g[he + j] = acc;
+  else {
+    Hss[(size_t)r * n_s + he + j] = acc;
+    Hss[(size_t)(he + j) * n_s + r] = acc;
+  }
 }
 
 }  // namespace mcba

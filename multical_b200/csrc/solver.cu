@@ -49,7 +49,6 @@ struct mcba_ctx {
   std::string err;
   int rank = 0, world = 1;
   int launches = 0;
-  bool solving = false;   // inside mcba_solve (the fp32-Hessian candidate is never used by the parity hooks)
   int num_sms = 132;
 
   bool uploaded = false;
@@ -66,8 +65,8 @@ struct mcba_ctx {
   // motion models: image heights (rolling), hand-eye pair (current / trial) with its pose table and the fixed arm poses
   DevBuf<double> img_h, he_rt, he_rt2; DevBuf<PoseT> he_T, arm_T;
   // solver buffers
-  DevBuf<double> moments, Hss, g, Hff, W, cost_part, view_cost, diag_s;
-  // fused linearisation (linearize.cuh): per-(CTA, camera) records of the shared blocks, per-camera board partials, per-frame costs
+  DevBuf<double> Hss, g, Hff, W, view_cost;
+  // linearisation (linearize.cuh): per-(CTA, camera) records of the shared blocks, per-camera board partials, per-frame costs
   DevBuf<double> spart, bpart, frame_cost, sred;
   DevBuf<unsigned> cam_counter;
   // device-resident trust-region loop (lm_kernel.cuh)
@@ -80,13 +79,9 @@ struct mcba_ctx {
   struct SolveGraph { cudaGraphExec_t exec = nullptr; cudaGraph_t graph = nullptr; std::vector<char> key; cudaStream_t stream = nullptr; int body_launches = 0; } sg;
   bool graph_launched = false;
   int lin_grid = 1, lin_split = 1, lin_warps = LIN_WARPS;
-  bool fused_lin = true;       // false for hand-eye frames: per-view moment records + the round-1 expand kernels (they carry the 12 shared motion parameters)
   DevBuf<double> x, x_new, sinv, d, gh, gn, Y, Lf, zf, S, rhs, red, Linv;
   DevBuf<SolverState> state;
-  DevBuf<unsigned> counter;
-  int shared_chunks = 1;
-  int cur_loss = 0; double cur_f_scale = 1.0;     // loss of the linearisation in flight (k_point_blocks re-derives the row weights)
-  // peer-memory all-reduce (peer_allreduce.cuh)
+  // NVLink peer-memory exchange of the solver kernel (lm_kernel.cuh LmPeer)
   double* peer_own = nullptr; int peer_cap = 0; bool peer_ready = false;
   double* peer_base[PEER_MAX_WORLD] = {nullptr};
   std::vector<void*> peer_opened;
@@ -123,8 +118,6 @@ struct mcba_ctx {
   do { if (!(cond)) { ctx->err = msg; return code; } } while (0)
 
 namespace {
-
-int nparts_for(int model) { return model == MODEL_STANDARD ? 2 : model == MODEL_RATIONAL ? 3 : model == MODEL_THIN_PRISM ? 4 : model == MODEL_TILTED ? 5 : 2; }
 
 // parameters of block-structured vector x (internal order) <-> full parameter state
 __global__ void k_scatter_params(DeviceProblem p, const double* x, double* cam_rt, double* board_rt, double* frame_rt, double* intr) {
@@ -174,29 +167,7 @@ int launch_views(mcba_ctx* ctx, const DeviceProblem& P, const ViewKernelArgs& a)
   return MCBA_OK;
 }
 
-// per-view moment records (hand-eye frames only: the fused pass of linearize.cuh covers static and rolling frames)
-int launch_moments(mcba_ctx* ctx, const DeviceProblem& P, const ViewKernelArgs& a) {
-  const int th = VIEW_WARPS * 32;
-  const int nc = mma_nc(P.model, false), npair = (nc / 8) * (nc / 8 + 1) / 2;
-  const size_t sm = ((size_t)VIEW_WARPS * nc * MMA_KPAD + (size_t)VIEW_WARPS * (2 * npair + 1) * 32) * sizeof(double);
-  cudaStream_t s = ctx->stream;
-  // few long views: let the 4 warps of a CTA share one view
-  const bool split = P.V < ctx->num_sms * 16;
-  const int blocks = split ? std::max(1, P.V) : std::max(1, std::min((P.V + VIEW_WARPS - 1) / VIEW_WARPS, ctx->num_sms * 16));
-#define LM(MODEL) if (split) k_views_mma<MODEL, VIEW_WARPS><<<blocks, th, sm, s>>>(P, a); else k_views_mma<MODEL, 1><<<blocks, th, sm, s>>>(P, a);
-  switch (P.model) {
-    case MODEL_STANDARD: LM(MODEL_STANDARD) break;
-    case MODEL_RATIONAL: LM(MODEL_RATIONAL) break;
-    case MODEL_THIN_PRISM: LM(MODEL_THIN_PRISM) break;
-    case MODEL_TILTED: LM(MODEL_TILTED) break;
-    default: LM(MODEL_FISHEYE) break;
-  }
-#undef LM
-  CKL();
-  return MCBA_OK;
-}
-
-// ---------------------------------------------------------------- fused linearisation (linearize.cuh)
+// ---------------------------------------------------------------- linearisation (linearize.cuh)
 template <int MODEL, bool ROLL>
 size_t lin_smem_bytes(const DeviceProblem& P, int warps) {
   using S = LinShape<MODEL, ROLL>;
@@ -272,43 +243,22 @@ int set_state_from_x(mcba_ctx* ctx, const double* x, bool trial) {
   return prepare(ctx, P);
 }
 
-size_t expand_shared_smem(const DeviceProblem& P) { return sizeof(double) * ((size_t)EXP_WARPS * exps_warp_doubles(P.T, P.D, P.B, P.npf) + P.T + 36); }
-size_t expand_hand_eye_smem(const DeviceProblem& P) { return sizeof(double) * ((size_t)EXP_WARPS * exph_warp_doubles(P.T, P.D, P.B)); }
-
-// per-view moment records of the (trial or current) state; the pose tables must already describe that state
-int moments_at(mcba_ctx* ctx, int loss, double f_scale, bool trial) {
-  ctx->cur_loss = loss; ctx->cur_f_scale = f_scale;
-  DeviceProblem P = with_state(ctx, trial);
-  if (ctx->fused_lin) return launch_linearize(ctx, P, loss, f_scale);
-  ViewKernelArgs a{}; a.loss = loss; a.f_scale = f_scale; a.moments = ctx->moments.p; a.view_cost = ctx->view_cost.p;
-  return launch_moments(ctx, P, a);
-}
-
-// records of the fused pass (or, hand-eye frames, per-view moment records) -> H_ss, g_s [, H_ff, W, g_f] and the cost partials;
-// pose tables = the state the pass ran at (trial: the trial parameter arrays)
-int expand(mcba_ctx* ctx, bool trial = false) {
+// The normal equations and the cost at the (trial or current) state, whose pose tables must already describe it: k_linearize, its per-CTA
+// records -> H_ss, g_s, cost (k_reduce_shared), then boards=True: the board-point blocks on top (k_point_blocks), then hand-eye: the
+// hand-eye rows and columns from the frame blocks (k_fold_hand_eye, last: it reads the point rows of W_f)
+int linearize(mcba_ctx* ctx, int loss, double f_scale, bool trial = false) {
   DeviceProblem P = with_state(ctx, trial);
   cudaStream_t s = ctx->stream;
-  const bool roll = P.motion == MOTION_ROLLING;
-  if (ctx->fused_lin) {
-    if (P.off_pt >= 0) {       // boards=True: k_point_blocks adds the point rows / columns on top (atomics): they start at zero
-      CK(cudaMemsetAsync(ctx->Hss.p, 0, sizeof(double) * (size_t)P.n_s * P.n_s, s));
-      CK(cudaMemsetAsync(ctx->g.p, 0, sizeof(double) * (size_t)std::max(P.n_s, 1), s));
-    }
-    int r = launch_reduce_shared(ctx, P); if (r) return r;
-  } else {
-    SolverBuffers sb{ctx->moments.p, ctx->Hss.p, ctx->g.p, ctx->Hff.p, ctx->W.p, ctx->cost_part.p, 0};
+  int r = launch_linearize(ctx, P, loss, f_scale); if (r) return r;
+  if (P.off_pt >= 0) {         // k_point_blocks adds the point rows / columns (atomics): they start at zero
     CK(cudaMemsetAsync(ctx->Hss.p, 0, sizeof(double) * (size_t)P.n_s * P.n_s, s));
-    CK(cudaMemsetAsync(ctx->g.p, 0, sizeof(double) * (size_t)std::max(P.n, 1), s));
-    const int nb = P.C * ctx->shared_chunks;
-    k_expand_shared<1><<<nb, EXP_THREADS, expand_shared_smem(P), s>>>(P, sb, ctx->shared_chunks); CKL();
-    if (P.off_he >= 0 && P.V > 0) {         // hand-eye: the 12 shared motion parameters and their couplings on top (atomics)
-      k_expand_hand_eye<<<nb, EXP_THREADS, expand_hand_eye_smem(P), s>>>(P, sb, ctx->shared_chunks); CKL();
-    }
+    CK(cudaMemsetAsync(ctx->g.p, 0, sizeof(double) * (size_t)std::max(P.n_s, 1), s));
   }
-  if (P.off_pt >= 0 && P.V > 0) {           // boards=True: board-point blocks on top (atomics)
-    ViewKernelArgs a{}; a.loss = ctx->cur_loss; a.f_scale = ctx->cur_f_scale;
+  r = launch_reduce_shared(ctx, P); if (r) return r;
+  if (P.off_pt >= 0 && P.V > 0) {
+    ViewKernelArgs a{}; a.loss = loss; a.f_scale = f_scale;
     const int blocks = std::max(1, std::min((P.V + VIEW_WARPS - 1) / VIEW_WARPS, ctx->num_sms * 8));
+    const bool roll = P.motion == MOTION_ROLLING;
 #define PB(MODEL) if (roll) k_point_blocks<MODEL, 2><<<blocks, VIEW_WARPS * 32, 0, s>>>(P, a, ctx->Hss.p, ctx->W.p, ctx->g.p); \
                   else k_point_blocks<MODEL, 1><<<blocks, VIEW_WARPS * 32, 0, s>>>(P, a, ctx->Hss.p, ctx->W.p, ctx->g.p);
     switch (P.model) {
@@ -321,27 +271,11 @@ int expand(mcba_ctx* ctx, bool trial = false) {
 #undef PB
     CKL();
   }
-  return MCBA_OK;
-}
-
-// the cost of the linearisation -> red[RED_COST] (the fused pass has it there already)
-int finish_linearization(mcba_ctx* ctx) {
-  if (!ctx->fused_lin) {
-    const int nb = ctx->P.C * ctx->shared_chunks;
-    k_sum_partials<<<1, 256, 0, ctx->stream>>>(ctx->cost_part.p, nb, 1, 1, ctx->red.p + RED_COST); CKL();
+  if (P.off_he >= 0) {
+    k_fold_hand_eye<<<P.n_s + 1, FOLD_THREADS, 0, s>>>(P, ctx->Hff.p, ctx->W.p, ctx->Hss.p, ctx->g.p);
+    CKL();
   }
   return MCBA_OK;
-}
-
-// legacy (hand-eye) pass: the trial cost as a one-entry "per-frame cost" list for k_lm
-__global__ void k_copy_view_costs(const double* cost, double* frame_cost, int F) {
-  for (int f = 0; f < F; f++) frame_cost[f] = f == 0 ? *cost : 0.0;
-}
-
-int linearize(mcba_ctx* ctx, int loss, double f_scale) {
-  int r = moments_at(ctx, loss, f_scale, false); if (r) return r;
-  r = expand(ctx); if (r) return r;
-  return finish_linearization(ctx);
 }
 
 // cost at the TRIAL state -> red[RED_COSTNEW]
@@ -389,19 +323,6 @@ LmArgs make_lm_args(mcba_ctx* ctx, int log_cap) {
   return a;
 }
 
-// The trial state's normal equations: fused pass (+ the kernels that add the board-point / hand-eye blocks), H_ss, g_s and the cost.
-// With hand-eye frames the pass is the round-1 pipeline (per-view moment records, then the expand kernels).
-int linearize_trial(mcba_ctx* ctx, int loss, double f_scale) {
-  int r = moments_at(ctx, loss, f_scale, true); if (r) return r;
-  r = expand(ctx, true); if (r) return r;
-  if (!ctx->fused_lin) {
-    const int nb = ctx->P.C * ctx->shared_chunks;
-    k_sum_partials<<<1, 256, 0, ctx->stream>>>(ctx->cost_part.p, nb, 1, 1, ctx->red.p + RED_COST); CKL();
-    k_copy_view_costs<<<1, 1, 0, ctx->stream>>>(ctx->red.p + RED_COST, ctx->frame_cost.p, ctx->P.F); CKL();
-  }
-  return MCBA_OK;
-}
-
 int launch_lm(mcba_ctx* ctx, const LmArgs& a) {
   const size_t sm = sizeof(double) * lm_smem_doubles(ctx->P.n_s, ctx->P.fb);
   LmArgs args = a;
@@ -420,7 +341,7 @@ int launch_lm(mcba_ctx* ctx, const LmArgs& a) {
 
 // one pass of the loop body: linearise the trial state, then accept / solve / step (k_lm)
 int lm_body(mcba_ctx* ctx, int loss, double f_scale, const LmArgs& a) {
-  int r = linearize_trial(ctx, loss, f_scale); if (r) return r;
+  int r = linearize(ctx, loss, f_scale, true); if (r) return r;
   return launch_lm(ctx, a);
 }
 
@@ -509,6 +430,7 @@ int setup_problem(mcba_ctx* ctx, const mcba_problem_desc* desc, int64_t N, int V
   P.off_pt = (opt & MCBA_OPT_BOARDS) ? off : -1; if (P.off_pt >= 0) off += 3 * B * Pn;
   P.off_he = (P.motion == MOTION_HAND_EYE && (opt & MCBA_OPT_MOTION)) ? off : -1; if (P.off_he >= 0) off += 12;
   P.n_s = off; P.n_f = P.motion_on ? P.fb * F : 0; P.n = P.n_s + P.n_f;
+  P.frame_blocks = (P.motion_on || P.off_he >= 0) ? 1 : 0;      // hand-eye: k_fold_hand_eye reads H_ff, W_f, g_f of the derived frames
   // internal -> canonical permutation: canonical = [cp | bp | motion | cameras]
   ctx->perm.assign((size_t)P.n, 0);
   {
@@ -534,10 +456,7 @@ int setup_problem(mcba_ctx* ctx, const mcba_problem_desc* desc, int64_t N, int V
   CK(ctx->img_h.alloc(C)); CK(ctx->he_rt.alloc(12)); CK(ctx->he_rt2.alloc(12)); CK(ctx->he_T.alloc(2)); CK(ctx->arm_T.alloc(std::max(F, 1)));
   CK(ctx->board_pts2.alloc((size_t)B * Pn * 3));
   // solver buffers
-  ctx->shared_chunks = std::max(1, std::min(32, (ctx->num_sms * 2) / std::max(C, 1)));
-  if (V / std::max(C, 1) < 64) ctx->shared_chunks = 1;
-  ctx->fused_lin = P.motion != MOTION_HAND_EYE;
-  if (ctx->fused_lin) {
+  {
     // static frame -> CTA map (bit-reproducible partial sums): the smallest grid that keeps every CTA at ceil(F / resident CTAs) frames
     int split = 1;
     while (split < LIN_WARPS && C * split * 2 <= LIN_WARPS) split *= 2;      // few cameras: several warps share a view
@@ -571,14 +490,12 @@ int setup_problem(mcba_ctx* ctx, const mcba_problem_desc* desc, int64_t N, int V
     CK(ctx->sred.alloc((size_t)C * lin_record_doubles(P.T, P.D, B)));
     CK(ctx->cam_counter.alloc((size_t)C + 1)); CK(cudaMemsetAsync(ctx->cam_counter.p, 0, sizeof(unsigned) * ((size_t)C + 1), ctx->stream));
     CK(ctx->frame_cost.alloc((size_t)std::max(F, 1)));
-    CK(ctx->moments.alloc(1));
-  } else {
-    CK(ctx->moments.alloc((size_t)std::max(V, 1) * P.T));
   }
   CK(ctx->Hss.alloc((size_t)std::max(P.n_s, 1) * std::max(P.n_s, 1)));
   CK(cudaMemsetAsync(ctx->Hss.p, 0, sizeof(double) * (size_t)std::max(P.n_s, 1) * std::max(P.n_s, 1), ctx->stream));      // blocks no kernel writes (camera x other camera ...) stay zero
-  CK(ctx->g.alloc((size_t)std::max(P.n, 1)));
-  CK(cudaMemsetAsync(ctx->g.p, 0, sizeof(double) * (size_t)std::max(P.n, 1), ctx->stream));
+  const size_t ng = std::max<size_t>(std::max(P.n, 1), (size_t)P.n_s + (P.frame_blocks ? (size_t)F * fbs : 0));      // g_f of every frame block
+  CK(ctx->g.alloc(ng));
+  CK(cudaMemsetAsync(ctx->g.p, 0, sizeof(double) * ng, ctx->stream));
   CK(ctx->Hff.alloc((size_t)std::max(F, 1) * fbs * fbs));
   CK(ctx->W.alloc((size_t)std::max(F, 1) * std::max(P.n_s, 1) * fbs));
   {   // Y tile-major [row tile][frame][32][fb], rows beyond n_s stay zero (lm_kernel.cuh syrk_tile_acc)
@@ -586,8 +503,7 @@ int setup_problem(mcba_ctx* ctx, const mcba_problem_desc* desc, int64_t N, int V
     CK(ctx->Y.alloc(ny)); CK(cudaMemsetAsync(ctx->Y.p, 0, sizeof(double) * ny, ctx->stream));
   }
   CK(ctx->Lf.alloc((size_t)std::max(F, 1) * fbs * fbs)); CK(ctx->zf.alloc((size_t)std::max(F, 1) * fbs));
-  CK(ctx->cost_part.alloc((size_t)C * ctx->shared_chunks)); CK(ctx->view_cost.alloc((size_t)std::max(V, 1)));
-  CK(ctx->diag_s.alloc((size_t)std::max(P.n_s, 1)));
+  CK(ctx->view_cost.alloc((size_t)std::max(V, 1)));
   const size_t nn = (size_t)std::max(P.n, 1);
   CK(ctx->x.alloc(nn)); CK(ctx->x_new.alloc(nn)); CK(ctx->sinv.alloc(nn)); CK(ctx->d.alloc(nn)); CK(ctx->gh.alloc(nn)); CK(ctx->gn.alloc(nn));
   CK(ctx->S.alloc((size_t)std::max(P.n_s, 1) * std::max(P.n_s, 1))); CK(ctx->rhs.alloc((size_t)std::max(P.n_s, 1)));
@@ -613,10 +529,8 @@ int setup_problem(mcba_ctx* ctx, const mcba_problem_desc* desc, int64_t N, int V
     CK(ctx->prof.alloc(16)); CK(cudaMemsetAsync(ctx->prof.p, 0, 16 * sizeof(unsigned long long), ctx->stream));
     CK(ctx->lm_bar.alloc(2)); CK(cudaMemsetAsync(ctx->lm_bar.p, 0, 2 * sizeof(unsigned long long), ctx->stream));
     if (!ctx->peer_seq_dev.p) { CK(ctx->peer_seq_dev.alloc(1)); CK(cudaMemsetAsync(ctx->peer_seq_dev.p, 0, sizeof(unsigned long long), ctx->stream)); }
-    CK(ctx->frame_cost.alloc((size_t)std::max(F, 1)));
   }
   CK(ctx->state.alloc(1));
-  CK(ctx->counter.alloc(8)); CK(cudaMemsetAsync(ctx->counter.p, 0, 8 * sizeof(unsigned), ctx->stream));
   if (!keep_state) {     // a re-selection of the resident table (mcba_table_select) keeps the parameter state
     CK(cudaMemsetAsync(ctx->cam_rt.p, 0, sizeof(double) * C * 6, ctx->stream));
     CK(cudaMemsetAsync(ctx->board_rt.p, 0, sizeof(double) * B * 6, ctx->stream));
@@ -642,8 +556,6 @@ int setup_problem(mcba_ctx* ctx, const mcba_problem_desc* desc, int64_t N, int V
   P.cam_rt = ctx->cam_rt.p; P.board_rt = ctx->board_rt.p; P.frame_rt = ctx->frame_rt.p; P.intr = ctx->intr.p;
   P.cam_T = ctx->cam_T.p; P.frame_T = ctx->frame_T.p; P.board_T = ctx->board_T.p;
   P.img_h = ctx->img_h.p; P.he_rt = ctx->he_rt.p; P.he_T = ctx->he_T.p; P.arm_T = ctx->arm_T.p;
-  REQUIRE(expand_hand_eye_smem(P) <= 200 * 1024, MCBA_ERR_UNSUPPORTED, "shared-parameter block too large for the hand-eye expand kernel");
-  REQUIRE(expand_shared_smem(P) <= 200 * 1024, MCBA_ERR_UNSUPPORTED, "shared-parameter block too large for the expand kernels");
   return MCBA_OK;
 }
 // MCBA_PROF=1: host wall clock at checkpoints of the upload path, on stderr (no synchronisation is added: it times what the host waits for)
@@ -736,17 +648,13 @@ int mcba_create(int device, mcba_ctx** out) {
   ctx->stream = ctx->own_stream;
   { const char* e = getenv("MCBA_GRAPH"); if (e && std::string(e) == "0") ctx->use_graph = false; }
   { const char* e = getenv("MCBA_PROF"); if (e && std::string(e) == "1") { ctx->profiling = true; ctx->use_graph = false; } }
-#define MMA_ATTR(MODEL) \
-  cudaFuncSetAttribute(k_views_mma<MODEL, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024); \
-  cudaFuncSetAttribute(k_views_mma<MODEL, VIEW_WARPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024); \
+#define LIN_ATTR(MODEL) \
   cudaFuncSetAttribute(k_linearize<MODEL, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024); \
   cudaFuncSetAttribute(k_linearize<MODEL, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
-  MMA_ATTR(MODEL_STANDARD) MMA_ATTR(MODEL_RATIONAL) MMA_ATTR(MODEL_THIN_PRISM) MMA_ATTR(MODEL_FISHEYE) MMA_ATTR(MODEL_TILTED)
-#undef MMA_ATTR
+  LIN_ATTR(MODEL_STANDARD) LIN_ATTR(MODEL_RATIONAL) LIN_ATTR(MODEL_THIN_PRISM) LIN_ATTR(MODEL_FISHEYE) LIN_ATTR(MODEL_TILTED)
+#undef LIN_ATTR
   cudaFuncSetAttribute(k_reduce_shared<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
   cudaFuncSetAttribute(k_reduce_shared<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-  cudaFuncSetAttribute(k_expand_shared<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-  cudaFuncSetAttribute(k_expand_hand_eye, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
   cudaFuncSetAttribute(k_lm<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
   cudaFuncSetAttribute(k_lm<12>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
   *out = ctx;
@@ -1446,17 +1354,11 @@ int mcba_residuals(mcba_ctx* ctx, const double* x, double* r_out, double* cost) 
   if (!ctx) return MCBA_ERR_ARG;
   REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "mcba_upload has not been called");
   CK(cudaSetDevice(ctx->device));
-  const DeviceProblem& P0 = ctx->P;
   bool trial = false;
   if (x) {
     // evaluate at x without disturbing the stored parameters: trial state = current state overwritten by x
-    CK(cudaMemcpyAsync(ctx->cam_rt2.p, ctx->cam_rt.p, sizeof(double) * P0.C * 6, cudaMemcpyDeviceToDevice, ctx->stream));
-    CK(cudaMemcpyAsync(ctx->board_rt2.p, ctx->board_rt.p, sizeof(double) * P0.B * 6, cudaMemcpyDeviceToDevice, ctx->stream));
-    if (P0.F && P0.fb) CK(cudaMemcpyAsync(ctx->frame_rt2.p, ctx->frame_rt.p, sizeof(double) * P0.F * P0.fb, cudaMemcpyDeviceToDevice, ctx->stream));
-    CK(cudaMemcpyAsync(ctx->he_rt2.p, ctx->he_rt.p, sizeof(double) * 12, cudaMemcpyDeviceToDevice, ctx->stream));
-    CK(cudaMemcpyAsync(ctx->intr2.p, ctx->intr.p, sizeof(double) * P0.C * P0.kint, cudaMemcpyDeviceToDevice, ctx->stream));
-    CK(cudaMemcpyAsync(ctx->board_pts2.p, ctx->board_pts.p, sizeof(double) * P0.B * P0.P * 3, cudaMemcpyDeviceToDevice, ctx->stream));
-    int r = write_x_canonical(ctx, x, ctx->x_new.p); if (r) return r;
+    int r = copy_state_to_trial(ctx); if (r) return r;
+    r = write_x_canonical(ctx, x, ctx->x_new.p); if (r) return r;
     r = set_state_from_x(ctx, ctx->x_new.p, true); if (r) return r;
     trial = true;
   } else {
@@ -1543,10 +1445,8 @@ int mcba_solve(mcba_ctx* ctx, const mcba_solve_opts* opts, mcba_solve_result* re
   cudaStream_t s = ctx->stream;
   const int n = P.n;
   memset(result, 0, sizeof(*result));
-  struct SolvingFlag { bool& f; explicit SolvingFlag(bool& r) : f(r) { f = true; } ~SolvingFlag() { f = false; } } solving_flag(ctx->solving);
   ctx->launches = 0;
   ctx->errors_current = false;
-  ctx->cur_loss = opts->loss; ctx->cur_f_scale = opts->f_scale;
   struct EventPair {       // destroyed on every return path
     cudaEvent_t a = nullptr, b = nullptr;
     ~EventPair() { if (a) cudaEventDestroy(a); if (b) cudaEventDestroy(b); }
@@ -1609,12 +1509,10 @@ int mcba_bench_info(mcba_ctx* ctx, int which, int64_t* corners, int64_t* bytes, 
   if (!ctx) return MCBA_ERR_ARG;
   REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "mcba_upload has not been called");
   const DeviceProblem& P = ctx->P;
-  const int np = nparts_for(P.model);
   int64_t per_corner = 18, per_view = 16, l = 1;
-  if (which == MCBA_BENCH_LINEARIZE) { l = 1; (void)np; }
-  else if (which == MCBA_BENCH_RESIDUAL) { per_corner = 18 + 4 + 16; }
+  if (which == MCBA_BENCH_RESIDUAL) per_corner = 18 + 4 + 16;
   if (corners) *corners = P.N;
-  if (bytes) *bytes = per_corner * P.N + per_view * P.V;      // per LAUNCH (each PART re-reads the corners)
+  if (bytes) *bytes = per_corner * P.N + per_view * P.V;      // per launch
   if (launches) *launches = (int32_t)l;
   return MCBA_OK;
 }
@@ -1627,10 +1525,9 @@ int mcba_bench_launch(mcba_ctx* ctx, int which, int repeats) {
   int r;
   if (!(which & MCBA_BENCH_NO_PREPARE)) { r = prepare(ctx, P); if (r) return r; }
   which &= ~MCBA_BENCH_NO_PREPARE;
-  struct SolvingFlag { bool& f; explicit SolvingFlag(bool& r) : f(r) { f = true; } ~SolvingFlag() { f = false; } } solving_flag(ctx->solving);   // time what a solve runs
   for (int i = 0; i < repeats; i++) {
     ViewKernelArgs a{}; a.loss = 0; a.f_scale = 1.0;
-    if (which == MCBA_BENCH_LINEARIZE) { if (ctx->fused_lin) r = launch_linearize(ctx, P, 0, 1.0); else { a.moments = ctx->moments.p; r = launch_moments(ctx, P, a); } }
+    if (which == MCBA_BENCH_LINEARIZE) r = launch_linearize(ctx, P, 0, 1.0);
     else if (which == MCBA_BENCH_COST) { a.view_cost = ctx->view_cost.p; r = launch_views<MODE_COST>(ctx, P, a); }
     else { ctx->err = "unsupported bench kernel"; return MCBA_ERR_ARG; }
     if (r) return r;

@@ -33,12 +33,12 @@ enum {
   RED_GMAX_F,                                                    // k_scale                     (all-reduce, max)
   RED_AGG, RED_AGN, RED_ANN, RED_DOTGN_F, RED_GN2_F,           // quadratic forms + dots      (1 all-reduce, sum)
   RED_COSTNEW, RED_STEP2_F, RED_XN2_F,                          // trial step                  (1 all-reduce, sum)
-  RED_COST,                                                      // cost at the linearisation   (grouped with g_s, diag_s)
+  RED_COST,                                                      // cost at the linearisation   (grouped with g_s)
   RED_GH2_S, RED_XS2_S, RED_GMAX_S, RED_DOTGN_S, RED_GN2_S, RED_STEP2_S, RED_XN2_S,   // replicated (shared) parts: never reduced
   RED_COUNT
 };
 
-// ---- NVLink peer-memory exchange (peer_allreduce.cuh): argument block, also taken by the kernels that run an exchange as their tail
+// ---- NVLink peer-memory exchange of k_lm (lm_kernel.cuh LmPeer): layout of the per-rank buffers
 constexpr int PEER_MAX_WORLD = 16;
 constexpr int PEER_MAX_SEG = 6;
 constexpr int PEER_FLAG_STRIDE = 8;      // doubles (64 B) between flags

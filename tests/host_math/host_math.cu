@@ -54,6 +54,9 @@ int hm_project(int model, int n, const double* X, const double* k, double* uv, d
 void hm_rodrigues(const double* r, double* R, double* JL) { rodrigues(r, R, JL); }
 void hm_matrix_to_rtvec(const double* T, double* rt) { matrix_to_rtvec(T, rt); }
 void hm_twist_map(const double* Rl, const double* JL, const double* t, double* A) { twist_map(Rl, JL, t, A); }
+void hm_hand_eye_frame_map(const double* RG, const double* RA, const double* JLW, const double* JLG, const double* tG, const double* tf, double* M) {
+  hand_eye_frame_map(RG, RA, JLW, JLG, tG, tf, M);
+}
 void hm_tr2d(double b11, double b12, double b22, double g1, double g2, double Delta, double* p) { solve_tr_2d(b11, b12, b22, g1, g2, Delta, p[0], p[1]); }
 void hm_loss(int loss, double z, double* r) { loss_rho(loss, z, r[0], r[1], r[2]); }
 }

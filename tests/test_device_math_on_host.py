@@ -36,6 +36,7 @@ def hm():
   lib.hm_spd_solve8.argtypes = [D, D]
   lib.hm_rodrigues.argtypes = [D, D, D]
   lib.hm_twist_map.argtypes = [D, D, D, D]
+  lib.hm_hand_eye_frame_map.argtypes = [D] * 7
   lib.hm_matrix_to_rtvec.argtypes = [D, D]
   lib.hm_tr2d.argtypes = [C.c_double] * 6 + [D]
   lib.hm_loss.argtypes = [C.c_int, C.c_double, D]
@@ -144,6 +145,31 @@ def test_twist_map_is_the_derivative_of_the_pose_chain(hm):
     num = (xcam(rf + d[:3], tf + d[3:]) - xcam(rf - d[:3], tf - d[3:])) / 2e-6
     xi = A[:, j]                                      # (omega, v)
     assert np.abs(np.cross(xi[:3], x0) + xi[3:] - num).max() < 1e-8
+
+
+
+def test_hand_eye_frame_map_factors_the_hand_eye_twist_maps(hm):
+  """Hand-eye frame T_f = G A_f W.  The maps of W (left part T_c G A_f, chain translation t_cf) and of G (left part T_c, chain translation
+  R_c t_G + t_c) are the frame's own map, taken with JL = I, times M_f (csrc/kernels.cuh hand_eye_frame_map): what lets k_fold_hand_eye
+  build the hand-eye blocks from the per-frame ones."""
+  rng = np.random.default_rng(5)
+  c = lambda a: np.ascontiguousarray(a, dtype=np.float64)
+  def tmap(Rl, JL, t):
+    A = np.zeros(36); hm.hm_twist_map(dp(c(Rl.ravel())), dp(c(JL.ravel())), dp(c(t)), dp(A)); return A.reshape(6, 6)
+  for trial in range(20):
+    Rc, RG, RA, RW = (Rotation.from_rotvec(rng.normal(0, 1.0, 3)).as_matrix() for _ in range(4))
+    tc, tG, tA, tW = (rng.normal(0, 0.5, 3) for _ in range(4))
+    JLW, JLG = np.zeros(9), np.zeros(9)
+    hm.hm_rodrigues(dp(c(rng.normal(0, 1.0, 3))), dp(np.zeros(9)), dp(JLW))
+    hm.hm_rodrigues(dp(c(rng.normal(0, 1.0, 3))), dp(np.zeros(9)), dp(JLG))
+    JLW, JLG = JLW.reshape(3, 3), JLG.reshape(3, 3)
+    RGA, tGA = RG @ RA, RG @ tA + tG
+    tf = RGA @ tW + tGA
+    tcf = Rc @ tf + tc
+    M = np.zeros(72)
+    hm.hm_hand_eye_frame_map(dp(c(RG.ravel())), dp(c(RA.ravel())), dp(c(JLW.ravel())), dp(c(JLG.ravel())), dp(c(tG)), dp(c(tf)), dp(M))
+    Eh = np.hstack([tmap(Rc @ RGA, JLW, tcf), tmap(Rc, JLG, Rc @ tG + tc)])
+    assert np.abs(tmap(Rc, np.eye(3), tcf) @ M.reshape(6, 12) - Eh).max() < 1e-14 * max(1.0, np.abs(Eh).max())
 
 
 def test_trust_region_2d_matches_scipy(hm):

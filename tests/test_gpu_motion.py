@@ -196,6 +196,21 @@ def test_mirror_classes_keep_the_reference_semantics(name):
   assert sorted(clone.motion.__getstate__()) == sorted(calib.motion.__getstate__())
 
 
+
+def test_two_identical_hand_eye_solves_agree_bit_for_bit():
+  """Hand-eye frames go through the same linearisation as static frames (the hand-eye blocks are fixed-order folds of the per-frame
+  blocks, k_fold_hand_eye): two identical solves, and two linearisations at the same point, agree bit for bit."""
+  z, calib, prob = make("handeye_2x6")
+  runs = [calib.bundle_adjust(tolerance=1e-9, max_iterations=30) for _ in range(2)]
+  assert runs[1].last_solve.cost == runs[0].last_solve.cost
+  assert np.array_equal(np.array(runs[1].last_solve.log, float), np.array(runs[0].last_solve.log, float), equal_nan=True)
+  assert np.array_equal(runs[1].param_vec, runs[0].param_vec)
+  eng = calib._upload(calib.inliers)
+  H0, g0, c0 = eng.linearize(z["x1"])
+  H1, g1, c1 = eng.linearize(z["x1"])
+  assert np.array_equal(H0, H1) and np.array_equal(g0, g1) and c0 == c1
+
+
 def test_hand_eye_calibration_wrapper_from_arm_poses():
   """HandEyeCalibration (optimization/hand_eye.py:13-97): robot-world initialisation from the arm's poses, then the GPU bundle adjustment
   over the 12 hand-eye parameters (+ board poses); the known transforms of the fixture are recovered."""

@@ -137,6 +137,7 @@ test_rolling_projection_without_measurements_iterates_like_the_reference = gm.te
 test_motion_state_entry_points_refuse_the_wrong_problem = gm.test_motion_state_entry_points_refuse_the_wrong_problem
 test_motion_mirror_classes_keep_the_reference_semantics = gm.test_mirror_classes_keep_the_reference_semantics
 test_hand_eye_calibration_wrapper_from_arm_poses = gm.test_hand_eye_calibration_wrapper_from_arm_poses
+test_two_identical_hand_eye_solves_agree_bit_for_bit = gm.test_two_identical_hand_eye_solves_agree_bit_for_bit
 test_motion_board_points_as_parameters_under_a_motion_model = gm.test_board_points_as_parameters_under_a_motion_model
 test_motion_outlier_loop_on_the_resident_table_equals_the_host_loop = gm.test_outlier_loop_on_the_resident_table_equals_the_host_loop
 
