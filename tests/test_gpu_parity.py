@@ -3,7 +3,7 @@
 Tolerances (all fp64 on the device):
   indexing / parameter layout ........ bit exact
   residuals at identical x ........... <= 1e-9 px       (observed ~5e-13)
-  J^T J, J^T r vs oracle 3-point FD .. <= 1e-6 relative (FD noise ~1e-8)
+  J^T J, J^T r vs oracle 5-point FD .. J^T J <= 1e-9 over sqrt(H_ii H_jj), J^T r <= 1e-10 max|J^T r| (FD noise ~1e-11)
   converged cost vs dense exact-TR oracle (scipy tr_solver='exact', tight tolerances) <= 1e-8 relative
   gauge-normalised converged parameters vs the same oracle: intrinsics rel 1e-6, poses 1e-6
   final cost at the reference's default tolerance: never worse than the reference's own result (+1e-6 rel)
@@ -17,6 +17,7 @@ from conftest import GOLDEN_CASES, load_golden, optimize_of
 from multical_b200 import synthetic
 from multical_b200.calibration import from_scene, select_threshold
 from oracle.ba_oracle import Problem, matrix_to_rtvec
+from test_gpu_step_parity import fd5_jacobian
 
 pytestmark = pytest.mark.gpu
 
@@ -58,16 +59,17 @@ def test_normal_equations_match_finite_differences(name):
   scene, z, calib, prob = make(name)
   eng = calib._upload(calib.inliers)
   x1 = z["x1"]
-  S = prob.sparsity_matrix()
-  J = approx_derivative(prob.residuals, x1, method="3-point", sparsity=(S, group_columns(S))).toarray()
+  J = fd5_jacobian(prob, x1)
   r = prob.residuals(x1)
-  H, g = J.T @ J, J.T @ r
+  H, g = (J.T @ J).toarray(), J.T @ r
   JtJ, Jtr, cost = eng.linearize(x1)
   nrm = np.sqrt(np.outer(np.diag(H), np.diag(H)))
   live = nrm > 0
-  assert (np.abs(JtJ - H)[live] / nrm[live]).max() < 1e-6
+  # fisheye k4 (theta^9) is so weakly excited (H_ii ~ 1e-2) that the rounding of the pixel values (~1e-13 px) over the difference step
+  # already moves its finite-difference entries by ~1e-9 of sqrt(H_ii H_jj)
+  assert (np.abs(JtJ - H)[live] / nrm[live]).max() < (3e-9 if name == "fisheye_3x5" else 1e-9)
   assert np.abs(JtJ[~live]).max(initial=0.0) == 0.0                   # dead columns (skew, invalid poses) stay exactly zero
-  assert np.abs(Jtr - g).max() < 1e-6 * np.abs(g).max()
+  assert np.abs(Jtr - g).max() < 1e-10 * np.abs(g).max()
   assert abs(cost - 0.5 * r @ r) < 1e-12 * cost
   assert np.abs(JtJ - JtJ.T).max() <= 1e-12 * np.abs(JtJ).max()
 
@@ -248,12 +250,11 @@ def test_fixed_blocks_and_fix_aspect():
   assert np.abs(eng2.param_vec - x0).max() < 1e-13
   x1 = x0 + np.random.default_rng(4).normal(0, 1e-3, x0.size)
   assert np.abs(eng2.residuals(x1) - prob2.residuals(x1)).max() < 1e-9
-  S = prob2.sparsity_matrix()
-  J = approx_derivative(prob2.residuals, x1, method="3-point", sparsity=(S, group_columns(S))).toarray()
+  J = fd5_jacobian(prob2, x1)
   JtJ, Jtr, _ = eng2.linearize(x1)
-  H = J.T @ J
+  H = (J.T @ J).toarray()
   nrm = np.sqrt(np.outer(np.diag(H), np.diag(H))); live = nrm > 0
-  assert (np.abs(JtJ - H)[live] / nrm[live]).max() < 1e-6
+  assert (np.abs(JtJ - H)[live] / nrm[live]).max() < 1e-9
   out2 = calib2.bundle_adjust(tolerance=1e-10)
   for c in out2.cameras: assert c.intrinsic[0, 0] == c.intrinsic[1, 1]
 
@@ -364,17 +365,18 @@ def test_board_points_as_parameters():
   x1 = x0 + np.random.default_rng(8).normal(0, 1e-3, x0.size)
   r1 = eng.residuals(calib._to_engine_vec(x1))
   assert np.abs(r1 - prob.residuals(x1)).max() < 1e-9
-  S = prob.sparsity_matrix()
-  J = approx_derivative(prob.residuals, x1, method="3-point", sparsity=(S, group_columns(S))).toarray()
-  H, g = J.T @ J, J.T @ prob.residuals(x1)
+  J = fd5_jacobian(prob, x1)
+  H, g = (J.T @ J).toarray(), J.T @ prob.residuals(x1)
   JtJ, Jtr, cost = eng.linearize(calib._to_engine_vec(x1))
   keep = calib._board_block_slices()
   head = JtJ.shape[0] - keep.size
   sel = np.concatenate([np.ones(head, bool), keep])
   JtJ, Jtr = JtJ[np.ix_(sel, sel)], Jtr[sel]
   nrm = np.sqrt(np.outer(np.diag(H), np.diag(H))); live = nrm > 0
-  assert (np.abs(JtJ - H)[live] / nrm[live]).max() < 1e-6
-  assert np.abs(Jtr - g).max() < 1e-6 * np.abs(g).max()
+  # k3 (r^6) of these small cube boards has H_ii ~ 1e-3: the rounding of the pixel values alone moves its finite-difference entries by
+  # ~4e-9 of sqrt(H_ii H_jj)
+  assert (np.abs(JtJ - H)[live] / nrm[live]).max() < 1e-8
+  assert np.abs(Jtr - g).max() < 1e-10 * np.abs(g).max()
   # the solve: never worse than the reference algorithm, and board points actually move
   out = calib.bundle_adjust(tolerance=1e-8, max_iterations=60)
   _, ref = prob.bundle_adjust(tolerance=1e-8, max_iterations=60)
@@ -428,11 +430,11 @@ def test_degenerate_block_selections(opt):
     x1 = x0 + np.random.default_rng(9).normal(0, 1e-3, x0.size)
     assert np.abs(eng.residuals(x1) - prob.residuals(x1)).max() < 1e-9
     S = prob.sparsity_matrix()
-    J = approx_derivative(prob.residuals, x1, method="3-point", sparsity=(S, group_columns(S))).toarray()
+    J = fd5_jacobian(prob, x1)
     JtJ, Jtr, _ = eng.linearize(x1)
-    H = J.T @ J
+    H = (J.T @ J).toarray()
     nrm = np.sqrt(np.outer(np.diag(H), np.diag(H))); live = nrm > 0
-    assert (np.abs(JtJ - H)[live] / nrm[live]).max() < 1e-6
+    assert (np.abs(JtJ - H)[live] / nrm[live]).max() < 1e-9
   out = calib.bundle_adjust(tolerance=1e-10, max_iterations=60)
   r0 = prob.residuals()
   assert out.last_solve.cost <= 0.5 * r0 @ r0 * (1 + 1e-12)

@@ -106,3 +106,23 @@ def test_oracle_against_live_reference():
   S = prob.sparsity_matrix().tocsr(); S.sort_indices()
   assert tuple(S.shape) == tuple(z["sp_shape"])
   assert np.array_equal(S.indptr, z["sp_indptr"]) and np.array_equal(S.indices, z["sp_indices"])
+
+
+def test_fourth_order_differences_are_converged():
+  """fd5_jacobian (tests/test_gpu_step_parity.py), the reference of the 1e-9 normal-equation bar: halving its step moves J^T J by
+  less than 1e-10 (entries over sqrt(H_ii H_jj)) and J^T r by less than 1e-11 max|J^T r| on a 2-camera, 30-frame scene, and it agrees
+  with scipy's 3-point differences to their own noise (~1e-9)."""
+  from scipy.optimize._numdiff import approx_derivative, group_columns
+  from multical_b200 import synthetic
+  from test_gpu_step_parity import fd5_jacobian, normalised_h_error
+  scene = synthetic.make_scene(C=2, F=30, vis=0.3, seed=5)
+  prob = Problem.from_scene(scene, optimize=dict(cameras=True))
+  x = prob.param_vec
+  r = prob.residuals(x)
+  J, J2 = fd5_jacobian(prob, x), fd5_jacobian(prob, x, rel_step=5e-4)
+  H, H2 = (J.T @ J).toarray(), (J2.T @ J2).toarray()
+  assert normalised_h_error(H2, H) < 1e-10
+  assert np.abs(J.T @ r - J2.T @ r).max() < 1e-11 * np.abs(J.T @ r).max()
+  S = prob.sparsity_matrix()
+  J3 = approx_derivative(prob.residuals, x, method="3-point", sparsity=(S, group_columns(S)))
+  assert normalised_h_error((J3.T @ J3).toarray(), H) < 1e-8

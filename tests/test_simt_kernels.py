@@ -16,6 +16,7 @@ import test_gpu_parity as gp
 import test_gpu_table as gt
 import test_gpu_motion as gm
 import test_gpu_pnp as gn
+import test_gpu_step_parity as sp
 from multical_b200 import _native, calibration
 
 
@@ -118,6 +119,33 @@ def test_rolling_frames_with_a_frame_count_that_ends_in_a_partial_syrk_step():
                                max_nfev=200, method="trf", tr_solver="exact")
   out = calib.bundle_adjust(tolerance=1e-13, xtol=1e-13, gtol=1e-13, max_iterations=200)
   assert abs(out.last_solve.cost - ref.cost) <= 1e-8 * ref.cost, (out.last_solve.cost, ref.cost)
+
+
+# ---- tests/test_gpu_step_parity.py on the interpreter (the cheap shapes; the interpreter has 132 SMs unless SIMT_SMS says otherwise)
+@pytest.mark.parametrize("C", [1, 2, 3, 5])
+def test_step_parity_views_that_end_a_corner_chunk(C):
+  sp.run_chunk_tails(C)
+
+
+@pytest.mark.parametrize("motion", ["static", "rolling"])
+def test_step_parity_ctas_that_own_several_frames(motion, monkeypatch):
+  """One SM: 2 resident CTAs, 24 frames -> 12 frames per CTA (set before the first engine of the test is created)."""
+  monkeypatch.setenv("SIMT_SMS", "1")
+  sp.run_frames_per_cta(motion, 24, 1)
+
+
+def test_step_parity_hand_eye_beyond_one_fold_batch():
+  """70 frames: fold batches of 64 + 6."""
+  sp.run_hand_eye_folds(70, False)
+
+
+@pytest.mark.parametrize("n_s", [127, 128])
+def test_step_parity_reduced_solve_at_the_cholesky_boundary(n_s):
+  assert sp.run_reduced_solve(n_s, "static", 6, 132) == (8, 1)
+
+
+def test_step_parity_robust_loss():
+  sp.run_robust_loss("cauchy")
 
 
 # ---- tests/test_gpu_table.py on the interpreter
