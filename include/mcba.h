@@ -223,6 +223,27 @@ int  mcba_pnp_views(mcba_ctx* ctx, const mcba_problem_desc* desc, const int64_t*
                     const double* det_xy, const double* board_points, const double* intrinsics, const int32_t* board_grid,
                     double* poses, double* errors, int32_t* num_points, uint8_t* valid);
 
+/* -- single-camera intrinsic calibration (Camera.calibrate, camera.py:68-105: cv2.calibrateCameraExtended without an initial matrix) --
+ * mcba_intrinsic_init: the initialisation of every camera at once.  Detection lists and board_grid as for mcba_pnp_views;
+ * image_sizes int32[C][2] = (width, height); view_use uint8[C*F*B] selects the views of the current round (list w = (c*F+f)*B+b).
+ * Per camera: a homography per used view (board plane z = 0 -> pixels; board points and corners rounded to float32): normalised DLT,
+ * refined by Levenberg-Marquardt on its pixel reprojection error as cv2.findHomography does,
+ * then OpenCV's initIntrinsicParams2D (what cv2.initCameraMatrix2D exposes): principal point ((w-1)/2, (h-1)/2), (1/fx^2, 1/fy^2) by
+ * least squares over two vanishing-point rows per view; desc->optimize & MCBA_OPT_FIX_ASPECT gives fx = fy = their mean.
+ * Out: intrinsics f64[C][5+nd] = [fx fy cx cy 0 | zeros] (NaN focal lengths for a camera without a usable view), poses f64[C*F*B][4][4]
+ * (board wrt camera, k_pnp_views under K0 and zero distortion: OpenCV's findExtrinsicCameraParams2), ok uint8[C*F*B] (0 for unused views).
+ * Boards with any z != 0 fail with MCBA_ERR_UNSUPPORTED, as OpenCV refuses non-planar rigs without an initial matrix; so does the
+ * fisheye model.  Does not touch the uploaded problem.
+ * The solve itself is the engine's own: one camera, the used views as frames (frame pose = board wrt camera), camera and board poses at
+ * identity and fixed, optimize = MCBA_OPT_MOTION | MCBA_OPT_CAMERAS [| MCBA_OPT_FIX_ASPECT].  It iterates to its own tolerances: the
+ * minimum OpenCV's LM approaches, not the point where OpenCV's iteration limit stops it.
+ * mcba_view_errors: per view of the packed problem at the current parameters, sumsq f64[C*F*B] = sum of squared pixel errors (u and v)
+ * and count int64[C*F*B] = corners (both zero where there is no view): calibrateCameraExtended's perViewErrors = sqrt(sumsq / count). */
+int  mcba_intrinsic_init(mcba_ctx* ctx, const mcba_problem_desc* desc, const int64_t* det_start, const int32_t* det_ids,
+                         const double* det_xy, const double* board_points, const int32_t* board_grid, const int32_t* image_sizes,
+                         const uint8_t* view_use, double* intrinsics, double* poses, uint8_t* ok);
+int  mcba_view_errors(mcba_ctx* ctx, double* sumsq, int64_t* count);
+
 /* -- measurement hooks (bench.py): launch one kernel family on the context stream -------------- */
 enum { MCBA_BENCH_LINEARIZE = 0, MCBA_BENCH_RESIDUAL = 1, MCBA_BENCH_COST = 2,
        MCBA_BENCH_NO_PREPARE = 256 /* or-ed in: reuse the pose tables of the previous call (times the kernel alone) */ };

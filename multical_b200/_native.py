@@ -28,7 +28,8 @@ EXPORTS = ["mcba_create", "mcba_destroy", "mcba_last_error", "mcba_set_stream", 
            "mcba_num_params", "mcba_get_param_vec", "mcba_set_param_vec", "mcba_residuals",
            "mcba_linearize", "mcba_reprojection_error", "mcba_solve", "mcba_bench_launch", "mcba_bench_info",
            "mcba_table_upload", "mcba_table_from_detections", "mcba_table_download", "mcba_table_set_inliers",
-           "mcba_table_get_inliers", "mcba_table_select", "mcba_pnp_views", "mcba_table_errors", "mcba_table_error_ranks", "mcba_table_count_below", "mcba_table_reject"]
+           "mcba_table_get_inliers", "mcba_table_select", "mcba_pnp_views", "mcba_table_errors", "mcba_table_error_ranks", "mcba_table_count_below", "mcba_table_reject",
+           "mcba_intrinsic_init", "mcba_view_errors"]
 TABLE_VALID, TABLE_INLIERS = 0, 1
 
 
@@ -119,6 +120,8 @@ def load():
   lib.mcba_table_error_ranks.argtypes = [P, C.c_int, I64, C.c_int32, D]
   lib.mcba_table_count_below.argtypes = [P, C.c_int, D, C.c_int32, I64]
   lib.mcba_table_reject.argtypes = [P, C.c_double, I64, I64]
+  lib.mcba_intrinsic_init.argtypes = [P, C.POINTER(ProblemDesc), I64, I32, D, D, I32, I32, U8, D, D, U8]
+  lib.mcba_view_errors.argtypes = [P, D, I64]
   _lib = lib
   return lib
 

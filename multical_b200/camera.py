@@ -16,7 +16,8 @@ DIST_SIZE = dict(standard=5, rational=8, thin_prism=12, tilted=14, fisheye=4)
 class Camera(Parameters):
   engine_model = None      # resolved from .model
 
-  def __init__(self, image_size, intrinsic, dist, model="standard", fix_aspect=False, has_skew=False, **_):
+  def __init__(self, image_size, intrinsic, dist, model="standard", fix_aspect=False, has_skew=False, error_perview=None,
+               intrinsic_dataset={}, **_):
     assert model in MODELS, f"unknown camera model {model} options are {list(MODELS)}"
     self.model = model
     self.image_size = tuple(image_size)
@@ -24,6 +25,16 @@ class Camera(Parameters):
     self.dist = np.zeros(5) if dist is None else np.asarray(dist, np.float64)
     self.fix_aspect = fix_aspect
     self.has_skew = has_skew
+    self.error_perview = error_perview              # per-view RMS of the last intrinsic calibration (camera.py:40-41)
+    self.intrinsic_dataset = intrinsic_dataset      # {'board_ids', 'image_ids'} of the views it kept
+
+  @staticmethod
+  def calibrate(boards, intrinsic_error_limit, detections, image_size, max_iter=10, eps=1e-3, model="standard", fix_aspect=False,
+                has_skew=False, flags=0, max_images=None, **solve_opts):
+    """camera.py:68-105 on the GPU (multical_b200/intrinsics.py): (Camera, err)."""
+    from .intrinsics import calibrate
+    return calibrate(boards, intrinsic_error_limit, detections, image_size, max_iter=max_iter, eps=eps, model=model, fix_aspect=fix_aspect,
+                     has_skew=has_skew, flags=flags, max_images=max_images, **solve_opts)
 
   def __repr__(self): return f"Camera(intrinsic={self.intrinsic!r}, dist={self.dist!r}, image_size={self.image_size})"
 
@@ -72,6 +83,12 @@ class CameraFisheye(Camera):
     self.dist = np.zeros((4, 1)) if dist is None else np.asarray(dist, np.float64)
     self.fix_aspect = fix_aspect
     self.has_skew = has_skew
+
+
+def calibrate_cameras(boards, points, image_sizes, intrinsic_error_limit, **kwargs):
+  """camera.py:237-241 on the GPU (multical_b200/intrinsics.py): (cameras, errs)."""
+  from .intrinsics import calibrate_cameras
+  return calibrate_cameras(boards, points, image_sizes, intrinsic_error_limit, **kwargs)
 
 
 def engine_model_of(camera):

@@ -19,6 +19,7 @@
 #include "pack_kernels.cuh"
 #include "table_kernels.cuh"
 #include "pnp_kernels.cuh"
+#include "intrinsics_kernels.cuh"
 
 using namespace mcba;
 
@@ -98,6 +99,10 @@ struct mcba_ctx {
   struct PnpBuffers {
     DevBuf<int64_t> start; DevBuf<int32_t> ids, grid, n; DevBuf<double2> xy, und; DevBuf<double> bp, in, pose, err; DevBuf<uint8_t> ok;
   } pnp;
+  // intrinsic initialisation (mcba_intrinsic_init): used views, their homographies, K0
+  struct IntrinsicBuffers {
+    DevBuf<int32_t> used, cam_start, size; DevBuf<double> H, k0; DevBuf<uint8_t> hok;
+  } intrinsic;
 };
 
 #define CK(call)                                                                                   \
@@ -1015,6 +1020,114 @@ int mcba_pnp_views(mcba_ctx* ctx, const mcba_problem_desc* desc, const int64_t* 
   CK(cudaMemcpyAsync(errors, d_err.p, sizeof(double) * (size_t)nv, cudaMemcpyDeviceToHost, s));
   CK(cudaMemcpyAsync(num_points, d_n.p, sizeof(int32_t) * (size_t)nv, cudaMemcpyDeviceToHost, s));
   CK(cudaMemcpyAsync(valid, d_ok.p, (size_t)nv, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  return MCBA_OK;
+}
+
+// Initialisation of single-camera intrinsic calibration (intrinsics_kernels.cuh): one homography per used view, K0 per camera
+// (initIntrinsicParams2D), the initial per-view poses from k_pnp_views under K0 and zero distortion.  Independent of the uploaded problem.
+int mcba_intrinsic_init(mcba_ctx* ctx, const mcba_problem_desc* desc, const int64_t* det_start, const int32_t* det_ids, const double* det_xy,
+                        const double* board_points, const int32_t* board_grid, const int32_t* image_sizes, const uint8_t* view_use,
+                        double* intrinsics, double* poses, uint8_t* ok) {
+  if (!ctx || !desc) return MCBA_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  { int r = check_desc(ctx, desc); if (r) return r; }
+  REQUIRE(det_start && board_points && board_grid && image_sizes && view_use && intrinsics && poses && ok, MCBA_ERR_ARG, "null argument");
+  REQUIRE(desc->model != MODEL_FISHEYE, MCBA_ERR_UNSUPPORTED, "the intrinsic initialisation is for the pinhole camera models");
+  const int C = desc->C, F = desc->F, B = desc->B, Pn = desc->P, nv = C * F * B;
+  const int kint = 5 + model_nd(desc->model);
+  const int64_t total = det_start[nv];
+  REQUIRE(det_start[0] == 0 && total >= 0 && total < ((int64_t)1 << 31), MCBA_ERR_ARG, "bad detection offsets");
+  REQUIRE(total == 0 || (det_ids && det_xy), MCBA_ERR_ARG, "null detection arrays");
+  for (int w = 0; w < nv; w++) REQUIRE(det_start[w + 1] >= det_start[w], MCBA_ERR_ARG, "detection offsets are not a monotone CSR over C*F*B lists");
+  for (int64_t i = 0; i < total; i++) REQUIRE(det_ids[i] >= 0 && det_ids[i] < Pn, MCBA_ERR_ARG, "detection id outside [0, P)");
+  for (int b = 0; b < B; b++)
+    REQUIRE(board_grid[5 * b] > 0 && board_grid[5 * b + 1] > 0 && board_grid[5 * b + 2] > 0 && board_grid[5 * b] <= 64 && board_grid[5 * b + 1] <= 64,
+            MCBA_ERR_UNSUPPORTED, "id grids are limited to 64 x 64 (bit masks of the occupied rows / columns)");
+  for (int c = 0; c < C; c++) REQUIRE(image_sizes[2 * c] > 0 && image_sizes[2 * c + 1] > 0, MCBA_ERR_ARG, "image sizes must be positive");
+  // OpenCV estimates an initial camera matrix only for planar targets (all object points at z = 0)
+  for (size_t i = 0; i < (size_t)B * Pn; i++)
+    REQUIRE(board_points[3 * i + 2] == 0.0, MCBA_ERR_UNSUPPORTED, "non-planar board (z != 0): the initial camera matrix needs planar targets");
+  // used views grouped by camera, board-major inside a camera (the order of calibration_points, camera.py:229-235); the detection lists
+  // of unused views are emptied, so that k_pnp_views sees only the used ones
+  std::vector<int32_t> used, cam_start((size_t)C + 1, 0);
+  for (int c = 0; c < C; c++) {
+    for (int b = 0; b < B; b++) for (int f = 0; f < F; f++) { const int w = (c * F + f) * B + b; if (view_use[w]) used.push_back(w); }
+    cam_start[(size_t)c + 1] = (int32_t)used.size();
+  }
+  std::vector<int64_t> start((size_t)nv + 1, 0);
+  std::vector<int32_t> ids; std::vector<double> xy;
+  for (int w = 0; w < nv; w++) {
+    if (view_use[w]) {
+      ids.insert(ids.end(), det_ids + det_start[w], det_ids + det_start[w + 1]);
+      xy.insert(xy.end(), det_xy + 2 * det_start[w], det_xy + 2 * det_start[w + 1]);
+    }
+    start[(size_t)w + 1] = (int64_t)ids.size();
+  }
+  const int n_used = (int)used.size();
+  const int64_t kept = start[nv];
+  cudaStream_t s = ctx->stream;
+  auto& pb = ctx->pnp; auto& ib = ctx->intrinsic;
+  const size_t tot = (size_t)std::max<int64_t>(kept, 1);
+  CK(pb.start.alloc((size_t)nv + 1)); CK(pb.ids.alloc(tot)); CK(pb.xy.alloc(tot)); CK(pb.und.alloc(tot)); CK(pb.grid.alloc((size_t)B * 5));
+  CK(pb.bp.alloc((size_t)B * Pn * 3)); CK(pb.pose.alloc((size_t)nv * 16)); CK(pb.err.alloc(nv)); CK(pb.n.alloc(nv)); CK(pb.ok.alloc(nv));
+  CK(ib.used.alloc((size_t)std::max(n_used, 1))); CK(ib.cam_start.alloc((size_t)C + 1)); CK(ib.size.alloc((size_t)C * 2));
+  CK(ib.H.alloc((size_t)std::max(n_used, 1) * 9)); CK(ib.hok.alloc((size_t)std::max(n_used, 1))); CK(ib.k0.alloc((size_t)C * kint));
+  CK(cudaMemcpyAsync(pb.start.p, start.data(), sizeof(int64_t) * start.size(), cudaMemcpyHostToDevice, s));
+  if (kept) {
+    CK(cudaMemcpyAsync(pb.ids.p, ids.data(), sizeof(int32_t) * ids.size(), cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(pb.xy.p, xy.data(), sizeof(double) * xy.size(), cudaMemcpyHostToDevice, s));
+  }
+  CK(cudaMemcpyAsync(pb.grid.p, board_grid, sizeof(int32_t) * (size_t)B * 5, cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(pb.bp.p, board_points, sizeof(double) * (size_t)B * Pn * 3, cudaMemcpyHostToDevice, s));
+  if (n_used) CK(cudaMemcpyAsync(ib.used.p, used.data(), sizeof(int32_t) * used.size(), cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(ib.cam_start.p, cam_start.data(), sizeof(int32_t) * cam_start.size(), cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(ib.size.p, image_sizes, sizeof(int32_t) * (size_t)C * 2, cudaMemcpyHostToDevice, s));
+  if (n_used) {
+    HomographyArgs h{};
+    h.n_used = n_used; h.B = B; h.P = Pn; h.used = ib.used.p; h.det_start = pb.start.p; h.det_ids = pb.ids.p; h.det_xy = pb.xy.p;
+    h.board_pts = pb.bp.p; h.H = ib.H.p; h.ok = ib.hok.p;
+    k_view_homography<<<(n_used + HOMOG_WARPS - 1) / HOMOG_WARPS, HOMOG_WARPS * 32, 0, s>>>(h); CKL();
+  }
+  ZhangArgs z{};
+  z.kint = kint; z.fix_aspect = (desc->optimize & MCBA_OPT_FIX_ASPECT) ? 1 : 0; z.cam_start = ib.cam_start.p; z.image_size = ib.size.p;
+  z.H = ib.H.p; z.ok = ib.hok.p; z.intr = ib.k0.p;
+  k_zhang_init<<<C, ZHANG_THREADS, 0, s>>>(z); CKL();
+  if (nv) {
+    PnpArgs a{};
+    a.C = C; a.F = F; a.B = B; a.P = Pn; a.model = MODEL_STANDARD; a.kint = kint; a.nv = nv;
+    a.det_start = pb.start.p; a.det_ids = pb.ids.p; a.det_xy = pb.xy.p; a.board_pts = pb.bp.p; a.intr = ib.k0.p; a.grid = pb.grid.p;
+    a.und = pb.und.p; a.poses = pb.pose.p; a.err = pb.err.p; a.npts = pb.n.p; a.valid = pb.ok.p; a.max_iters = 50;
+    k_pnp_views<MODEL_STANDARD><<<(nv + PNP_WARPS - 1) / PNP_WARPS, PNP_WARPS * 32, 0, s>>>(a); CKL();     // zero distortion: the pinhole K0
+    CK(cudaMemcpyAsync(poses, pb.pose.p, sizeof(double) * 16 * (size_t)nv, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(ok, pb.ok.p, (size_t)nv, cudaMemcpyDeviceToHost, s));
+  }
+  CK(cudaMemcpyAsync(intrinsics, ib.k0.p, sizeof(double) * (size_t)C * kint, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  return MCBA_OK;
+}
+
+// Per-view sums of squared pixel errors and corner counts of the packed problem at the current parameters (intrinsics_kernels.cuh)
+int mcba_view_errors(mcba_ctx* ctx, double* sumsq, int64_t* count) {
+  if (!ctx || !sumsq || !count) return MCBA_ERR_ARG;
+  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "mcba_upload has not been called");
+  CK(cudaSetDevice(ctx->device));
+  DeviceProblem P = with_state(ctx, false);
+  const size_t nv = (size_t)P.C * P.F * P.B;
+  if (nv == 0) return MCBA_OK;
+  int r = prepare(ctx, P); if (r) return r;
+  DevBuf<double> ds; DevBuf<int64_t> dn;
+  CK(ds.alloc(nv)); CK(dn.alloc(nv));
+  cudaStream_t s = ctx->stream;
+  CK(cudaMemsetAsync(ds.p, 0, sizeof(double) * nv, s)); CK(cudaMemsetAsync(dn.p, 0, sizeof(int64_t) * nv, s));
+  if (P.V > 0) {
+    ViewKernelArgs a{}; a.loss = MCBA_LOSS_LINEAR; a.f_scale = 1.0; a.view_cost = ctx->view_cost.p;
+    r = launch_views<MODE_COST>(ctx, P, a); if (r) return r;
+    k_view_sumsq<<<(P.V + 255) / 256, 256, 0, s>>>(P, ctx->view_cost.p, ds.p, dn.p);
+    CKL();
+  }
+  CK(cudaMemcpyAsync(sumsq, ds.p, sizeof(double) * nv, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(count, dn.p, sizeof(int64_t) * nv, cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
   return MCBA_OK;
 }

@@ -184,6 +184,40 @@ class Engine:
                                      ok.ctypes.data_as(C.POINTER(C.c_uint8))))
     return (poses[:nv].reshape(Cn, F, B, 4, 4), err[:nv].reshape(Cn, F, B), npts[:nv].reshape(Cn, F, B), ok[:nv].reshape(Cn, F, B).astype(bool))
 
+  def intrinsic_init(self, model, dims, det_start, det_ids, det_xy, board_points, board_grid, image_sizes, view_use, fix_aspect=False):
+    """Initialisation of single-camera intrinsic calibration (include/mcba.h mcba_intrinsic_init) for every camera at once: list
+    w = (c*F+f)*B+b of detected point ids and pixel corners, view_use [C,F,B] the views of this round -> (K0 parameters [C, 5+nd] with
+    zero distortion, initial board-wrt-camera poses [C,F,B,4,4], ok [C,F,B])."""
+    Cn, F, B, P = (int(v) for v in dims)
+    nv = Cn * F * B
+    det_start = np.ascontiguousarray(det_start, dtype=np.int64)
+    assert det_start.shape == (nv + 1,), f"expected {nv + 1} list offsets, got {det_start.shape}"
+    det_ids = np.ascontiguousarray(det_ids, dtype=np.int32).reshape(-1)
+    det_xy = nat.f64(det_xy).reshape(-1, 2)
+    assert det_ids.size == det_xy.shape[0] == int(det_start[-1]), "detection arrays do not match the offsets"
+    bp = nat.f64(board_points).reshape(B, P, 3)
+    grid = np.ascontiguousarray(board_grid, dtype=np.int32).reshape(B, 5)
+    sizes = np.ascontiguousarray(image_sizes, dtype=np.int32).reshape(Cn, 2)
+    use = np.ascontiguousarray(view_use, dtype=np.uint8).reshape(nv)
+    intr = np.zeros((Cn, 5 + nat.DIST_SIZES[model]))
+    poses, ok = np.zeros((max(nv, 1), 4, 4)), np.zeros(max(nv, 1), np.uint8)
+    d = nat.ProblemDesc(Cn, F, B, P, nat.MODEL_IDS[model], nat.OPT_FIX_ASPECT if fix_aspect else 0, 0)
+    u8 = lambda a: a.ctypes.data_as(C.POINTER(C.c_uint8))
+    self._ck(self.lib.mcba_intrinsic_init(self.h, C.byref(d), det_start.ctypes.data_as(C.POINTER(C.c_int64)), nat.iptr(det_ids),
+                                          nat.dptr(det_xy), nat.dptr(bp), nat.iptr(grid), nat.iptr(sizes), u8(use), nat.dptr(intr),
+                                          nat.dptr(poses), u8(ok)))
+    return intr, poses[:nv].reshape(Cn, F, B, 4, 4), ok[:nv].reshape(Cn, F, B).astype(bool)
+
+  def view_errors(self):
+    """Per-view sums of squared pixel errors and corner counts of the uploaded problem at the current parameters, both [C,F,B]
+    (zero where there is no view): include/mcba.h mcba_view_errors."""
+    shape = self._dense_shape()[:3]
+    n = max(int(np.prod(shape)), 1)
+    sumsq, count = np.zeros(n), np.zeros(n, np.int64)
+    self._ck(self.lib.mcba_view_errors(self.h, nat.dptr(sumsq), count.ctypes.data_as(C.POINTER(C.c_int64))))
+    m = int(np.prod(shape))
+    return sumsq[:m].reshape(shape), count[:m].reshape(shape)
+
   def _dense_shape(self):
     d = self.desc
     return (d.C, d.F, d.B, d.P)

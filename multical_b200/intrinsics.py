@@ -1,0 +1,193 @@
+"""Single-camera intrinsic calibration on the GPU: `Camera.calibrate` and `calibrate_cameras` of the reference (multical/camera.py:68-105,
+237-241), which call cv2.calibrateCameraExtended once per round of a view-rejection loop, one camera at a time.
+
+What stays on the host is the bookkeeping of the reference: the view set (calibration_points, camera.py:184-195, 229-235), the optional
+`max_images` selection (top_detection_coverage, camera.py:206-227, with the same np.random.normal draws in the same order) and the loop
+(camera.py:84-99).  Per round:
+  1. one mcba_intrinsic_init for every camera still in the loop (include/mcba.h): homographies, OpenCV's initIntrinsicParams2D, per-view
+     poses by PnP under K0 (csrc/intrinsics_kernels.cuh);
+  2. per camera, the bundle-adjustment engine on a problem of one camera whose frames are its views (frame pose = board wrt camera;
+     camera and board poses fixed at identity), optimising the frames and the intrinsics (fx = fy under fix_aspect; skew is a dead column
+     as in OpenCV);
+  3. mcba_view_errors: the per-view RMS and the total RMS of calibrateCameraExtended.
+
+The solve iterates to its own tolerances (ftol = xtol = gtol = 1e-10, at most 100 evaluations): it reaches the minimum that OpenCV's
+Levenberg-Marquardt approaches, not the point where OpenCV's criteria (`max_iter`, `eps`: accepted for the reference's signature, unused)
+stop it -- with the reference's (10, 1e-3), OpenCV stops ~1e-5 relative away from it in fx.  The calibration runs on an engine of its own, so
+the process-wide bundle-adjustment engine keeps its problem."""
+import numpy as np
+
+from . import _native as nat
+from .board import stack_boards
+from .camera import Camera
+from .structs import struct
+
+SUPPORTED_MODELS = ("standard",)
+UNSUPPORTED = {
+  "rational": "k1..k3 and k4..k6 are nearly degenerate; in that valley the engine's trust region stops on xtol 1.7e-4 - 1.8e-4 above the "
+              "RMS OpenCV's LM settles at (50-view scenes, restarts do not help), so the result would not be OpenCV's minimum",
+  "thin_prism": "under CALIB_THIN_PRISM_MODEL OpenCV keeps k4..k6 at zero, and the engine cannot fix single distortion coefficients",
+  "tilted": "under CALIB_TILTED_MODEL OpenCV keeps k4..k6 and s1..s4 at zero, and the engine cannot fix single distortion coefficients",
+  "fisheye": "the reference's fisheye intrinsic calibration (camera_fisheye.py) is broken, and the engine cannot fix single coefficients",
+}
+
+_engines = {}
+
+
+def intrinsics_engine(device=None):
+  """An engine used only by the intrinsic calibration (one per GPU), so that calibration.get_engine()'s problem survives it."""
+  from .calibration import default_device
+  from .engine import Engine
+  device = default_device() if device is None else device
+  if device not in _engines:
+    _engines[device] = Engine(device)
+  return _engines[device]
+
+
+def image_bins(image_size, approx_bins=10):
+  """Bin edges over the image: square bins of side min(w, h) / approx_bins (camera.py:212-216)."""
+  side = min(image_size[0] / approx_bins, image_size[1] / approx_bins)
+  return [np.linspace(0, image_size[axis], int(image_size[axis] / side)) for axis in (0, 1)]
+
+
+def top_detection_coverage(views, k, image_size, approx_bins=10, jitter=0.1):
+  """The k views whose corners occupy the most bins of the image, ties broken by normal jitter (camera.py:219-227).  Draws one
+  np.random.normal per view in view order, as the reference does."""
+  bins = image_bins(image_size, approx_bins=10)
+  scale = jitter * approx_bins * approx_bins
+  score = []
+  for v in views:
+    hist, _, _ = np.histogram2d(v.corners[:, 0], v.corners[:, 1], bins)
+    score.append(-np.count_nonzero(hist) + np.random.normal(0, scale))
+  return [views[i] for i in np.argsort(score)][:k]
+
+
+def calibration_points(boards, detections):
+  """One view per (frame, board) with board.has_min_detections, board-major (camera.py:184-195, 229-235).  Corners and object points
+  are rounded to float32, as the reference hands them to OpenCV."""
+  views = []
+  for b, board in enumerate(boards):
+    for f, frame in enumerate(detections):
+      d = frame[b]
+      if board.has_min_detections(d):
+        ids = np.asarray(d.ids).reshape(-1)
+        views.append(struct(frame=f, board=b, ids=ids, corners=np.asarray(d.corners, np.float32).reshape(-1, 2),
+                            object_points=np.asarray(board.points, np.float64)[ids].astype(np.float32)))
+  return views
+
+
+def _check_model(model, flags):
+  if model in UNSUPPORTED:
+    raise NotImplementedError(f"intrinsic calibration of the {model} model: {UNSUPPORTED[model]}")
+  assert model in SUPPORTED_MODELS, f"unknown camera model {model}"
+  if flags:
+    raise NotImplementedError(f"extra OpenCV calibration flags ({flags}) are not supported")
+
+
+def _solve_camera(eng, model, fix_aspect, views, k0, poses, board_points, solve_opts):
+  """One calibrateCameraExtended: the views as frames of a one-camera problem, started from K0 and the PnP poses."""
+  nv = len(views)
+  B, P = board_points.shape[:2]
+  rows = np.concatenate([np.stack([np.zeros(v.ids.size, np.int32), np.full(v.ids.size, i, np.int32), np.full(v.ids.size, v.board, np.int32),
+                                   v.ids.astype(np.int32)], axis=1) for i, v in enumerate(views)])
+  obs = np.concatenate([v.corners.astype(np.float64) for v in views])
+  bits = nat.OPT_BITS["motion"] | nat.OPT_BITS["cameras"] | (nat.OPT_FIX_ASPECT if fix_aspect else 0)
+  eng.upload(model, bits, (1, nv, B, P), rows, obs, board_points)
+  mats = np.concatenate([np.eye(4)[None], np.tile(np.eye(4), (B, 1, 1)), poses])
+  eng.set_state_matrices(mats, k0[None])
+  info = eng.solve(**solve_opts)
+  sumsq, count = eng.view_errors()
+  per_view = np.array([sumsq[0, i, v.board] for i, v in enumerate(views)])
+  n = np.array([count[0, i, v.board] for i, v in enumerate(views)])
+  _, _, frame_rt, intr = eng.get_params()
+  return struct(intrinsics=intr[0], rtvecs=frame_rt, per_view=np.sqrt(per_view / n), rms=float(np.sqrt(per_view.sum() / n.sum())),
+                solve=info)
+
+
+def calibrate_views(boards, cam_views, image_sizes, model="standard", fix_aspect=False, engine=None, camera_ids=None, **solve_opts):
+  """One calibrateCameraExtended for each camera's list of views (calibration_points entries, any order): returns per camera a struct of
+  the intrinsics [fx fy cx cy skew dist...], the views' rtvecs (board wrt camera), per-view RMS, total RMS, K0 and the solve summary.
+  camera_ids: how errors name the cameras (default: their position in cam_views)."""
+  eng = engine or intrinsics_engine()
+  opts = dict(ftol=1e-10, xtol=1e-10, gtol=1e-10, max_nfev=100)
+  opts.update(solve_opts)
+  board_points = stack_boards(boards)[0].astype(np.float32).astype(np.float64)
+  F = max(max((v.frame for v in views), default=0) for views in cam_views) + 1
+  B, P = board_points.shape[:2]
+  Cn = len(cam_views)
+  # detection lists of the views only: every other list of the [C, F, B] grid is empty
+  counts = np.zeros(Cn * F * B, np.int64)
+  order = sorted(((c, v.frame, v.board, v) for c, views in enumerate(cam_views) for v in views), key=lambda t: (t[0] * F + t[1]) * B + t[2])
+  for c, f, b, v in order: counts[(c * F + f) * B + b] = v.ids.size
+  det_start = np.concatenate([[0], np.cumsum(counts)]).astype(np.int64)
+  det_ids = np.concatenate([t[3].ids for t in order]).astype(np.int32) if order else np.zeros(0, np.int32)
+  det_xy = np.concatenate([t[3].corners.astype(np.float64) for t in order]) if order else np.zeros((0, 2))
+  use = counts.reshape(Cn, F, B) > 0
+  grid = np.array([[1, 1, 1, 0, 0]] * B, np.int32)              # the views are chosen already: no minimum-detections rule on the device
+  k0, poses, ok = eng.intrinsic_init(model, (Cn, F, B, P), det_start, det_ids, det_xy, board_points, grid, image_sizes, use, fix_aspect)
+  out = []
+  names = list(range(len(cam_views))) if camera_ids is None else list(camera_ids)
+  for c, views in enumerate(cam_views):
+    if not np.isfinite(k0[c]).all():
+      raise ValueError(f"camera {names[c]}: no initial camera matrix (degenerate homographies)")
+    sel = [(v.frame, v.board) for v in views]
+    if not all(ok[c, f, b] for f, b in sel):
+      raise ValueError(f"camera {names[c]}: the initial pose of a view failed")
+    res = _solve_camera(eng, model, fix_aspect, views, k0[c], np.stack([poses[c, f, b] for f, b in sel]), board_points, opts)
+    res.k0 = k0[c]
+    out.append(res)
+  return out
+
+
+def _camera_of(res, image_size, model, fix_aspect, has_skew, views, per_view):
+  x = res.intrinsics
+  K = np.array([[x[0], 0.0, x[2]], [0.0, x[1], x[3]], [0.0, 0.0, 1.0]])
+  return Camera(image_size=image_size, intrinsic=K, dist=x[5:].reshape(1, -1), model=model, fix_aspect=fix_aspect, has_skew=has_skew,
+                error_perview=per_view.reshape(-1, 1),
+                intrinsic_dataset={"board_ids": [np.float64(v.board) for v in views], "image_ids": [v.frame for v in views]})
+
+
+def calibrate_cameras(boards, points, image_sizes, intrinsic_error_limit, max_iter=10, eps=1e-3, model="standard", fix_aspect=False,
+                      has_skew=False, flags=0, max_images=None, **solve_opts):
+  """camera.py:237-241: (cameras, errs) for the nested detections points[camera][frame][board] = struct(corners, ids).  Every camera runs
+  the loop of camera.py:84-99 on its own views; the initialisation of a round is one launch for all cameras still in the loop.
+  `max_iter` / `eps` are accepted for the reference's signature: the device solves to its own tolerances (module docstring); the keyword
+  arguments ftol, xtol, gtol, max_nfev go to the solve."""
+  del max_iter, eps
+  _check_model(model, flags)
+  Cn = len(points)
+  views, err, result, per_view = [], [None] * Cn, [None] * Cn, [None] * Cn
+  for c in range(Cn):
+    v = calibration_points(boards, points[c])
+    if not v:
+      raise ValueError(f"camera {c}: no view with the minimum detections of its board")
+    if max_images is not None:
+      v = top_detection_coverage(v, max_images, image_sizes[c])
+    views.append(v)
+  active = list(range(Cn))
+  while active:
+    res = calibrate_views(boards, [views[c] for c in active], [image_sizes[c] for c in active], model, fix_aspect, camera_ids=active,
+                          **solve_opts)
+    still = []
+    for c, r in zip(active, res):
+      result[c], per_view[c] = r, r.per_view
+      if len(views[c]) >= 15:
+        err[c] = float("{:.2f}".format(r.rms))
+        threshold = np.quantile(r.per_view, 0.95)
+        views[c] = [v for v, e in zip(views[c], r.per_view) if e < threshold]
+        if abs(err[c]) >= intrinsic_error_limit: still.append(c)
+      else:
+        # the reference raises its limit by 0.1 and calibrates the same views again until the limit passes the (unrounded) error:
+        # identical input, identical result
+        err[c] = r.rms
+    active = still
+  cams = [_camera_of(result[c], tuple(image_sizes[c]), model, fix_aspect, has_skew, views[c], per_view[c]) for c in range(Cn)]
+  return cams, err
+
+
+def calibrate(boards, intrinsic_error_limit, detections, image_size, max_iter=10, eps=1e-3, model="standard", fix_aspect=False,
+              has_skew=False, flags=0, max_images=None, **solve_opts):
+  """Camera.calibrate (camera.py:68-105) for one camera's detections[frame][board]: (Camera, err)."""
+  cams, errs = calibrate_cameras(boards, [detections], [image_size], intrinsic_error_limit, max_iter=max_iter, eps=eps, model=model,
+                                 fix_aspect=fix_aspect, has_skew=has_skew, flags=flags, max_images=max_images, **solve_opts)
+  return cams[0], errs[0]

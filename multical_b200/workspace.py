@@ -1,5 +1,7 @@
-"""The two `Workspace` methods either side of the hot path, as functions over a `Calibration` (the rest of the reference's `Workspace` --
-image loading, detection, export -- is out of scope and stays the reference's own):
+"""The `Workspace` methods around the hot path, as functions over a `Calibration` or the detections (the rest of the reference's
+`Workspace` -- image loading, detection, export -- is out of scope and stays the reference's own):
+  calibrate_single(boards, detected_points, ...)   = Workspace.calibrate_single   multical/workspace.py:165-194 (the pinhole branch:
+                                    every camera's intrinsics, multical_b200/intrinsics.py)
 
   calibrate(calib, ...)          = Workspace.calibrate          multical/workspace.py:228-247  (enable the chosen blocks, then the outlier
                                     loop around bundle_adjust with the quantile selectors the command line builds, config/workspace.py:47-58)
@@ -9,7 +11,15 @@ image loading, detection, export -- is out of scope and stays the reference's ow
 A `Workspace` keeps working unchanged when its module imports `Calibration`, `select_threshold` and `tables.make_pose_table` from this
 package (INTEGRATION.md A, D); these functions are the same steps for callers that do not carry a `Workspace` around (bench.py, tests)."""
 from .calibration import Calibration, select_threshold
+from .intrinsics import calibrate_cameras
 from .tables import make_pose_table
+
+
+def calibrate_single(boards, detected_points, image_sizes, camera_model, intrinsic_error_limit, fix_aspect=False, has_skew=False,
+                     max_images=None):
+  """workspace.py:165-180 (the pinhole branch): every camera's intrinsics from its detections[frame][board] -> (cameras, errs)."""
+  return calibrate_cameras(boards, detected_points, image_sizes, intrinsic_error_limit, model=camera_model, fix_aspect=fix_aspect,
+                           has_skew=has_skew, max_images=max_images)
 
 
 def calibrate(calib: Calibration, camera_poses=True, motion=True, board_poses=True, cameras=False, boards=False,
