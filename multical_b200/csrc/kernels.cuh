@@ -1,6 +1,6 @@
 // kernels.cuh — sm_90a kernels of the bundle-adjustment hot path.
 //
-// Data layout in HBM (built once by mcba_upload, solver.cu): corners are stored FRAME-MAJOR, sorted by
+// Data layout in HBM (built once per upload: on the host by mcba_upload, on the device by pack_kernels.cuh): corners are stored FRAME-MAJOR, sorted by
 // (frame, camera, board, point), so that every "view" (frame,camera,board) is one contiguous run and all
 // views of one frame are contiguous (frames are also the multi-GPU sharding unit, SURVEY.md §8e):
 //   obs   double2[N]   observed (u,v)                       16 B / corner   (point_table.points, calibration.py:206)
@@ -34,11 +34,9 @@ struct DeviceProblem {
   const int* view_frame;
   const int* view_board;
   const int* frame_view_start;   // [F+1]
-  const int* cam_view_start;     // [C+1]
-  const int* cam_view_list;      // [V] view ids grouped by camera
   double* board_pts;             // [B][P][3]  (parameters when off_pt >= 0: boards=True, board/charuco.py:112-117)
-  // parameter state (full, including fixed blocks)
-  double* cam_rt;    // [C][6]
+  // parameter state (full, including fixed blocks): one block laid out by state_layout (solver.cu), board_pts and he_rt included
+  double* cam_rt;    // [C][6]   first: the base of the block
   double* board_rt;  // [B][6]
   double* frame_rt;  // [F][6]
   double* intr;      // [C][kint]
@@ -176,15 +174,15 @@ __global__ void k_state_to_matrices(int C, int B, int F, const double* cam_rt, c
 
 // trial parameter state = current state with the free blocks replaced by x (internal order), and the pose tables of that state (item i
 // of one pass of k_lm).  One item per pose, then one per camera (intrinsics), per board point, and one for the hand-eye pair (which
-// must be complete before the derived frame poses: those items recompute it themselves).
-__device__ __forceinline__ void make_trial_item(const DeviceProblem& p, const double* x, double* cam_o, double* board_o, double* frame_o, double* intr_o,
-                                                double* bpts_o, double* he_o, int i) {
+// must be complete before the derived frame poses: those items recompute it themselves).  `trial` has the layout of the current state.
+__device__ __forceinline__ void make_trial_item(const DeviceProblem& p, const double* x, double* trial, int i) {
   const int nfp = p.F * p.npf;
   const int np = p.C + p.B + nfp;
+  auto to_trial = [&](const double* cur) { return trial + (cur - p.cam_rt); };      // the twin of a current-state entry
   if (i < np) {
     const double* cur; const double* src = nullptr; double* dst; PoseT* tab;
-    if (i < p.C) { cur = p.cam_rt + 6 * i; dst = cam_o + 6 * i; tab = p.cam_T + i; if (p.off_cp >= 0) src = x + p.off_cp + 6 * i; }
-    else if (i < p.C + p.B) { const int b = i - p.C; cur = p.board_rt + 6 * b; dst = board_o + 6 * b; tab = p.board_T + b; if (p.off_bp >= 0) src = x + p.off_bp + 6 * b; }
+    if (i < p.C) { cur = p.cam_rt + 6 * i; dst = to_trial(cur); tab = p.cam_T + i; if (p.off_cp >= 0) src = x + p.off_cp + 6 * i; }
+    else if (i < p.C + p.B) { const int b = i - p.C; cur = p.board_rt + 6 * b; dst = to_trial(cur); tab = p.board_T + b; if (p.off_bp >= 0) src = x + p.off_bp + 6 * b; }
     else {
       const int q = i - p.C - p.B;
       if (p.motion == MOTION_HAND_EYE) {
@@ -194,7 +192,7 @@ __device__ __forceinline__ void make_trial_item(const DeviceProblem& p, const do
         PoseT t; hand_eye_frame(he, p.arm_T[q], t); p.frame_T[q] = t;
         return;
       }
-      cur = p.frame_rt + 6 * q; dst = frame_o + 6 * q; tab = p.frame_T + q; if (p.motion_on) src = x + p.n_s + 6 * q;
+      cur = p.frame_rt + 6 * q; dst = to_trial(cur); tab = p.frame_T + q; if (p.motion_on) src = x + p.n_s + 6 * q;
     }
     if (!src) src = cur;
     double v[6];
@@ -206,21 +204,24 @@ __device__ __forceinline__ void make_trial_item(const DeviceProblem& p, const do
   } else if (i < np + p.C) {
     const int c = i - np;
     const double* src = p.off_in >= 0 ? x + p.off_in + p.kint * c : p.intr + p.kint * c;
+    double* dst = to_trial(p.intr + p.kint * c);
     for (int j = 0; j < p.kint; j++) {
       double v = __ldcg(&src[j]);
       if (j == 1 && p.fix_aspect && p.off_in >= 0) v = __ldcg(&src[0]);      // fy follows fx (camera.py:159-160)
-      intr_o[p.kint * c + j] = v;
+      dst[j] = v;
     }
   } else if (i < np + p.C + p.B * p.P) {
     const int q = i - np - p.C;                                       // padded board point index b*P + p
     const double* src = p.off_pt >= 0 ? x + p.off_pt + 3 * q : p.board_pts + 3 * q;
-    bpts_o[3 * q] = __ldcg(&src[0]); bpts_o[3 * q + 1] = __ldcg(&src[1]); bpts_o[3 * q + 2] = __ldcg(&src[2]);
+    double* dst = to_trial(p.board_pts + 3 * q);
+    dst[0] = __ldcg(&src[0]); dst[1] = __ldcg(&src[1]); dst[2] = __ldcg(&src[2]);
   } else if (i < np + p.C + p.B * p.P + 2 && p.motion == MOTION_HAND_EYE) {
     const int j = i - np - p.C - p.B * p.P;
     const double* src = p.off_he >= 0 ? x + p.off_he + 6 * j : p.he_rt + 6 * j;
+    double* dst = to_trial(p.he_rt + 6 * j);
     double v[6];
 #pragma unroll
-    for (int k = 0; k < 6; k++) { v[k] = __ldcg(&src[k]); he_o[6 * j + k] = v[k]; }
+    for (int k = 0; k < 6; k++) { v[k] = __ldcg(&src[k]); dst[k] = v[k]; }
     PoseT t;
     pose_from_rt(v, t);
     p.he_T[j] = t;

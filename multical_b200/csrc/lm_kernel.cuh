@@ -25,7 +25,6 @@ namespace mcba {
 
 constexpr int LM_THREADS = 256;
 constexpr int LM_WARPS = LM_THREADS / 32;
-constexpr int LM_MAX_SEG = 8;
 
 __device__ __forceinline__ unsigned long long lm_ld_volatile(const unsigned long long* p) {
   unsigned long long v;
@@ -76,7 +75,7 @@ struct LmPeer {                      // NVLink peer-memory exchange (one buffer 
 
 struct LmArgs {
   DeviceProblem P;                   // parameter pointers = the CURRENT state; pose tables = the state last linearised (the trial)
-  double *cam_rt2, *board_rt2, *frame_rt2, *intr2, *board_pts2, *he_rt2;      // TRIAL parameter state (what k_linearize reads)
+  double* trial; int state_len;      // TRIAL parameter state (what k_linearize reads): the layout of the current one, state_len doubles
   int n, n_s, F, fb, n_items;
   // linearisation at the trial point (k_linearize + k_reduce_shared [+ add-on kernels])
   const double* Hss; const double* Hff; const double* W; const double* g; const double* frame_cost; const double* lin_cost;
@@ -90,7 +89,6 @@ struct LmArgs {
   SolverState* st;
   mcba_log_row* log; int log_cap;
   unsigned long long* bar;
-  int opt_loss;                      // unused by the kernel (the linearisation kernels apply the loss); kept for the log
   LmPeer peer;
   unsigned long long cond_handle; int use_cond;      // CUDA-graph WHILE node: the kernel sets the loop condition itself
   unsigned long long* prof;          // MCBA_PROF=1: %globaltimer at the phase boundaries of the last launch (CTA 0), else null
@@ -799,24 +797,15 @@ k_lm(LmArgs a) {
       exchange(a, seg, 3, ++xseq, &xerr);
       cost_new = __ldcg(&a.part_quad[0]); s2f = __ldcg(&a.part_quad[1]); x2f = __ldcg(&a.part_quad[2]);
     }
-    if (tid == 0) {
-      double red[RED_COUNT];
-      red[RED_COSTNEW] = cost_new; red[RED_STEP2_S] = S.step2_s; red[RED_STEP2_F] = s2f; red[RED_XN2_S] = S.xn2_s; red[RED_XN2_F] = x2f;
-      accept_compute(&S, red);
-    }
+    if (tid == 0) accept_compute(&S, cost_new, S.step2_s, s2f, S.xn2_s, x2f);
     __syncthreads();
     const bool accepted = S.accepted != 0, may_retry = S.status == -99 && S.nfev < S.max_nfev;
     __syncthreads();                                    // thread 0 updates S below: every thread has its copy of the decision first
     if (accepted) {
       // x = x_new ; cost = cost_new ; J = jac(x)  (trf.py): the trial state becomes the current one
       for (int i = gthread; i < n; i += gstride) a.x[i] = a.x_new[i];
-      const DeviceProblem& p = a.P;
-      for (int i = gthread; i < 6 * p.C; i += gstride) p.cam_rt[i] = a.cam_rt2[i];
-      for (int i = gthread; i < 6 * p.B; i += gstride) p.board_rt[i] = a.board_rt2[i];
-      for (int i = gthread; i < p.F * (p.fb > 0 ? p.fb : 6) && p.motion != MOTION_HAND_EYE; i += gstride) p.frame_rt[i] = a.frame_rt2[i];
-      for (int i = gthread; i < p.kint * p.C; i += gstride) p.intr[i] = a.intr2[i];
-      for (int i = gthread; i < 3 * p.B * p.P && p.off_pt >= 0; i += gstride) p.board_pts[i] = a.board_pts2[i];
-      for (int i = gthread; i < 12 && p.motion == MOTION_HAND_EYE; i += gstride) p.he_rt[i] = a.he_rt2[i];
+      // (the fixed blocks of the trial state equal the current ones: the solve starts from a copy, make_trial_item copies them)
+      for (int i = gthread; i < a.state_len; i += gstride) a.P.cam_rt[i] = a.trial[i];
       if (tid == 0) {
         S.cost = S.cost_new; S.njev += 1; S.last_reduction = S.actual_reduction; S.last_step_norm = S.step_norm;
         S.iteration += 1; S.accepted = 0; S.pending = 0;
@@ -883,10 +872,7 @@ k_lm(LmArgs a) {
         gh2f = __ldcg(&a.part_quad[0]); xs2f = __ldcg(&a.part_quad[1]); gmf = __ldcg(&a.part_quad[2]);
       }
       if (tid == 0) {
-        double red[RED_COUNT];
-        red[RED_GH2_S] = gh2s; red[RED_GH2_F] = gh2f; red[RED_GMAX_S] = gms; red[RED_GMAX_F] = gmf; red[RED_XS2_S] = xs2s; red[RED_XS2_F] = xs2f;
-        red[RED_COST] = multi ? first_cost : lin_cost;                    // only read on the first call (begin_iteration)
-        begin_iteration(&S, red);
+        begin_iteration(&S, gh2s, gh2f, gms, gmf, xs2s, xs2f, multi ? first_cost : lin_cost);     // the cost is read on the first call only
         if (!isfinite(S.cost)) { S.done = 1; S.status = -2; }          // non-finite residuals at the initial point (scipy raises ValueError)
       }
       __syncthreads();
@@ -969,7 +955,7 @@ k_lm(LmArgs a) {
         exchange(a, seg, 1, ++xseq, &xerr);
         agg = __ldcg(&a.part_quad[0]);
       }
-      if (tid == 0) { double red[RED_COUNT]; red[RED_AGG] = agg; reg_compute(&S, red); S.agg = agg; }
+      if (tid == 0) { reg_compute(&S, agg); S.agg = agg; }
       __syncthreads();
     }
     LMPH(4)
@@ -1112,12 +1098,7 @@ k_lm(LmArgs a) {
         exchange(a, seg, 1, ++xseq, &xerr);
         agn = __ldcg(&a.part_quad[0]); ann = __ldcg(&a.part_quad[1]); dtf = __ldcg(&a.part_quad[2]); g2f = __ldcg(&a.part_quad[3]);
       }
-      if (tid == 0) {
-        double red[RED_COUNT];
-        red[RED_AGG] = S.agg; red[RED_AGN] = agn; red[RED_ANN] = ann;
-        red[RED_DOTGN_S] = dts; red[RED_DOTGN_F] = dtf; red[RED_GN2_S] = g2s; red[RED_GN2_F] = g2f;
-        subspace_compute(&S, red);
-      }
+      if (tid == 0) subspace_compute(&S, S.agg, agn, ann, dts, dtf, g2s, g2f);
       __syncthreads();
     }
   }
@@ -1128,12 +1109,12 @@ k_lm(LmArgs a) {
   __syncthreads();
   {
     const double al = S.alpha, be = S.beta;
-    double s2s = 0, s2f = 0, x2s = 0, x2f = 0;
+    double s2f = 0, x2f = 0;
     for (int i = gthread; i < n; i += gstride) {
       const double stp = a.d[i] * (al * a.gh[i] + be * __ldcg(&a.gn[i]));
       const double xi = a.x[i];
       a.x_new[i] = xi + stp;
-      if (i < n_s) { s2s += stp * stp; x2s += xi * xi; } else { s2f += stp * stp; x2f += xi * xi; }
+      if (i >= n_s) { s2f += stp * stp; x2f += xi * xi; }
     }
     // the shared entries are few (n_s): every CTA sums them itself (replicated); the frame parts go to per-CTA records for the next launch
     double ss = 0, xs = 0;
@@ -1144,12 +1125,11 @@ k_lm(LmArgs a) {
     }
     ss = block_sum_all(ss, sm); xs = block_sum_all(xs, sm);
     const double r0 = block_sum_all(s2f, sm), r1 = block_sum_all(x2f, sm);
-    (void)s2s; (void)x2s;
     if (tid == 0) { a.part_step[(size_t)blockIdx.x * 2] = r0; a.part_step[(size_t)blockIdx.x * 2 + 1] = r1; S.step2_s = ss; S.xn2_s = xs; S.step_parts = nblk; S.pending = 1; }
   }
   grid_barrier(a.bar, nblk);
   for (int i = gthread; i < a.n_items; i += gstride)
-    make_trial_item(a.P, a.x_new, a.cam_rt2, a.board_rt2, a.frame_rt2, a.intr2, a.board_pts2, a.he_rt2, i);
+    make_trial_item(a.P, a.x_new, a.trial, i);
   __syncthreads();
   LMPH(10)
   if (writer) {

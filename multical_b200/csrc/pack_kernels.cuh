@@ -8,9 +8,10 @@
 
 namespace mcba {
 
-// one warp per view (c,f,b): number of selected points; written in canonical (c,f,b) and frame-major (f,c,b) order
-// view_valid (may be null): views whose camera / frame / board pose is invalid select nothing (calibration.py:73-79)
-__global__ void k_pack_count(const uint8_t* mask, const uint8_t* view_valid, int C, int F, int B, int P, int* cnt_can, int* cnt_fm, int* flag_can, int* flag_fm) {
+// one warp per view (c,f,b): number of selected points, written in canonical (c,f,b) and frame-major (f,c,b) order, and whether the
+// view has any (frame-major order).  view_valid (may be null): views whose camera / frame / board pose is invalid select nothing
+// (calibration.py:73-79)
+__global__ void k_pack_count(const uint8_t* mask, const uint8_t* view_valid, int C, int F, int B, int P, int* cnt_can, int* cnt_fm, int* flag_fm) {
   const int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (w >= C * F * B) return;
   const int b = w % B, f = (w / B) % F, c = w / (B * F);
@@ -22,7 +23,7 @@ __global__ void k_pack_count(const uint8_t* mask, const uint8_t* view_valid, int
   for (int o = 16; o > 0; o >>= 1) n += __shfl_xor_sync(0xffffffffu, n, o);
   if (lane == 0) {
     const int wf = (f * C + c) * B + b;
-    cnt_can[w] = n; cnt_fm[wf] = n; flag_can[w] = n > 0; flag_fm[wf] = n > 0;
+    cnt_can[w] = n; cnt_fm[wf] = n; flag_fm[wf] = n > 0;
   }
 }
 
@@ -61,7 +62,7 @@ __global__ void k_scan_exclusive(int* data_all, int n, int stride) {
 struct PackOut {
   double2* obs; uint16_t* pid; uint32_t* orig;
   int* view_start; int* view_cam; int* view_frame; int* view_board;
-  int* frame_view_start; int* cam_view_start; int* cam_view_list;
+  int* frame_view_start;
 };
 
 // one warp per view: scatter the selected corners to their frame-major slot; lane 0 emits the view record
@@ -69,16 +70,15 @@ struct PackOut {
 // float32), the packed observations are f64 either way (exact)
 template <typename PT>
 __global__ void k_pack_scatter(const uint8_t* mask, const PT* points, int C, int F, int B, int P,
-                               const int* off_can, const int* off_fm, const int* vid_can, const int* vid_fm, PackOut o) {
+                               const int* off_can, const int* off_fm, const int* vid_fm, PackOut o) {
   const int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   const int nv = C * F * B;
   if (w >= nv) return;
   const int b = w % B, f = (w / B) % F, c = w / (B * F);
   const int wf = (f * C + c) * B + b;
   if (lane == 0) {
-    if (b == 0 && f == 0) o.cam_view_start[c] = vid_can[w];
     if (b == 0 && c == 0) o.frame_view_start[f] = vid_fm[wf];
-    if (w == nv - 1) { o.cam_view_start[C] = vid_can[nv]; o.frame_view_start[F] = vid_fm[nv]; o.view_start[vid_fm[nv]] = off_fm[nv]; }
+    if (w == nv - 1) { o.frame_view_start[F] = vid_fm[nv]; o.view_start[vid_fm[nv]] = off_fm[nv]; }
   }
   const int base_fm = off_fm[wf], base_can = off_can[w];
   const int count = off_can[w + 1] - base_can;
@@ -86,7 +86,6 @@ __global__ void k_pack_scatter(const uint8_t* mask, const PT* points, int C, int
   if (lane == 0) {
     const int vid = vid_fm[wf];
     o.view_start[vid] = base_fm; o.view_cam[vid] = c; o.view_frame[vid] = f; o.view_board[vid] = b;
-    o.cam_view_list[vid_can[w]] = vid;
   }
   const uint8_t* m = mask + (size_t)w * P;
   const PT* pt = points + (size_t)w * P;

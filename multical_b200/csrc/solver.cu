@@ -10,6 +10,7 @@
 #include <cstdlib>
 #include <string>
 #include <chrono>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/mcba.h"
@@ -41,6 +42,38 @@ struct DevBuf {
   }
 };
 
+// The parameter state is one block of doubles, [cam_rt 6C | board_rt 6B | frame_rt F fbs | intr kint C | he_rt 12 | board_pts 3BP] with
+// fbs = max(fb, 6) doubles per frame: the current state (ctx->params) and the trial state (ctx->trial: what k_lm proposes, k_linearize
+// evaluates) share it.  The board points come last: the uploads write them before the problem is set up, which zeroes everything in
+// front of them.
+struct StateLayout { size_t board, frame, intr, he, pts, len; };      // offsets of the blocks (cam_rt at 0) and the length
+
+StateLayout state_layout(const mcba_problem_desc& d) {
+  const size_t fbs = (d.optimize & MCBA_MOTION_ROLLING) ? 12 : 6;
+  StateLayout L;
+  L.board = 6 * (size_t)d.C; L.frame = L.board + 6 * (size_t)d.B; L.intr = L.frame + fbs * d.F;
+  L.he = L.intr + (size_t)(5 + model_nd(d.model)) * d.C; L.pts = L.he + 12; L.len = L.pts + 3 * (size_t)d.B * d.P;
+  return L;
+}
+
+// the parameter pointers of P into a state block
+void set_state_pointers(DeviceProblem& P, double* base, const StateLayout& L) {
+  P.cam_rt = base; P.board_rt = base + L.board; P.frame_rt = base + L.frame; P.intr = base + L.intr; P.he_rt = base + L.he; P.board_pts = base + L.pts;
+}
+
+// calls f(integral_constant<int, MODEL>, bool_constant<ROLL>) with the runtime camera model and rolling-shutter choice as constants
+template <typename Fn>
+void with_model(int model, bool roll, Fn&& f) {
+  auto pick = [&](auto M) { if (roll) f(M, std::true_type{}); else f(M, std::false_type{}); };
+  switch (model) {
+    case MODEL_STANDARD: pick(std::integral_constant<int, MODEL_STANDARD>{}); break;
+    case MODEL_RATIONAL: pick(std::integral_constant<int, MODEL_RATIONAL>{}); break;
+    case MODEL_THIN_PRISM: pick(std::integral_constant<int, MODEL_THIN_PRISM>{}); break;
+    case MODEL_TILTED: pick(std::integral_constant<int, MODEL_TILTED>{}); break;
+    default: pick(std::integral_constant<int, MODEL_FISHEYE>{}); break;
+  }
+}
+
 }  // namespace
 
 struct mcba_ctx {
@@ -56,15 +89,15 @@ struct mcba_ctx {
   DeviceProblem P{};
   // problem arrays
   DevBuf<double2> obs; DevBuf<uint16_t> pid; DevBuf<uint32_t> orig;
-  DevBuf<int> view_start, view_cam, view_frame, view_board, frame_view_start, cam_view_start, cam_view_list;
-  DevBuf<double> board_pts, cam_rt, board_rt, frame_rt, intr;
+  DevBuf<int> view_start, view_cam, view_frame, view_board, frame_view_start;
   DevBuf<uint8_t> dense_mask, view_valid; DevBuf<double2> dense_pts; DevBuf<float2> dense_pts32; DevBuf<int> scan;
   cudaStream_t copy_stream = nullptr; cudaEvent_t copy_done = nullptr, copy_go = nullptr;      // observations of mcba_upload_dense* in flight beside the view count
   DevBuf<PoseT> cam_T, frame_T, board_T;
-  // trial parameter state
-  DevBuf<double> cam_rt2, board_rt2, frame_rt2, intr2, board_pts2, pose_mats;
-  // motion models: image heights (rolling), hand-eye pair (current / trial) with its pose table and the fixed arm poses
-  DevBuf<double> img_h, he_rt, he_rt2; DevBuf<PoseT> he_T, arm_T;
+  // parameter state (state_layout): current and trial
+  StateLayout layout{};
+  DevBuf<double> params, trial, pose_mats;
+  // motion models: image heights (rolling), the hand-eye pose table and the fixed arm poses
+  DevBuf<double> img_h; DevBuf<PoseT> he_T, arm_T;
   // solver buffers
   DevBuf<double> Hss, g, Hff, W, view_cost;
   // linearisation (linearize.cuh): per-(CTA, camera) records of the shared blocks, per-camera board partials, per-frame costs
@@ -80,7 +113,8 @@ struct mcba_ctx {
   struct SolveGraph { cudaGraphExec_t exec = nullptr; cudaGraph_t graph = nullptr; std::vector<char> key; cudaStream_t stream = nullptr; int body_launches = 0; } sg;
   bool graph_launched = false;
   int lin_grid = 1, lin_split = 1, lin_warps = LIN_WARPS;
-  DevBuf<double> x, x_new, sinv, d, gh, gn, Y, Lf, zf, S, rhs, red, Linv;
+  DevBuf<double> x, x_new, sinv, d, gh, gn, Y, Lf, zf, S, rhs, Linv;
+  DevBuf<double> lin_cost, eval_cost;     // cost at the last linearisation (k_reduce_shared), cost of mcba_residuals
   DevBuf<SolverState> state;
   // NVLink peer-memory exchange of the solver kernel (lm_kernel.cuh LmPeer)
   double* peer_own = nullptr; int peer_cap = 0; bool peer_ready = false;
@@ -159,36 +193,22 @@ int launch_views(mcba_ctx* ctx, const DeviceProblem& P, const ViewKernelArgs& a)
   const int blocks = std::max(1, std::min((P.V + VIEW_WARPS - 1) / VIEW_WARPS, ctx->num_sms * 8));
   const int th = VIEW_WARPS * 32;
   cudaStream_t s = ctx->stream;
-#define LV(MODEL) if (P.motion == MOTION_ROLLING) k_views<MODEL, MODE, true><<<blocks, th, 0, s>>>(P, a); else k_views<MODEL, MODE, false><<<blocks, th, 0, s>>>(P, a);
-  switch (P.model) {
-    case MODEL_STANDARD: LV(MODEL_STANDARD) break;
-    case MODEL_RATIONAL: LV(MODEL_RATIONAL) break;
-    case MODEL_THIN_PRISM: LV(MODEL_THIN_PRISM) break;
-    case MODEL_TILTED: LV(MODEL_TILTED) break;
-    default: LV(MODEL_FISHEYE) break;
-  }
-#undef LV
+  with_model(P.model, P.motion == MOTION_ROLLING, [&](auto M, auto R) {
+    constexpr int MODEL = decltype(M)::value; constexpr bool ROLL = decltype(R)::value;
+    k_views<MODEL, MODE, ROLL><<<blocks, th, 0, s>>>(P, a);
+  });
   CKL();
   return MCBA_OK;
 }
 
 // ---------------------------------------------------------------- linearisation (linearize.cuh)
-template <int MODEL, bool ROLL>
-size_t lin_smem_bytes(const DeviceProblem& P, int warps) {
-  using S = LinShape<MODEL, ROLL>;
-  return sizeof(double) * lin_smem_doubles(S::NC, S::T, S::D, S::FB, S::NIN, P.B, S::NP, warps);
-}
 size_t lin_smem_for(const DeviceProblem& P, int warps) {
-  const bool roll = P.motion == MOTION_ROLLING;
-#define LS(MODEL) return roll ? lin_smem_bytes<MODEL, true>(P, warps) : lin_smem_bytes<MODEL, false>(P, warps);
-  switch (P.model) {
-    case MODEL_STANDARD: LS(MODEL_STANDARD)
-    case MODEL_RATIONAL: LS(MODEL_RATIONAL)
-    case MODEL_THIN_PRISM: LS(MODEL_THIN_PRISM)
-    case MODEL_TILTED: LS(MODEL_TILTED)
-    default: LS(MODEL_FISHEYE)
-  }
-#undef LS
+  size_t bytes = 0;
+  with_model(P.model, P.motion == MOTION_ROLLING, [&](auto M, auto R) {
+    using S = LinShape<decltype(M)::value, decltype(R)::value>;
+    bytes = sizeof(double) * lin_smem_doubles(S::NC, S::T, S::D, S::FB, S::NIN, P.B, S::NP, warps);
+  });
+  return bytes;
 }
 // one launch: H_ff, g_f, W_f, frame costs and the per-CTA records of the shared blocks at the (trial or current) state
 int launch_linearize(mcba_ctx* ctx, const DeviceProblem& P, int loss, double f_scale) {
@@ -196,25 +216,19 @@ int launch_linearize(mcba_ctx* ctx, const DeviceProblem& P, int loss, double f_s
   LinArgs a{}; a.loss = loss; a.f_scale = f_scale; a.split = ctx->lin_split;
   a.Hff = ctx->Hff.p; a.g = ctx->g.p; a.W = ctx->W.p; a.spart = ctx->spart.p; a.frame_cost = ctx->frame_cost.p;
   const size_t sm = lin_smem_for(P, ctx->lin_warps);
-  const bool roll = P.motion == MOTION_ROLLING;
   const int th = ctx->lin_warps * 32;
   cudaStream_t s = ctx->stream;
-#define LL(MODEL) if (roll) k_linearize<MODEL, true><<<ctx->lin_grid, th, sm, s>>>(P, a); else k_linearize<MODEL, false><<<ctx->lin_grid, th, sm, s>>>(P, a);
-  switch (P.model) {
-    case MODEL_STANDARD: LL(MODEL_STANDARD) break;
-    case MODEL_RATIONAL: LL(MODEL_RATIONAL) break;
-    case MODEL_THIN_PRISM: LL(MODEL_THIN_PRISM) break;
-    case MODEL_TILTED: LL(MODEL_TILTED) break;
-    default: LL(MODEL_FISHEYE) break;
-  }
-#undef LL
+  with_model(P.model, P.motion == MOTION_ROLLING, [&](auto M, auto R) {
+    constexpr int MODEL = decltype(M)::value; constexpr bool ROLL = decltype(R)::value;
+    k_linearize<MODEL, ROLL><<<ctx->lin_grid, th, sm, s>>>(P, a);
+  });
   CKL();
   return MCBA_OK;
 }
 // per-CTA records -> H_ss, g_s, cost (stores, fixed summation order)
 int launch_reduce_shared(mcba_ctx* ctx, const DeviceProblem& P) {
   ReduceArgs r{}; r.spart = ctx->spart.p; r.nparts = P.F > 0 ? ctx->lin_grid : 0; r.Hss = ctx->Hss.p; r.g = ctx->g.p; r.bpart = ctx->bpart.p;
-  r.frame_cost = ctx->frame_cost.p; r.F = P.F; r.cost_out = ctx->red.p + RED_COST; r.cam_counter = ctx->cam_counter.p; r.sred = ctx->sred.p;
+  r.frame_cost = ctx->frame_cost.p; r.F = P.F; r.cost_out = ctx->lin_cost.p; r.cam_counter = ctx->cam_counter.p; r.sred = ctx->sred.p;
   const size_t sm = sizeof(double) * reduce_smem_doubles(P.T, P.D, P.B);
   const int grid = P.C * reduce_slices(lin_record_doubles(P.T, P.D, P.B));
   if (P.motion == MOTION_ROLLING) k_reduce_shared<2><<<grid, RED_THREADS, sm, ctx->stream>>>(P, r);
@@ -226,7 +240,7 @@ int launch_reduce_shared(mcba_ctx* ctx, const DeviceProblem& P) {
 // DeviceProblem view whose parameter pointers are the trial state
 DeviceProblem with_state(const mcba_ctx* ctx, bool trial) {
   DeviceProblem P = ctx->P;
-  if (trial) { P.cam_rt = ctx->cam_rt2.p; P.board_rt = ctx->board_rt2.p; P.frame_rt = ctx->frame_rt2.p; P.intr = ctx->intr2.p; P.board_pts = ctx->board_pts2.p; P.he_rt = ctx->he_rt2.p; }
+  if (trial) set_state_pointers(P, ctx->trial.p, ctx->layout);
   return P;
 }
 
@@ -263,17 +277,10 @@ int linearize(mcba_ctx* ctx, int loss, double f_scale, bool trial = false) {
   if (P.off_pt >= 0 && P.V > 0) {
     ViewKernelArgs a{}; a.loss = loss; a.f_scale = f_scale;
     const int blocks = std::max(1, std::min((P.V + VIEW_WARPS - 1) / VIEW_WARPS, ctx->num_sms * 8));
-    const bool roll = P.motion == MOTION_ROLLING;
-#define PB(MODEL) if (roll) k_point_blocks<MODEL, 2><<<blocks, VIEW_WARPS * 32, 0, s>>>(P, a, ctx->Hss.p, ctx->W.p, ctx->g.p); \
-                  else k_point_blocks<MODEL, 1><<<blocks, VIEW_WARPS * 32, 0, s>>>(P, a, ctx->Hss.p, ctx->W.p, ctx->g.p);
-    switch (P.model) {
-      case MODEL_STANDARD: PB(MODEL_STANDARD) break;
-      case MODEL_RATIONAL: PB(MODEL_RATIONAL) break;
-      case MODEL_THIN_PRISM: PB(MODEL_THIN_PRISM) break;
-      case MODEL_TILTED: PB(MODEL_TILTED) break;
-      default: PB(MODEL_FISHEYE) break;
-    }
-#undef PB
+    with_model(P.model, P.motion == MOTION_ROLLING, [&](auto M, auto R) {
+      constexpr int MODEL = decltype(M)::value; constexpr int NP = decltype(R)::value ? 2 : 1;
+      k_point_blocks<MODEL, NP><<<blocks, VIEW_WARPS * 32, 0, s>>>(P, a, ctx->Hss.p, ctx->W.p, ctx->g.p);
+    });
     CKL();
   }
   if (P.off_he >= 0) {
@@ -283,26 +290,19 @@ int linearize(mcba_ctx* ctx, int loss, double f_scale, bool trial = false) {
   return MCBA_OK;
 }
 
-// cost at the TRIAL state -> red[RED_COSTNEW]
-int trial_cost(mcba_ctx* ctx, int loss, double f_scale, bool trial, int slot) {
+// cost at the (trial or current) state -> eval_cost
+int trial_cost(mcba_ctx* ctx, int loss, double f_scale, bool trial) {
   DeviceProblem P = with_state(ctx, trial);
   ViewKernelArgs a{}; a.loss = loss; a.f_scale = f_scale; a.view_cost = ctx->view_cost.p;
   int r = launch_views<MODE_COST>(ctx, P, a); if (r) return r;
-  k_sum_partials<<<1, 1024, 0, ctx->stream>>>(ctx->view_cost.p, P.V, 1, 1, ctx->red.p + slot); CKL();
+  k_sum_partials<<<1, 1024, 0, ctx->stream>>>(ctx->view_cost.p, P.V, 1, 1, ctx->eval_cost.p); CKL();
   return MCBA_OK;
 }
 
 // ---------------------------------------------------------------- the device-resident trust-region loop (lm_kernel.cuh)
 // trial parameter state := current state
 int copy_state_to_trial(mcba_ctx* ctx) {
-  const DeviceProblem& P = ctx->P;
-  cudaStream_t s = ctx->stream;
-  CK(cudaMemcpyAsync(ctx->cam_rt2.p, ctx->cam_rt.p, sizeof(double) * P.C * 6, cudaMemcpyDeviceToDevice, s));
-  CK(cudaMemcpyAsync(ctx->board_rt2.p, ctx->board_rt.p, sizeof(double) * P.B * 6, cudaMemcpyDeviceToDevice, s));
-  if (P.F && P.fb) CK(cudaMemcpyAsync(ctx->frame_rt2.p, ctx->frame_rt.p, sizeof(double) * P.F * P.fb, cudaMemcpyDeviceToDevice, s));
-  CK(cudaMemcpyAsync(ctx->he_rt2.p, ctx->he_rt.p, sizeof(double) * 12, cudaMemcpyDeviceToDevice, s));
-  CK(cudaMemcpyAsync(ctx->intr2.p, ctx->intr.p, sizeof(double) * P.C * P.kint, cudaMemcpyDeviceToDevice, s));
-  CK(cudaMemcpyAsync(ctx->board_pts2.p, ctx->board_pts.p, sizeof(double) * P.B * P.P * 3, cudaMemcpyDeviceToDevice, s));
+  CK(cudaMemcpyAsync(ctx->trial.p, ctx->params.p, sizeof(double) * ctx->layout.len, cudaMemcpyDeviceToDevice, ctx->stream));
   return MCBA_OK;
 }
 
@@ -310,12 +310,11 @@ LmArgs make_lm_args(mcba_ctx* ctx, int log_cap) {
   const DeviceProblem& P = ctx->P;
   LmArgs a{};
   a.P = P;
-  a.cam_rt2 = ctx->cam_rt2.p; a.board_rt2 = ctx->board_rt2.p; a.frame_rt2 = ctx->frame_rt2.p; a.intr2 = ctx->intr2.p;
-  a.board_pts2 = ctx->board_pts2.p; a.he_rt2 = ctx->he_rt2.p;
+  a.trial = ctx->trial.p; a.state_len = (int)ctx->layout.len;
   a.n = P.n; a.n_s = P.n_s; a.F = P.F; a.fb = P.fb;
   a.n_items = P.C + P.B + P.F * P.npf + P.C + P.B * P.P + 2;
   a.Hss = ctx->Hss.p; a.Hff = ctx->Hff.p; a.W = ctx->W.p; a.g = ctx->g.p;
-  a.frame_cost = ctx->frame_cost.p; a.lin_cost = ctx->red.p + RED_COST;
+  a.frame_cost = ctx->frame_cost.p; a.lin_cost = ctx->lin_cost.p;
   a.x = ctx->x.p; a.x_new = ctx->x_new.p; a.sinv = ctx->sinv.p; a.d = ctx->d.p; a.gh = ctx->gh.p; a.gn = ctx->gn.p;
   a.Y = ctx->Y.p; a.Lf = ctx->Lf.p; a.zf = ctx->zf.p; a.S = ctx->S.p; a.rhs = ctx->rhs.p; a.Spart = ctx->Spart.p; a.rpart = ctx->rpart.p; a.Linv = ctx->Linv.p;
   a.syrk_chunks = ctx->syrk_chunks; a.syrk_cf = ctx->syrk_cf;
@@ -413,6 +412,15 @@ int run_lm_loop(mcba_ctx* ctx, int loss, double f_scale, int log_cap) {
   return MCBA_OK;
 }
 
+// the current and trial parameter state of `desc` (kept when they already fit: a re-selected table keeps its state); board_pts, if not
+// null, receives where the uploads write the board points
+int alloc_state(mcba_ctx* ctx, const mcba_problem_desc* desc, double** board_pts) {
+  ctx->layout = state_layout(*desc);
+  CK(ctx->params.alloc(ctx->layout.len)); CK(ctx->trial.alloc(ctx->layout.len));
+  if (board_pts) *board_pts = ctx->params.p + ctx->layout.pts;
+  return MCBA_OK;
+}
+
 // dimensions, variable layout, permutation and every solver buffer that depends on (C,F,B,P,N,V)
 int setup_problem(mcba_ctx* ctx, const mcba_problem_desc* desc, int64_t N, int V, bool keep_state = false) {
   const int C = desc->C, F = desc->F, B = desc->B, Pn = desc->P;
@@ -455,11 +463,9 @@ int setup_problem(mcba_ctx* ctx, const mcba_problem_desc* desc, int64_t N, int V
   }
 
   const size_t fbs = (size_t)std::max(P.fb, 6);      // doubles per frame in frame_rt and in the per-frame solver blocks
-  CK(ctx->cam_rt.alloc((size_t)C * 6)); CK(ctx->board_rt.alloc((size_t)B * 6)); CK(ctx->frame_rt.alloc((size_t)std::max(F, 1) * fbs)); CK(ctx->intr.alloc((size_t)C * P.kint));
-  CK(ctx->cam_rt2.alloc((size_t)C * 6)); CK(ctx->board_rt2.alloc((size_t)B * 6)); CK(ctx->frame_rt2.alloc((size_t)std::max(F, 1) * fbs)); CK(ctx->intr2.alloc((size_t)C * P.kint));
+  { int r = alloc_state(ctx, desc, nullptr); if (r) return r; }
   CK(ctx->cam_T.alloc(C)); CK(ctx->frame_T.alloc((size_t)std::max(F, 1) * P.npf)); CK(ctx->board_T.alloc(B));
-  CK(ctx->img_h.alloc(C)); CK(ctx->he_rt.alloc(12)); CK(ctx->he_rt2.alloc(12)); CK(ctx->he_T.alloc(2)); CK(ctx->arm_T.alloc(std::max(F, 1)));
-  CK(ctx->board_pts2.alloc((size_t)B * Pn * 3));
+  CK(ctx->img_h.alloc(C)); CK(ctx->he_T.alloc(2)); CK(ctx->arm_T.alloc(std::max(F, 1)));
   // solver buffers
   {
     // static frame -> CTA map (bit-reproducible partial sums): the smallest grid that keeps every CTA at ceil(F / resident CTAs) frames
@@ -513,7 +519,8 @@ int setup_problem(mcba_ctx* ctx, const mcba_problem_desc* desc, int64_t N, int V
   CK(ctx->x.alloc(nn)); CK(ctx->x_new.alloc(nn)); CK(ctx->sinv.alloc(nn)); CK(ctx->d.alloc(nn)); CK(ctx->gh.alloc(nn)); CK(ctx->gn.alloc(nn));
   CK(ctx->S.alloc((size_t)std::max(P.n_s, 1) * std::max(P.n_s, 1))); CK(ctx->rhs.alloc((size_t)std::max(P.n_s, 1)));
   CK(ctx->Linv.alloc((size_t)((std::max(P.n_s, 1) + CHOL_NB - 1) / CHOL_NB) * CHOL_NB * CHOL_NB));
-  CK(ctx->red.alloc(RED_COUNT)); CK(cudaMemsetAsync(ctx->red.p, 0, sizeof(double) * RED_COUNT, ctx->stream));
+  CK(ctx->lin_cost.alloc(1)); CK(cudaMemsetAsync(ctx->lin_cost.p, 0, sizeof(double), ctx->stream));
+  CK(ctx->eval_cost.alloc(1)); CK(cudaMemsetAsync(ctx->eval_cost.p, 0, sizeof(double), ctx->stream));
   // persistent trust-region kernel (lm_kernel.cuh): grid, frame chunks of the Schur SYRK, partial-sum records, barrier words
   {
     const int F_free = P.motion_on ? F : 0;
@@ -537,14 +544,10 @@ int setup_problem(mcba_ctx* ctx, const mcba_problem_desc* desc, int64_t N, int V
   }
   CK(ctx->state.alloc(1));
   if (!keep_state) {     // a re-selection of the resident table (mcba_table_select) keeps the parameter state
-    CK(cudaMemsetAsync(ctx->cam_rt.p, 0, sizeof(double) * C * 6, ctx->stream));
-    CK(cudaMemsetAsync(ctx->board_rt.p, 0, sizeof(double) * B * 6, ctx->stream));
-    CK(cudaMemsetAsync(ctx->frame_rt.p, 0, sizeof(double) * std::max(F, 1) * fbs, ctx->stream));
-    CK(cudaMemsetAsync(ctx->intr.p, 0, sizeof(double) * C * P.kint, ctx->stream));
+    CK(cudaMemsetAsync(ctx->params.p, 0, sizeof(double) * ctx->layout.pts, ctx->stream));      // all but the uploaded board points
     // motion-model state: identity arm / hand-eye poses, unit image heights until mcba_set_rolling / mcba_set_hand_eye
     // (never read under static frames: no copies, no extra synchronisation on the BASELINE path)
     if (P.motion != MOTION_STATIC) {
-      CK(cudaMemsetAsync(ctx->he_rt.p, 0, sizeof(double) * 12, ctx->stream));
       std::vector<double> ones((size_t)C, 1.0);
       CK(cudaMemcpyAsync(ctx->img_h.p, ones.data(), sizeof(double) * C, cudaMemcpyHostToDevice, ctx->stream));
       PoseT id{}; id.R[0] = id.R[4] = id.R[8] = 1.0;
@@ -556,11 +559,10 @@ int setup_problem(mcba_ctx* ctx, const mcba_problem_desc* desc, int64_t N, int V
 
   P.obs = ctx->obs.p; P.pid = ctx->pid.p; P.orig = ctx->orig.p;
   P.view_start = ctx->view_start.p; P.view_cam = ctx->view_cam.p; P.view_frame = ctx->view_frame.p; P.view_board = ctx->view_board.p;
-  P.frame_view_start = ctx->frame_view_start.p; P.cam_view_start = ctx->cam_view_start.p; P.cam_view_list = ctx->cam_view_list.p;
-  P.board_pts = ctx->board_pts.p;
-  P.cam_rt = ctx->cam_rt.p; P.board_rt = ctx->board_rt.p; P.frame_rt = ctx->frame_rt.p; P.intr = ctx->intr.p;
+  P.frame_view_start = ctx->frame_view_start.p;
+  set_state_pointers(P, ctx->params.p, ctx->layout);
   P.cam_T = ctx->cam_T.p; P.frame_T = ctx->frame_T.p; P.board_T = ctx->board_T.p;
-  P.img_h = ctx->img_h.p; P.he_rt = ctx->he_rt.p; P.he_T = ctx->he_T.p; P.arm_T = ctx->arm_T.p;
+  P.img_h = ctx->img_h.p; P.he_T = ctx->he_T.p; P.arm_T = ctx->arm_T.p;
   return MCBA_OK;
 }
 // MCBA_PROF=1: host wall clock at checkpoints of the upload path, on stderr (no synchronisation is added: it times what the host waits for)
@@ -586,15 +588,15 @@ int pack_dense(mcba_ctx* ctx, const mcba_problem_desc* desc, const uint8_t* d_ma
   const int C = desc->C, F = desc->F, B = desc->B, Pn = desc->P;
   const int nv = C * F * B;
   cudaStream_t s = ctx->stream;
-  CK(ctx->scan.alloc((size_t)4 * (nv + 1)));
-  int* cnt_can = ctx->scan.p; int* cnt_fm = cnt_can + (nv + 1); int* flag_can = cnt_fm + (nv + 1); int* flag_fm = flag_can + (nv + 1);
+  CK(ctx->scan.alloc((size_t)3 * (nv + 1)));
+  int* cnt_can = ctx->scan.p; int* cnt_fm = cnt_can + (nv + 1); int* flag_fm = cnt_fm + (nv + 1);
   int totals[2] = {0, 0};
   UploadClock clk(ctx->profiling);
   if (nv > 0) {
-    k_pack_count<<<(unsigned)(((size_t)nv * 32 + 255) / 256), 256, 0, s>>>(d_mask, d_view_valid, C, F, B, Pn, cnt_can, cnt_fm, flag_can, flag_fm); CKL();
-    k_scan_exclusive<<<4, 1024, 0, s>>>(cnt_can, nv, nv + 1); CKL();      // cnt_can | cnt_fm | flag_can | flag_fm
+    k_pack_count<<<(unsigned)(((size_t)nv * 32 + 255) / 256), 256, 0, s>>>(d_mask, d_view_valid, C, F, B, Pn, cnt_can, cnt_fm, flag_fm); CKL();
+    k_scan_exclusive<<<3, 1024, 0, s>>>(cnt_can, nv, nv + 1); CKL();      // cnt_can | cnt_fm | flag_fm
     CK(cudaMemcpyAsync(&totals[0], cnt_can + nv, sizeof(int), cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(&totals[1], flag_can + nv, sizeof(int), cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(&totals[1], flag_fm + nv, sizeof(int), cudaMemcpyDeviceToHost, s));
     clk.mark("pack: count/scan/d2h issued");
     CK(cudaStreamSynchronize(s));
     clk.mark("pack: totals on the host");
@@ -602,17 +604,16 @@ int pack_dense(mcba_ctx* ctx, const mcba_problem_desc* desc, const uint8_t* d_ma
   const int64_t N = totals[0]; const int V = totals[1];
   CK(ctx->obs.alloc((size_t)std::max<int64_t>(N, 1))); CK(ctx->pid.alloc((size_t)std::max<int64_t>(N, 1))); CK(ctx->orig.alloc((size_t)std::max<int64_t>(N, 1)));
   CK(ctx->view_start.alloc((size_t)V + 1)); CK(ctx->view_cam.alloc((size_t)std::max(V, 1))); CK(ctx->view_frame.alloc((size_t)std::max(V, 1))); CK(ctx->view_board.alloc((size_t)std::max(V, 1)));
-  CK(ctx->frame_view_start.alloc((size_t)F + 1)); CK(ctx->cam_view_start.alloc((size_t)C + 1)); CK(ctx->cam_view_list.alloc((size_t)std::max(V, 1)));
+  CK(ctx->frame_view_start.alloc((size_t)F + 1));
   if (points_ready) CK(cudaStreamWaitEvent(s, points_ready, 0));
   if (nv > 0) {
     PackOut o{ctx->obs.p, ctx->pid.p, ctx->orig.p, ctx->view_start.p, ctx->view_cam.p, ctx->view_frame.p, ctx->view_board.p,
-              ctx->frame_view_start.p, ctx->cam_view_start.p, ctx->cam_view_list.p};
+              ctx->frame_view_start.p};
     const unsigned blocks = (unsigned)(((size_t)nv * 32 + 255) / 256);
-    if (points_f32) { k_pack_scatter<float2><<<blocks, 256, 0, s>>>(d_mask, (const float2*)ctx->dense_pts32.p, C, F, B, Pn, cnt_can, cnt_fm, flag_can, flag_fm, o); CKL(); }
-    else { k_pack_scatter<double2><<<blocks, 256, 0, s>>>(d_mask, (const double2*)ctx->dense_pts.p, C, F, B, Pn, cnt_can, cnt_fm, flag_can, flag_fm, o); CKL(); }
+    if (points_f32) { k_pack_scatter<float2><<<blocks, 256, 0, s>>>(d_mask, (const float2*)ctx->dense_pts32.p, C, F, B, Pn, cnt_can, cnt_fm, flag_fm, o); CKL(); }
+    else { k_pack_scatter<double2><<<blocks, 256, 0, s>>>(d_mask, (const double2*)ctx->dense_pts.p, C, F, B, Pn, cnt_can, cnt_fm, flag_fm, o); CKL(); }
   } else {
     CK(cudaMemsetAsync(ctx->view_start.p, 0, sizeof(int), s)); CK(cudaMemsetAsync(ctx->frame_view_start.p, 0, sizeof(int) * (F + 1), s));
-    CK(cudaMemsetAsync(ctx->cam_view_start.p, 0, sizeof(int) * (C + 1), s));
   }
   clk.mark("pack: scatter issued");
   { int r = setup_problem(ctx, desc, N, V, keep_state); if (r) return r; }
@@ -653,11 +654,11 @@ int mcba_create(int device, mcba_ctx** out) {
   ctx->stream = ctx->own_stream;
   { const char* e = getenv("MCBA_GRAPH"); if (e && std::string(e) == "0") ctx->use_graph = false; }
   { const char* e = getenv("MCBA_PROF"); if (e && std::string(e) == "1") { ctx->profiling = true; ctx->use_graph = false; } }
-#define LIN_ATTR(MODEL) \
-  cudaFuncSetAttribute(k_linearize<MODEL, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024); \
-  cudaFuncSetAttribute(k_linearize<MODEL, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
-  LIN_ATTR(MODEL_STANDARD) LIN_ATTR(MODEL_RATIONAL) LIN_ATTR(MODEL_THIN_PRISM) LIN_ATTR(MODEL_FISHEYE) LIN_ATTR(MODEL_TILTED)
-#undef LIN_ATTR
+  for (int model = MODEL_STANDARD; model <= MODEL_TILTED; model++)
+    for (bool roll : {false, true})
+      with_model(model, roll, [](auto M, auto R) {
+        cudaFuncSetAttribute(k_linearize<decltype(M)::value, decltype(R)::value>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
+      });
   cudaFuncSetAttribute(k_reduce_shared<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
   cudaFuncSetAttribute(k_reduce_shared<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
   cudaFuncSetAttribute(k_lm<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
@@ -791,21 +792,15 @@ int mcba_upload(mcba_ctx* ctx, const mcba_problem_desc* desc, const int32_t* cam
     for (int f = 0; f < F; f++) cnt[(size_t)f + 1] += cnt[f];
     fvs = cnt;
   }
-  std::vector<int> cvs((size_t)C + 1, 0), cvl((size_t)V);
-  {
-    for (int v = 0; v < V; v++) cvs[(size_t)vcam[v] + 1]++;
-    for (int c = 0; c < C; c++) cvs[(size_t)c + 1] += cvs[c];
-    std::vector<int> cur(cvs.begin(), cvs.end() - 1);
-    for (int v = 0; v < V; v++) cvl[(size_t)cur[vcam[v]]++] = v;
-  }
 
 #define UP(buf, vec) do { CK(ctx->buf.alloc((vec).size())); if (!(vec).empty()) CK(cudaMemcpyAsync(ctx->buf.p, (vec).data(), (vec).size() * sizeof((vec)[0]), cudaMemcpyHostToDevice, ctx->stream)); } while (0)
   UP(obs, h_obs); UP(pid, h_pid); UP(orig, order);
   UP(view_start, vstart); UP(view_cam, vcam); UP(view_frame, vframe); UP(view_board, vboard);
-  UP(frame_view_start, fvs); UP(cam_view_start, cvs); UP(cam_view_list, cvl);
+  UP(frame_view_start, fvs);
 #undef UP
-  CK(ctx->board_pts.alloc((size_t)B * Pn * 3));
-  CK(cudaMemcpyAsync(ctx->board_pts.p, board_points, sizeof(double) * (size_t)B * Pn * 3, cudaMemcpyHostToDevice, ctx->stream));
+  double* bpts = nullptr;
+  { int r = alloc_state(ctx, desc, &bpts); if (r) return r; }
+  CK(cudaMemcpyAsync(bpts, board_points, sizeof(double) * (size_t)B * Pn * 3, cudaMemcpyHostToDevice, ctx->stream));
   { int r = setup_problem(ctx, desc, N, V); if (r) return r; }
   CK(cudaStreamSynchronize(ctx->stream));    // host staging vectors go out of scope
   ctx->uploaded = true;
@@ -828,8 +823,9 @@ int upload_dense_any(mcba_ctx* ctx, const mcba_problem_desc* desc, const uint8_t
   CK(ctx->dense_mask.alloc(std::max<size_t>(dense, 1)));
   if (points_f32) CK(ctx->dense_pts32.alloc(std::max<size_t>(dense, 1))); else CK(ctx->dense_pts.alloc(std::max<size_t>(dense, 1)));
   CK(ctx->view_valid.alloc(std::max<size_t>((size_t)nv, 1)));
-  CK(ctx->scan.alloc((size_t)4 * (nv + 1)));
-  CK(ctx->board_pts.alloc((size_t)B * Pn * 3));
+  CK(ctx->scan.alloc((size_t)3 * (nv + 1)));
+  double* bpts = nullptr;
+  { int r = alloc_state(ctx, desc, &bpts); if (r) return r; }
   cudaEvent_t ready = nullptr;
   UploadClock clk(ctx->profiling);
   if (dense) {
@@ -839,7 +835,7 @@ int upload_dense_any(mcba_ctx* ctx, const mcba_problem_desc* desc, const uint8_t
     if (view_valid) CK(cudaMemcpyAsync(ctx->view_valid.p, view_valid, (size_t)nv, cudaMemcpyHostToDevice, s));
     // the small copies from pageable memory go BEFORE the table: such a copy returns when it is done, and behind 100 MB on the copy engine
     // it would hold the host back until the table has crossed the link -- with it the count / scan kernels that should run beside it
-    CK(cudaMemcpyAsync(ctx->board_pts.p, board_points, sizeof(double) * (size_t)B * Pn * 3, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(bpts, board_points, sizeof(double) * (size_t)B * Pn * 3, cudaMemcpyHostToDevice, s));
     if (!ctx->copy_stream) { CK(cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking)); CK(cudaEventCreateWithFlags(&ctx->copy_done, cudaEventDisableTiming)); CK(cudaEventCreateWithFlags(&ctx->copy_go, cudaEventDisableTiming)); }
     CK(cudaEventRecord(ctx->copy_go, s));                          // work queued on `s` before this call may still read dense_pts
     CK(cudaStreamWaitEvent(ctx->copy_stream, ctx->copy_go, 0));
@@ -849,7 +845,7 @@ int upload_dense_any(mcba_ctx* ctx, const mcba_problem_desc* desc, const uint8_t
     ready = ctx->copy_done;
     clk.mark("upload: copies issued");
   } else {
-    CK(cudaMemcpyAsync(ctx->board_pts.p, board_points, sizeof(double) * (size_t)B * Pn * 3, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(bpts, board_points, sizeof(double) * (size_t)B * Pn * 3, cudaMemcpyHostToDevice, s));
   }
   ctx->table = false; ctx->table_selected = -1; ctx->errors_current = false;
   return pack_dense(ctx, desc, ctx->dense_mask.p, false, n_corners, view_valid ? ctx->view_valid.p : nullptr, ready, points_f32);
@@ -883,8 +879,9 @@ int table_begin(mcba_ctx* ctx, const mcba_problem_desc* desc, const double* boar
   const size_t dense = (size_t)desc->C * desc->F * desc->B * desc->P;
   CK(ctx->valid_mask.alloc(std::max<size_t>(dense, 1))); CK(ctx->inlier_mask.alloc(std::max<size_t>(dense, 1)));
   CK(ctx->dense_pts.alloc(std::max<size_t>(dense, 1)));
-  CK(ctx->board_pts.alloc((size_t)desc->B * desc->P * 3));
-  CK(cudaMemcpyAsync(ctx->board_pts.p, board_points, sizeof(double) * (size_t)desc->B * desc->P * 3, cudaMemcpyHostToDevice, ctx->stream));
+  double* bpts = nullptr;
+  { int r = alloc_state(ctx, desc, &bpts); if (r) return r; }
+  CK(cudaMemcpyAsync(bpts, board_points, sizeof(double) * (size_t)desc->B * desc->P * 3, cudaMemcpyHostToDevice, ctx->stream));
   ctx->table = false; ctx->table_selected = -1; ctx->errors_current = false;
   *dense_out = dense;
   return MCBA_OK;
@@ -969,6 +966,62 @@ int mcba_table_from_detections(mcba_ctx* ctx, const mcba_problem_desc* desc, con
   return table_finish(ctx, desc, dense, n_valid);
 }
 
+namespace {
+
+// The caller's detection lists: list w = (c*F+f)*B+b of the C*F*B views holds point ids det_ids[det_start[w]:det_start[w+1]] in [0, P) and
+// their pixel corners det_xy (a CSR layout); the boards' id grids are at most 64 x 64.
+int check_detections(mcba_ctx* ctx, const mcba_problem_desc* desc, const int64_t* det_start, const int32_t* det_ids, const double* det_xy,
+                     const int32_t* board_grid) {
+  const int nv = desc->C * desc->F * desc->B;
+  const int64_t total = det_start[nv];
+  REQUIRE(det_start[0] == 0 && total >= 0 && total < ((int64_t)1 << 31), MCBA_ERR_ARG, "bad detection offsets");
+  REQUIRE(total == 0 || (det_ids && det_xy), MCBA_ERR_ARG, "null detection arrays");
+  for (int w = 0; w < nv; w++) REQUIRE(det_start[w + 1] >= det_start[w], MCBA_ERR_ARG, "detection offsets are not a monotone CSR over C*F*B lists");
+  for (int64_t i = 0; i < total; i++) REQUIRE(det_ids[i] >= 0 && det_ids[i] < desc->P, MCBA_ERR_ARG, "detection id outside [0, P)");
+  for (int b = 0; b < desc->B; b++)
+    REQUIRE(board_grid[5 * b] > 0 && board_grid[5 * b + 1] > 0 && board_grid[5 * b + 2] > 0 && board_grid[5 * b] <= 64 && board_grid[5 * b + 1] <= 64,
+            MCBA_ERR_UNSUPPORTED, "id grids are limited to 64 x 64 (bit masks of the occupied rows / columns)");
+  return MCBA_OK;
+}
+
+// detection lists in that layout, the id grids and the board points -> ctx->pnp, with room for the outputs of k_pnp_views
+int stage_detections(mcba_ctx* ctx, const mcba_problem_desc* desc, const int64_t* det_start, const int32_t* det_ids, const double* det_xy,
+                     const int32_t* board_grid, const double* board_points) {
+  const int nv = desc->C * desc->F * desc->B, B = desc->B, Pn = desc->P;
+  const int64_t total = det_start[nv];
+  cudaStream_t s = ctx->stream;
+  auto& pb = ctx->pnp;
+  const size_t tot = (size_t)std::max<int64_t>(total, 1);
+  CK(pb.start.alloc((size_t)nv + 1)); CK(pb.ids.alloc(tot)); CK(pb.xy.alloc(tot)); CK(pb.und.alloc(tot)); CK(pb.grid.alloc((size_t)B * 5));
+  CK(pb.bp.alloc((size_t)B * Pn * 3)); CK(pb.pose.alloc((size_t)nv * 16)); CK(pb.err.alloc(nv)); CK(pb.n.alloc(nv)); CK(pb.ok.alloc(nv));
+  CK(cudaMemcpyAsync(pb.start.p, det_start, sizeof(int64_t) * ((size_t)nv + 1), cudaMemcpyHostToDevice, s));
+  if (total) {
+    CK(cudaMemcpyAsync(pb.ids.p, det_ids, sizeof(int32_t) * (size_t)total, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(pb.xy.p, det_xy, sizeof(double2) * (size_t)total, cudaMemcpyHostToDevice, s));
+  }
+  CK(cudaMemcpyAsync(pb.grid.p, board_grid, sizeof(int32_t) * (size_t)B * 5, cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(pb.bp.p, board_points, sizeof(double) * (size_t)B * Pn * 3, cudaMemcpyHostToDevice, s));
+  return MCBA_OK;
+}
+
+// k_pnp_views over the staged lists: one warp per list, poses under the intrinsics intr [C][kint] (device) of camera model `model`
+int launch_pnp(mcba_ctx* ctx, const mcba_problem_desc* desc, int model, int kint, const double* intr) {
+  auto& pb = ctx->pnp;
+  PnpArgs a{};
+  a.C = desc->C; a.F = desc->F; a.B = desc->B; a.P = desc->P; a.model = model; a.kint = kint; a.nv = desc->C * desc->F * desc->B;
+  a.det_start = pb.start.p; a.det_ids = pb.ids.p; a.det_xy = pb.xy.p; a.board_pts = pb.bp.p; a.intr = intr; a.grid = pb.grid.p;
+  a.und = pb.und.p; a.poses = pb.pose.p; a.err = pb.err.p; a.npts = pb.n.p; a.valid = pb.ok.p; a.max_iters = 50;
+  const int blocks = (a.nv + PNP_WARPS - 1) / PNP_WARPS;
+  with_model(model, false, [&](auto M, auto) {
+    constexpr int MODEL = decltype(M)::value;
+    k_pnp_views<MODEL><<<blocks, PNP_WARPS * 32, 0, ctx->stream>>>(a);
+  });
+  CKL();
+  return MCBA_OK;
+}
+
+}  // namespace
+
 // Batched board-pose initialisation (pnp_kernels.cuh): one warp per detection list.  Independent of the uploaded problem.
 int mcba_pnp_views(mcba_ctx* ctx, const mcba_problem_desc* desc, const int64_t* det_start, const int32_t* det_ids, const double* det_xy,
                    const double* board_points, const double* intrinsics, const int32_t* board_grid,
@@ -979,47 +1032,18 @@ int mcba_pnp_views(mcba_ctx* ctx, const mcba_problem_desc* desc, const int64_t* 
   REQUIRE(det_start && board_points && intrinsics && board_grid && poses && errors && num_points && valid, MCBA_ERR_ARG, "null argument");
   const int nv = desc->C * desc->F * desc->B;
   if (nv == 0) return MCBA_OK;
-  const int64_t total = det_start[nv];
-  REQUIRE(det_start[0] == 0 && total >= 0 && total < ((int64_t)1 << 31), MCBA_ERR_ARG, "bad detection offsets");
-  REQUIRE(total == 0 || (det_ids && det_xy), MCBA_ERR_ARG, "null detection arrays");
-  for (int w = 0; w < nv; w++) REQUIRE(det_start[w + 1] >= det_start[w], MCBA_ERR_ARG, "detection offsets are not a monotone CSR over C*F*B lists");
-  for (int64_t i = 0; i < total; i++) REQUIRE(det_ids[i] >= 0 && det_ids[i] < desc->P, MCBA_ERR_ARG, "detection id outside [0, P)");
-  for (int b = 0; b < desc->B; b++)
-    REQUIRE(board_grid[5 * b] > 0 && board_grid[5 * b + 1] > 0 && board_grid[5 * b + 2] > 0 && board_grid[5 * b] <= 64 && board_grid[5 * b + 1] <= 64,
-            MCBA_ERR_UNSUPPORTED, "id grids are limited to 64 x 64 (bit masks of the occupied rows / columns)");
+  { int r = check_detections(ctx, desc, det_start, det_ids, det_xy, board_grid); if (r) return r; }
   const int kint = 5 + model_nd(desc->model);
   cudaStream_t s = ctx->stream;
-  auto& d_start = ctx->pnp.start; auto& d_ids = ctx->pnp.ids; auto& d_grid = ctx->pnp.grid; auto& d_n = ctx->pnp.n; auto& d_xy = ctx->pnp.xy; auto& d_und = ctx->pnp.und;
-  auto& d_bp = ctx->pnp.bp; auto& d_in = ctx->pnp.in; auto& d_pose = ctx->pnp.pose; auto& d_err = ctx->pnp.err; auto& d_ok = ctx->pnp.ok;
-  const size_t tot = (size_t)std::max<int64_t>(total, 1);
-  CK(d_start.alloc((size_t)nv + 1)); CK(d_ids.alloc(tot)); CK(d_xy.alloc(tot)); CK(d_und.alloc(tot)); CK(d_grid.alloc((size_t)desc->B * 5));
-  CK(d_bp.alloc((size_t)desc->B * desc->P * 3)); CK(d_in.alloc((size_t)desc->C * kint));
-  CK(d_pose.alloc((size_t)nv * 16)); CK(d_err.alloc(nv)); CK(d_n.alloc(nv)); CK(d_ok.alloc(nv));
-  CK(cudaMemcpyAsync(d_start.p, det_start, sizeof(int64_t) * ((size_t)nv + 1), cudaMemcpyHostToDevice, s));
-  if (total) {
-    CK(cudaMemcpyAsync(d_ids.p, det_ids, sizeof(int32_t) * (size_t)total, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(d_xy.p, det_xy, sizeof(double2) * (size_t)total, cudaMemcpyHostToDevice, s));
-  }
-  CK(cudaMemcpyAsync(d_grid.p, board_grid, sizeof(int32_t) * (size_t)desc->B * 5, cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(d_bp.p, board_points, sizeof(double) * (size_t)desc->B * desc->P * 3, cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(d_in.p, intrinsics, sizeof(double) * (size_t)desc->C * kint, cudaMemcpyHostToDevice, s));
-  PnpArgs a{};
-  a.C = desc->C; a.F = desc->F; a.B = desc->B; a.P = desc->P; a.model = desc->model; a.kint = kint; a.nv = nv;
-  a.det_start = d_start.p; a.det_ids = d_ids.p; a.det_xy = d_xy.p; a.board_pts = d_bp.p; a.intr = d_in.p; a.grid = d_grid.p;
-  a.und = d_und.p; a.poses = d_pose.p; a.err = d_err.p; a.npts = d_n.p; a.valid = d_ok.p; a.max_iters = 50;
-  const int blocks = (nv + PNP_WARPS - 1) / PNP_WARPS;
-  switch (desc->model) {
-    case MODEL_STANDARD: k_pnp_views<MODEL_STANDARD><<<blocks, PNP_WARPS * 32, 0, s>>>(a); break;
-    case MODEL_RATIONAL: k_pnp_views<MODEL_RATIONAL><<<blocks, PNP_WARPS * 32, 0, s>>>(a); break;
-    case MODEL_THIN_PRISM: k_pnp_views<MODEL_THIN_PRISM><<<blocks, PNP_WARPS * 32, 0, s>>>(a); break;
-    case MODEL_TILTED: k_pnp_views<MODEL_TILTED><<<blocks, PNP_WARPS * 32, 0, s>>>(a); break;
-    default: k_pnp_views<MODEL_FISHEYE><<<blocks, PNP_WARPS * 32, 0, s>>>(a); break;
-  }
-  CKL();
-  CK(cudaMemcpyAsync(poses, d_pose.p, sizeof(double) * 16 * (size_t)nv, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(errors, d_err.p, sizeof(double) * (size_t)nv, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(num_points, d_n.p, sizeof(int32_t) * (size_t)nv, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(valid, d_ok.p, (size_t)nv, cudaMemcpyDeviceToHost, s));
+  auto& pb = ctx->pnp;
+  { int r = stage_detections(ctx, desc, det_start, det_ids, det_xy, board_grid, board_points); if (r) return r; }
+  CK(pb.in.alloc((size_t)desc->C * kint));
+  CK(cudaMemcpyAsync(pb.in.p, intrinsics, sizeof(double) * (size_t)desc->C * kint, cudaMemcpyHostToDevice, s));
+  { int r = launch_pnp(ctx, desc, desc->model, kint, pb.in.p); if (r) return r; }
+  CK(cudaMemcpyAsync(poses, pb.pose.p, sizeof(double) * 16 * (size_t)nv, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(errors, pb.err.p, sizeof(double) * (size_t)nv, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(num_points, pb.n.p, sizeof(int32_t) * (size_t)nv, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(valid, pb.ok.p, (size_t)nv, cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
   return MCBA_OK;
 }
@@ -1036,14 +1060,7 @@ int mcba_intrinsic_init(mcba_ctx* ctx, const mcba_problem_desc* desc, const int6
   REQUIRE(desc->model != MODEL_FISHEYE, MCBA_ERR_UNSUPPORTED, "the intrinsic initialisation is for the pinhole camera models");
   const int C = desc->C, F = desc->F, B = desc->B, Pn = desc->P, nv = C * F * B;
   const int kint = 5 + model_nd(desc->model);
-  const int64_t total = det_start[nv];
-  REQUIRE(det_start[0] == 0 && total >= 0 && total < ((int64_t)1 << 31), MCBA_ERR_ARG, "bad detection offsets");
-  REQUIRE(total == 0 || (det_ids && det_xy), MCBA_ERR_ARG, "null detection arrays");
-  for (int w = 0; w < nv; w++) REQUIRE(det_start[w + 1] >= det_start[w], MCBA_ERR_ARG, "detection offsets are not a monotone CSR over C*F*B lists");
-  for (int64_t i = 0; i < total; i++) REQUIRE(det_ids[i] >= 0 && det_ids[i] < Pn, MCBA_ERR_ARG, "detection id outside [0, P)");
-  for (int b = 0; b < B; b++)
-    REQUIRE(board_grid[5 * b] > 0 && board_grid[5 * b + 1] > 0 && board_grid[5 * b + 2] > 0 && board_grid[5 * b] <= 64 && board_grid[5 * b + 1] <= 64,
-            MCBA_ERR_UNSUPPORTED, "id grids are limited to 64 x 64 (bit masks of the occupied rows / columns)");
+  { int r = check_detections(ctx, desc, det_start, det_ids, det_xy, board_grid); if (r) return r; }
   for (int c = 0; c < C; c++) REQUIRE(image_sizes[2 * c] > 0 && image_sizes[2 * c + 1] > 0, MCBA_ERR_ARG, "image sizes must be positive");
   // OpenCV estimates an initial camera matrix only for planar targets (all object points at z = 0)
   for (size_t i = 0; i < (size_t)B * Pn; i++)
@@ -1065,21 +1082,11 @@ int mcba_intrinsic_init(mcba_ctx* ctx, const mcba_problem_desc* desc, const int6
     start[(size_t)w + 1] = (int64_t)ids.size();
   }
   const int n_used = (int)used.size();
-  const int64_t kept = start[nv];
   cudaStream_t s = ctx->stream;
   auto& pb = ctx->pnp; auto& ib = ctx->intrinsic;
-  const size_t tot = (size_t)std::max<int64_t>(kept, 1);
-  CK(pb.start.alloc((size_t)nv + 1)); CK(pb.ids.alloc(tot)); CK(pb.xy.alloc(tot)); CK(pb.und.alloc(tot)); CK(pb.grid.alloc((size_t)B * 5));
-  CK(pb.bp.alloc((size_t)B * Pn * 3)); CK(pb.pose.alloc((size_t)nv * 16)); CK(pb.err.alloc(nv)); CK(pb.n.alloc(nv)); CK(pb.ok.alloc(nv));
+  { int r = stage_detections(ctx, desc, start.data(), ids.data(), xy.data(), board_grid, board_points); if (r) return r; }
   CK(ib.used.alloc((size_t)std::max(n_used, 1))); CK(ib.cam_start.alloc((size_t)C + 1)); CK(ib.size.alloc((size_t)C * 2));
   CK(ib.H.alloc((size_t)std::max(n_used, 1) * 9)); CK(ib.hok.alloc((size_t)std::max(n_used, 1))); CK(ib.k0.alloc((size_t)C * kint));
-  CK(cudaMemcpyAsync(pb.start.p, start.data(), sizeof(int64_t) * start.size(), cudaMemcpyHostToDevice, s));
-  if (kept) {
-    CK(cudaMemcpyAsync(pb.ids.p, ids.data(), sizeof(int32_t) * ids.size(), cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(pb.xy.p, xy.data(), sizeof(double) * xy.size(), cudaMemcpyHostToDevice, s));
-  }
-  CK(cudaMemcpyAsync(pb.grid.p, board_grid, sizeof(int32_t) * (size_t)B * 5, cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(pb.bp.p, board_points, sizeof(double) * (size_t)B * Pn * 3, cudaMemcpyHostToDevice, s));
   if (n_used) CK(cudaMemcpyAsync(ib.used.p, used.data(), sizeof(int32_t) * used.size(), cudaMemcpyHostToDevice, s));
   CK(cudaMemcpyAsync(ib.cam_start.p, cam_start.data(), sizeof(int32_t) * cam_start.size(), cudaMemcpyHostToDevice, s));
   CK(cudaMemcpyAsync(ib.size.p, image_sizes, sizeof(int32_t) * (size_t)C * 2, cudaMemcpyHostToDevice, s));
@@ -1094,11 +1101,7 @@ int mcba_intrinsic_init(mcba_ctx* ctx, const mcba_problem_desc* desc, const int6
   z.H = ib.H.p; z.ok = ib.hok.p; z.intr = ib.k0.p;
   k_zhang_init<<<C, ZHANG_THREADS, 0, s>>>(z); CKL();
   if (nv) {
-    PnpArgs a{};
-    a.C = C; a.F = F; a.B = B; a.P = Pn; a.model = MODEL_STANDARD; a.kint = kint; a.nv = nv;
-    a.det_start = pb.start.p; a.det_ids = pb.ids.p; a.det_xy = pb.xy.p; a.board_pts = pb.bp.p; a.intr = ib.k0.p; a.grid = pb.grid.p;
-    a.und = pb.und.p; a.poses = pb.pose.p; a.err = pb.err.p; a.npts = pb.n.p; a.valid = pb.ok.p; a.max_iters = 50;
-    k_pnp_views<MODEL_STANDARD><<<(nv + PNP_WARPS - 1) / PNP_WARPS, PNP_WARPS * 32, 0, s>>>(a); CKL();     // zero distortion: the pinhole K0
+    { int r = launch_pnp(ctx, desc, MODEL_STANDARD, kint, ib.k0.p); if (r) return r; }      // zero distortion: the pinhole K0
     CK(cudaMemcpyAsync(poses, pb.pose.p, sizeof(double) * 16 * (size_t)nv, cudaMemcpyDeviceToHost, s));
     CK(cudaMemcpyAsync(ok, pb.ok.p, (size_t)nv, cudaMemcpyDeviceToHost, s));
   }
@@ -1284,10 +1287,10 @@ int mcba_set_params(mcba_ctx* ctx, const double* cam_rt, const double* board_rt,
   const DeviceProblem& P = ctx->P;
   CK(cudaSetDevice(ctx->device));
   ctx->errors_current = false;
-  CK(cudaMemcpyAsync(ctx->cam_rt.p, cam_rt, sizeof(double) * P.C * 6, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(ctx->board_rt.p, board_rt, sizeof(double) * P.B * 6, cudaMemcpyHostToDevice, ctx->stream));
-  if (P.F && P.fb) CK(cudaMemcpyAsync(ctx->frame_rt.p, frame_rt, sizeof(double) * P.F * P.fb, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(ctx->intr.p, intrinsics, sizeof(double) * P.C * P.kint, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(P.cam_rt, cam_rt, sizeof(double) * P.C * 6, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(P.board_rt, board_rt, sizeof(double) * P.B * 6, cudaMemcpyHostToDevice, ctx->stream));
+  if (P.F && P.fb) CK(cudaMemcpyAsync(P.frame_rt, frame_rt, sizeof(double) * P.F * P.fb, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(P.intr, intrinsics, sizeof(double) * P.C * P.kint, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   return MCBA_OK;
 }
@@ -1304,7 +1307,7 @@ int mcba_set_state_matrices(mcba_ctx* ctx, const double* mats, const double* int
   ctx->errors_current = false;
   CK(ctx->pose_mats.alloc((size_t)np * 16));
   CK(cudaMemcpyAsync(ctx->pose_mats.p, mats, sizeof(double) * 16 * np, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(ctx->intr.p, intrinsics, sizeof(double) * P.C * P.kint, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(P.intr, intrinsics, sizeof(double) * P.C * P.kint, cudaMemcpyHostToDevice, ctx->stream));
   k_matrices_to_state<<<(np + 127) / 128, 128, 0, ctx->stream>>>(P.C, P.B, P.F, ctx->pose_mats.p, P.cam_rt, P.board_rt, P.frame_rt, P.fb); CKL();
   CK(cudaStreamSynchronize(ctx->stream));     // the host arrays are borrowed only for the call
   return MCBA_OK;
@@ -1323,7 +1326,7 @@ int mcba_get_state_matrices(mcba_ctx* ctx, double* mats, double* intrinsics) {
     k_state_to_matrices<<<(np + 127) / 128, 128, 0, ctx->stream>>>(P.C, P.B, P.F, P.cam_rt, P.board_rt, P.frame_rt, ctx->pose_mats.p, P.fb, derived); CKL();
     CK(cudaMemcpyAsync(mats, ctx->pose_mats.p, sizeof(double) * 16 * np, cudaMemcpyDeviceToHost, ctx->stream));
   }
-  if (intrinsics) CK(cudaMemcpyAsync(intrinsics, ctx->intr.p, sizeof(double) * P.C * P.kint, cudaMemcpyDeviceToHost, ctx->stream));
+  if (intrinsics) CK(cudaMemcpyAsync(intrinsics, P.intr, sizeof(double) * P.C * P.kint, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   return MCBA_OK;
 }
@@ -1410,10 +1413,10 @@ int mcba_get_params(mcba_ctx* ctx, double* cam_rt, double* board_rt, double* fra
   REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "mcba_upload has not been called");
   const DeviceProblem& P = ctx->P;
   CK(cudaSetDevice(ctx->device));
-  if (cam_rt) CK(cudaMemcpyAsync(cam_rt, ctx->cam_rt.p, sizeof(double) * P.C * 6, cudaMemcpyDeviceToHost, ctx->stream));
-  if (board_rt) CK(cudaMemcpyAsync(board_rt, ctx->board_rt.p, sizeof(double) * P.B * 6, cudaMemcpyDeviceToHost, ctx->stream));
-  if (frame_rt && P.F && P.fb) CK(cudaMemcpyAsync(frame_rt, ctx->frame_rt.p, sizeof(double) * P.F * P.fb, cudaMemcpyDeviceToHost, ctx->stream));
-  if (intrinsics) CK(cudaMemcpyAsync(intrinsics, ctx->intr.p, sizeof(double) * P.C * P.kint, cudaMemcpyDeviceToHost, ctx->stream));
+  if (cam_rt) CK(cudaMemcpyAsync(cam_rt, P.cam_rt, sizeof(double) * P.C * 6, cudaMemcpyDeviceToHost, ctx->stream));
+  if (board_rt) CK(cudaMemcpyAsync(board_rt, P.board_rt, sizeof(double) * P.B * 6, cudaMemcpyDeviceToHost, ctx->stream));
+  if (frame_rt && P.F && P.fb) CK(cudaMemcpyAsync(frame_rt, P.frame_rt, sizeof(double) * P.F * P.fb, cudaMemcpyDeviceToHost, ctx->stream));
+  if (intrinsics) CK(cudaMemcpyAsync(intrinsics, P.intr, sizeof(double) * P.C * P.kint, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   return MCBA_OK;
 }
@@ -1486,8 +1489,8 @@ int mcba_residuals(mcba_ctx* ctx, const double* x, double* r_out, double* cost) 
     CK(cudaStreamSynchronize(ctx->stream));
   }
   if (cost) {
-    int r = trial_cost(ctx, 0, 1.0, trial, RED_COSTNEW); if (r) return r;
-    CK(cudaMemcpyAsync(cost, ctx->red.p + RED_COSTNEW, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    int r = trial_cost(ctx, 0, 1.0, trial); if (r) return r;
+    CK(cudaMemcpyAsync(cost, ctx->eval_cost.p, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
   }
   return MCBA_OK;
@@ -1524,7 +1527,7 @@ int mcba_linearize(mcba_ctx* ctx, const double* x, double* JtJ, double* Jtr, dou
   if (F) CK(cudaMemcpyAsync(hHff.data(), ctx->Hff.p, sizeof(double) * hHff.size(), cudaMemcpyDeviceToHost, ctx->stream));
   if (F && n_s) CK(cudaMemcpyAsync(hW.data(), ctx->W.p, sizeof(double) * hW.size(), cudaMemcpyDeviceToHost, ctx->stream));
   double hcost = 0;
-  CK(cudaMemcpyAsync(&hcost, ctx->red.p + RED_COST, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(&hcost, ctx->lin_cost.p, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   const std::vector<int>& pm = ctx->perm;
   if (JtJ) {
@@ -1577,7 +1580,7 @@ int mcba_solve(mcba_ctx* ctx, const mcba_solve_opts* opts, mcba_solve_result* re
     if (ctx->world > 1) {       // one number: the host's collective is the simplest exchange (no solver state involved)
       ctx->err = "nothing to optimise on several ranks: sum mcba_residuals' cost on the host"; return MCBA_ERR_UNSUPPORTED;
     }
-    CK(cudaMemcpyAsync(&h.cost, ctx->red.p + RED_COST, sizeof(double), cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(&h.cost, ctx->lin_cost.p, sizeof(double), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
     result->initial_cost = h.cost; result->cost = h.cost; result->nfev = 1; result->njev = 1; result->status = 1;
     if (log && log_capacity > 0) { log[0] = mcba_log_row{0, 1, h.cost, NAN, NAN, 0.0}; result->n_log = 1; }

@@ -26,21 +26,8 @@ struct SolverState {
   double step2_s, xn2_s, agg;                // shared (replicated) parts of ||step||^2 and ||x||^2 of the pending trial; g_h^T A g_h
 };
 
-// slots of the cross-rank reduction scratch `red` (doubles). Entries marked F hold only the contribution of
-// this rank's frames and are summed (or maxed) over ranks; S entries are computed from replicated data.
-enum {
-  RED_GH2_F = 0, RED_XS2_F,                                     // k_scale, frame parts        (1 all-reduce, sum)
-  RED_GMAX_F,                                                    // k_scale                     (all-reduce, max)
-  RED_AGG, RED_AGN, RED_ANN, RED_DOTGN_F, RED_GN2_F,           // quadratic forms + dots      (1 all-reduce, sum)
-  RED_COSTNEW, RED_STEP2_F, RED_XN2_F,                          // trial step                  (1 all-reduce, sum)
-  RED_COST,                                                      // cost at the linearisation   (grouped with g_s)
-  RED_GH2_S, RED_XS2_S, RED_GMAX_S, RED_DOTGN_S, RED_GN2_S, RED_STEP2_S, RED_XN2_S,   // replicated (shared) parts: never reduced
-  RED_COUNT
-};
-
 // ---- NVLink peer-memory exchange of k_lm (lm_kernel.cuh LmPeer): layout of the per-rank buffers
 constexpr int PEER_MAX_WORLD = 16;
-constexpr int PEER_MAX_SEG = 6;
 constexpr int PEER_FLAG_STRIDE = 8;      // doubles (64 B) between flags
 
 __host__ __device__ inline size_t peer_flag_off(int world, int parity, int src) { return (size_t)(parity * world + src) * PEER_FLAG_STRIDE; }
@@ -63,21 +50,6 @@ __device__ __forceinline__ double block_sum(double v, double* sm) {
     for (int o = 16; o > 0; o >>= 1) r += __shfl_xor_sync(0xffffffffu, r, o);
   }
   return r;   // valid in thread 0
-}
-__device__ __forceinline__ double block_max(double v, double* sm) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
-  __syncthreads();
-  if (lane == 0) sm[w] = v;
-  __syncthreads();
-  double r = 0.0;
-  if (w == 0) {
-    r = lane < nw ? sm[lane] : 0.0;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) r = fmax(r, __shfl_xor_sync(0xffffffffu, r, o));
-  }
-  return r;
 }
 
 // ---- bulk asynchronous copies (the 1-D form of the Tensor Memory Accelerator, cp.async.bulk) with an mbarrier as completion signal:
@@ -115,13 +87,15 @@ __global__ void k_sum_partials(const double* part, int count, int stride, int no
 }
 
 // trf.py top of the outer loop: ||g||_inf, gtol / max_nfev exits, first-iteration cost and Delta.
-__device__ inline void begin_iteration(SolverState* st, const double* red) {
-  const double gh2 = red[RED_GH2_S] + red[RED_GH2_F];
+// Every sum below is split into its shared (_s) and frame (_f) part; the frame parts are summed over the ranks.
+__device__ inline void begin_iteration(SolverState* st, double gh2_s, double gh2_f, double gmax_s, double gmax_f, double xs2_s, double xs2_f,
+                                       double cost) {
+  const double gh2 = gh2_s + gh2_f;
   st->gh_norm = sqrt(gh2);
-  st->g_norm = fmax(red[RED_GMAX_S], red[RED_GMAX_F]);
+  st->g_norm = fmax(gmax_s, gmax_f);
   if (st->first_scale) {
-    st->cost = red[RED_COST];
-    double D0 = sqrt(red[RED_XS2_S] + red[RED_XS2_F]);
+    st->cost = cost;
+    double D0 = sqrt(xs2_s + xs2_f);
     st->Delta = (D0 == 0.0) ? 1.0 : D0;
     st->first_scale = 0;
   }
@@ -131,16 +105,14 @@ __device__ inline void begin_iteration(SolverState* st, const double* red) {
 
 // trf.py: reg_term = -ag_value / Delta^2 with ag_value = min over [0, Delta/||g_h||] of a t^2 + b t,
 // a = g_h^T A g_h, b = -||g_h||^2 (build_quadratic_1d / minimize_quadratic_1d).
-__device__ inline void reg_compute(SolverState* st, const double* red) {
-  const double a = red[RED_AGG];
+__device__ inline void reg_compute(SolverState* st, double a) {
   const double gh2 = st->gh_norm * st->gh_norm;
   const double b = -gh2;
   const double ub = st->Delta / st->gh_norm;
   // minimize a t^2 + b t on [0, ub]
-  double best_t = 0.0, best = 0.0;
-  { const double yv = a * ub * ub + b * ub; if (yv < best) { best = yv; best_t = ub; } }
-  if (a != 0.0) { const double ext = -0.5 * b / a; if (ext > 0.0 && ext < ub) { const double yv = a * ext * ext + b * ext; if (yv < best) { best = yv; best_t = ext; } } }
-  (void)best_t;
+  double best = 0.0;
+  { const double yv = a * ub * ub + b * ub; if (yv < best) best = yv; }
+  if (a != 0.0) { const double ext = -0.5 * b / a; if (ext > 0.0 && ext < ub) { const double yv = a * ext * ext + b * ext; if (yv < best) best = yv; } }
   double reg = -best / (st->Delta * st->Delta);
   if (!(reg > st->reg_floor)) reg = st->reg_floor;
   st->reg = reg;
@@ -155,13 +127,12 @@ constexpr int CHOL_NB = 32;              // panel width of the cooperative block
 
 // trf.py: S = qr([g_h, gn_h]); B_S = (J_h S)^T (J_h S); g_S = S^T g_h   -- expressed through Gram-Schmidt
 // coefficients so that no basis vectors are materialised: q1 = gh/n1, q2 = (gn - mu q1)/n2.
-__device__ inline void subspace_compute(SolverState* st, const double* red) {
+__device__ inline void subspace_compute(SolverState* st, double agg, double agn, double ann, double dot_s, double dot_f, double gn2_s, double gn2_f) {
   const double n1 = st->gh_norm;
-  const double dot = red[RED_DOTGN_S] + red[RED_DOTGN_F];
-  const double gn2 = red[RED_GN2_S] + red[RED_GN2_F];
+  const double dot = dot_s + dot_f;
+  const double gn2 = gn2_s + gn2_f;
   const double mu = dot / n1;
   double n2sq = gn2 - mu * mu;
-  const double agg = red[RED_AGG], agn = red[RED_AGN], ann = red[RED_ANN];
   st->n1 = n1; st->mu = mu;
   st->B11 = agg / (n1 * n1);
   st->gS1 = n1; st->gS2 = 0.0;
@@ -235,9 +206,8 @@ __device__ inline void tr_step_compute(SolverState* st) {
 }
 
 // trf.py inner loop after fun(x_new): actual reduction, update_tr_radius, check_termination (one thread)
-__device__ inline void accept_compute(SolverState* st, const double* red) {
+__device__ inline void accept_compute(SolverState* st, double cost_new, double step2_s, double step2_f, double xn2_s, double xn2_f) {
   st->nfev += 1;
-  const double cost_new = red[RED_COSTNEW];
   st->cost_new = cost_new;
   const double shn = st->step_h_norm;
   if (!isfinite(cost_new)) {            // trf.py: non-finite f_new -> shrink and retry
@@ -253,8 +223,8 @@ __device__ inline void accept_compute(SolverState* st, const double* red) {
   double Dn = st->Delta;
   if (ratio < 0.25) Dn = 0.25 * shn;
   else if (ratio > 0.75 && shn > 0.95 * st->Delta) Dn = 2.0 * st->Delta;
-  const double step_norm = sqrt(red[RED_STEP2_S] + red[RED_STEP2_F]);
-  const double x_norm = sqrt(red[RED_XN2_S] + red[RED_XN2_F]);
+  const double step_norm = sqrt(step2_s + step2_f);
+  const double x_norm = sqrt(xn2_s + xn2_f);
   st->step_norm = step_norm; st->x_norm = x_norm; st->actual_reduction = actual; st->ratio = ratio;
   const bool ft = (actual < st->ftol * st->cost) && (ratio > 0.25);
   const bool xt = step_norm < st->xtol * (st->xtol + x_norm);

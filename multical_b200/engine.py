@@ -146,16 +146,22 @@ class Engine:
     self._table_ready(d, model, n.value)
     return n.value
 
-  def table_from_detections(self, model, optimize_bits, dims, det_start, det_ids, det_xy, board_points):
-    """Build the table on the device from detection lists: list w = (c*F+f)*B+b holds point ids
-    det_ids[det_start[w]:det_start[w+1]] and their pixel corners det_xy (what tables.make_point_table consumes)."""
+  @staticmethod
+  def _detections(dims, det_start, det_ids, det_xy, board_points):
+    """Detection lists as the C ABI takes them: list w = (c*F+f)*B+b holds point ids det_ids[det_start[w]:det_start[w+1]] and their
+    pixel corners det_xy.  Returns (C, F, B, P), the offsets, ids, corners and board points as contiguous arrays."""
     Cn, F, B, P = (int(v) for v in dims)
     det_start = np.ascontiguousarray(det_start, dtype=np.int64)
     assert det_start.shape == (Cn * F * B + 1,), f"expected {Cn * F * B + 1} list offsets, got {det_start.shape}"
     det_ids = np.ascontiguousarray(det_ids, dtype=np.int32).reshape(-1)
     det_xy = nat.f64(det_xy).reshape(-1, 2)
     assert det_ids.size == det_xy.shape[0] == int(det_start[-1]), "detection arrays do not match the offsets"
-    bp = nat.f64(board_points).reshape(B, P, 3)
+    return (Cn, F, B, P), det_start, det_ids, det_xy, nat.f64(board_points).reshape(B, P, 3)
+
+  def table_from_detections(self, model, optimize_bits, dims, det_start, det_ids, det_xy, board_points):
+    """Build the table on the device from detection lists: list w = (c*F+f)*B+b holds point ids
+    det_ids[det_start[w]:det_start[w+1]] and their pixel corners det_xy (what tables.make_point_table consumes)."""
+    (Cn, F, B, P), det_start, det_ids, det_xy, bp = self._detections(dims, det_start, det_ids, det_xy, board_points)
     d = nat.ProblemDesc(Cn, F, B, P, nat.MODEL_IDS[model], int(optimize_bits), 0)
     n = C.c_int64()
     self._ck(self.lib.mcba_table_from_detections(self.h, C.byref(d), det_start.ctypes.data_as(C.POINTER(C.c_int64)),
@@ -166,14 +172,8 @@ class Engine:
   def pnp_views(self, model, dims, det_start, det_ids, det_xy, board_points, intrinsics, board_grid):
     """Batched board-pose initialisation (include/mcba.h mcba_pnp_views): list w = (c*F+f)*B+b of detected point ids and pixel
     corners -> (poses [C,F,B,4,4], reprojection RMS [C,F,B], corner counts [C,F,B], valid [C,F,B])."""
-    Cn, F, B, P = (int(v) for v in dims)
+    (Cn, F, B, P), det_start, det_ids, det_xy, bp = self._detections(dims, det_start, det_ids, det_xy, board_points)
     nv = Cn * F * B
-    det_start = np.ascontiguousarray(det_start, dtype=np.int64)
-    assert det_start.shape == (nv + 1,), f"expected {nv + 1} list offsets, got {det_start.shape}"
-    det_ids = np.ascontiguousarray(det_ids, dtype=np.int32).reshape(-1)
-    det_xy = nat.f64(det_xy).reshape(-1, 2)
-    assert det_ids.size == det_xy.shape[0] == int(det_start[-1]), "detection arrays do not match the offsets"
-    bp = nat.f64(board_points).reshape(B, P, 3)
     intr = nat.f64(intrinsics).reshape(Cn, 5 + nat.DIST_SIZES[model])
     grid = np.ascontiguousarray(board_grid, dtype=np.int32).reshape(B, 5)
     poses, err = np.zeros((max(nv, 1), 4, 4)), np.zeros(max(nv, 1))
@@ -188,14 +188,8 @@ class Engine:
     """Initialisation of single-camera intrinsic calibration (include/mcba.h mcba_intrinsic_init) for every camera at once: list
     w = (c*F+f)*B+b of detected point ids and pixel corners, view_use [C,F,B] the views of this round -> (K0 parameters [C, 5+nd] with
     zero distortion, initial board-wrt-camera poses [C,F,B,4,4], ok [C,F,B])."""
-    Cn, F, B, P = (int(v) for v in dims)
+    (Cn, F, B, P), det_start, det_ids, det_xy, bp = self._detections(dims, det_start, det_ids, det_xy, board_points)
     nv = Cn * F * B
-    det_start = np.ascontiguousarray(det_start, dtype=np.int64)
-    assert det_start.shape == (nv + 1,), f"expected {nv + 1} list offsets, got {det_start.shape}"
-    det_ids = np.ascontiguousarray(det_ids, dtype=np.int32).reshape(-1)
-    det_xy = nat.f64(det_xy).reshape(-1, 2)
-    assert det_ids.size == det_xy.shape[0] == int(det_start[-1]), "detection arrays do not match the offsets"
-    bp = nat.f64(board_points).reshape(B, P, 3)
     grid = np.ascontiguousarray(board_grid, dtype=np.int32).reshape(B, 5)
     sizes = np.ascontiguousarray(image_sizes, dtype=np.int32).reshape(Cn, 2)
     use = np.ascontiguousarray(view_use, dtype=np.uint8).reshape(nv)
