@@ -244,6 +244,26 @@ int  mcba_intrinsic_init(mcba_ctx* ctx, const mcba_problem_desc* desc, const int
                          const uint8_t* view_use, double* intrinsics, double* poses, uint8_t* ok);
 int  mcba_view_errors(mcba_ctx* ctx, double* sumsq, int64_t* count);
 
+/* -- pose-graph initialisation (tables.initialise_poses, tables.py:354-377) ---------------------------------------------------------
+ * Every call of align_transforms_robust (transform/matrix.py:140-153) that initialise_poses makes, batched: mean_robust of the relative
+ * poses (Ward clustering of their rtvecs, transform/common.py:6-19), the inlier test at 1.5 x the upper quartile of the errors over
+ * all rows, mean_robust again over the inliers.  The table is poses f64[C][F][B][4][4] and valid uint8[C][F][B] of make_pose_table.
+ * mcba_pose_pairs: estimate_transform (tables.py:149-174) for each (parent, child) of pairs int32[n_pairs][2].  axis 0: cameras, rows
+ *   (f, b) f-major, m1 = table[parent], m2 = table[child]; axis 2: boards of the inverted table (estimate_relative_poses_inv), rows (c, f)
+ *   c-major, m1 = inv(table[:, :, parent]), m2 = inv(table[:, :, child]).  Out: t f64[n_pairs][4][4], inliers uint8[n_pairs][rows]
+ *   (rows = F*B or C*F), n_inliers int32[n_pairs].
+ * mcba_pose_times: the rig poses (relative_between_inv per frame): rows (c, b) in np.nonzero order with cam_valid[c] & valid[c, f, b] &
+ *   board_valid[b]; m1 = inv(cam[c]), m2 = inv(table[c, f, b] inv(board[b])); times[f] = inv(t), or the identity with times_valid[f] = 0
+ *   for a frame without rows.
+ * mcba_pose_cluster: mean_robust's clustering alone.  Sets of 6-vectors vecs f64[N][6] (CSR offsets set_start int64[n_sets + 1]) ->
+ *   mask uint8[N] of each set's largest cluster.
+ * Non-finite poses or vectors fail with MCBA_ERR_NONFINITE.  None of these touches the uploaded problem. */
+int  mcba_pose_pairs(mcba_ctx* ctx, int32_t C, int32_t F, int32_t B, const double* poses, const uint8_t* valid, int32_t axis,
+                     const int32_t* pairs, int32_t n_pairs, double* t, uint8_t* inliers, int32_t* n_inliers);
+int  mcba_pose_times(mcba_ctx* ctx, int32_t C, int32_t F, int32_t B, const double* poses, const uint8_t* valid, const double* cam_poses,
+                     const uint8_t* cam_valid, const double* board_poses, const uint8_t* board_valid, double* times, uint8_t* times_valid);
+int  mcba_pose_cluster(mcba_ctx* ctx, int32_t n_sets, const int64_t* set_start, const double* vecs, uint8_t* mask);
+
 /* -- measurement hooks (bench.py): launch one kernel family on the context stream -------------- */
 enum { MCBA_BENCH_LINEARIZE = 0, MCBA_BENCH_RESIDUAL = 1, MCBA_BENCH_COST = 2,
        MCBA_BENCH_NO_PREPARE = 256 /* or-ed in: reuse the pose tables of the previous call (times the kernel alone) */ };

@@ -21,6 +21,7 @@
 #include "table_kernels.cuh"
 #include "pnp_kernels.cuh"
 #include "intrinsics_kernels.cuh"
+#include "pose_init_kernels.cuh"
 
 using namespace mcba;
 
@@ -137,6 +138,11 @@ struct mcba_ctx {
   struct IntrinsicBuffers {
     DevBuf<int32_t> used, cam_start, size; DevBuf<double> H, k0; DevBuf<uint8_t> hok;
   } intrinsic;
+  // pose-graph initialisation (mcba_pose_pairs / mcba_pose_times / mcba_pose_cluster): the table, the gathered rows, per-item results
+  struct PoseInitBuffers {
+    DevBuf<double> poses, cam, board, m1, m2, vecs, t; DevBuf<uint8_t> valid, mask, inl; DevBuf<PoseRow> rows;
+    DevBuf<int64_t> start; DevBuf<int32_t> items, n_inl; DevBuf<char> work;
+  } pinit;
 };
 
 #define CK(call)                                                                                   \
@@ -663,6 +669,7 @@ int mcba_create(int device, mcba_ctx** out) {
   cudaFuncSetAttribute(k_reduce_shared<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
   cudaFuncSetAttribute(k_lm<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
   cudaFuncSetAttribute(k_lm<12>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+  cudaFuncSetAttribute(k_pose_align<PI_SMALL_THREADS, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, PI_SMALL_MAX * PI_ROW_BYTES);
   *out = ctx;
   return MCBA_OK;
 }
@@ -1132,6 +1139,188 @@ int mcba_view_errors(mcba_ctx* ctx, double* sumsq, int64_t* count) {
   CK(cudaMemcpyAsync(sumsq, ds.p, sizeof(double) * nv, cudaMemcpyDeviceToHost, s));
   CK(cudaMemcpyAsync(count, dn.p, sizeof(int64_t) * nv, cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
+  return MCBA_OK;
+}
+
+namespace {
+
+bool all_finite(const double* p, size_t n) {
+  for (size_t i = 0; i < n; i++) if (!std::isfinite(p[i])) return false;
+  return true;
+}
+
+int check_pose_dims(mcba_ctx* ctx, int32_t C, int32_t F, int32_t B) {
+  REQUIRE(C > 0 && F > 0 && B > 0, MCBA_ERR_ARG, "bad pose table dimensions");
+  REQUIRE((int64_t)C * F * B < ((int64_t)1 << 31), MCBA_ERR_UNSUPPORTED, "more than 2^31 views");
+  return MCBA_OK;
+}
+
+// Uploads the pose table, gathers the rows of every item (start: CSR row offsets, one segment per item) and runs align_transforms_robust
+// on each (pose_init_kernels.cuh): items above PI_SMALL_MAX rows on the large-item kernel, the rest on the shared-memory one.  Leaves
+// t [items][4][4], n_inl [items] and inl [rows] on the device.  vecs (host, [rows][6]) selects the cluster-only mode instead of rows.
+int run_pose_align(mcba_ctx* ctx, int C, int F, int B, const double* poses, const uint8_t* valid, const double* cam, const double* board,
+                   const std::vector<PoseRow>& rows, const std::vector<int64_t>& start, const double* vecs) {
+  auto& pb = ctx->pinit;
+  cudaStream_t s = ctx->stream;
+  const int n_items = (int)start.size() - 1;
+  const int64_t n_rows = start.back();
+  PoseAlignArgs a{};
+  a.C = C; a.F = F; a.B = B; a.n_rows = n_rows;
+  const size_t nv = (size_t)C * F * B;
+  if (poses) {
+    CK(pb.poses.alloc(16 * nv)); CK(pb.valid.alloc(nv));
+    CK(cudaMemcpyAsync(pb.poses.p, poses, sizeof(double) * 16 * nv, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(pb.valid.p, valid, nv, cudaMemcpyHostToDevice, s));
+    a.poses = pb.poses.p; a.valid = pb.valid.p;
+  }
+  if (cam) {
+    CK(pb.cam.alloc(16 * (size_t)C)); CK(pb.board.alloc(16 * (size_t)B));
+    CK(cudaMemcpyAsync(pb.cam.p, cam, sizeof(double) * 16 * C, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(pb.board.p, board, sizeof(double) * 16 * B, cudaMemcpyHostToDevice, s));
+    a.cam = pb.cam.p; a.board = pb.board.p;
+  }
+  const size_t nr = (size_t)std::max<int64_t>(n_rows, 1);
+  CK(pb.start.alloc(start.size())); CK(pb.items.alloc((size_t)std::max(n_items, 1)));
+  CK(pb.t.alloc(16 * (size_t)std::max(n_items, 1))); CK(pb.n_inl.alloc((size_t)std::max(n_items, 1))); CK(pb.inl.alloc(nr));
+  CK(cudaMemcpyAsync(pb.start.p, start.data(), sizeof(int64_t) * start.size(), cudaMemcpyHostToDevice, s));
+  a.row_start = pb.start.p; a.t = pb.t.p; a.n_inl = pb.n_inl.p; a.inl = pb.inl.p;
+  if (vecs) {
+    CK(pb.vecs.alloc(6 * nr));
+    CK(cudaMemcpyAsync(pb.vecs.p, vecs, sizeof(double) * 6 * n_rows, cudaMemcpyHostToDevice, s));
+    a.vecs = pb.vecs.p;
+  } else if (n_rows) {
+    CK(pb.rows.alloc(nr)); CK(pb.m1.alloc(12 * nr)); CK(pb.m2.alloc(12 * nr)); CK(pb.mask.alloc(nr));
+    CK(cudaMemcpyAsync(pb.rows.p, rows.data(), sizeof(PoseRow) * n_rows, cudaMemcpyHostToDevice, s));
+    a.rows = pb.rows.p; a.m1 = pb.m1.p; a.m2 = pb.m2.p; a.mask = pb.mask.p;
+    const int grid = (int)std::min<int64_t>((n_rows + 255) / 256, 8 * (int64_t)ctx->num_sms);
+    k_pose_gather<<<grid, 256, 0, s>>>(a); CKL();
+  }
+  // items by size class; the large ones first in the list
+  std::vector<int32_t> order;
+  int64_t large_rows = 0; int small_max = 0;
+  for (int i = 0; i < n_items; i++) {
+    const int64_t R = start[i + 1] - start[i];
+    if (R > PI_SMALL_MAX) { order.push_back(i); large_rows += R; }
+  }
+  const int n_large = (int)order.size();
+  for (int i = 0; i < n_items; i++) {
+    const int64_t R = start[i + 1] - start[i];
+    if (R > 0 && R <= PI_SMALL_MAX) { order.push_back(i); small_max = std::max(small_max, (int)R); }
+  }
+  if (order.empty()) return MCBA_OK;
+  CK(cudaMemcpyAsync(pb.items.p, order.data(), sizeof(int32_t) * order.size(), cudaMemcpyHostToDevice, s));
+  if (n_large) {
+    CK(pb.work.alloc((size_t)n_rows * PI_ROW_BYTES));
+    a.work = pb.work.p; a.items = pb.items.p;
+    k_pose_align<PI_LARGE_THREADS, true><<<n_large, PI_LARGE_THREADS, 0, s>>>(a); CKL();
+  }
+  const int n_small = (int)order.size() - n_large;
+  if (n_small) {
+    a.items = pb.items.p + n_large;
+    k_pose_align<PI_SMALL_THREADS, false><<<n_small, PI_SMALL_THREADS, (size_t)small_max * PI_ROW_BYTES, s>>>(a); CKL();
+  }
+  return MCBA_OK;
+}
+
+}  // namespace
+
+// Relative poses of estimate_relative_poses (axis 0) / estimate_relative_poses_inv (axis 2), every (parent, child) pair in one launch chain
+int mcba_pose_pairs(mcba_ctx* ctx, int32_t C, int32_t F, int32_t B, const double* poses, const uint8_t* valid, int32_t axis,
+                    const int32_t* pairs, int32_t n_pairs, double* t, uint8_t* inliers, int32_t* n_inliers) {
+  if (!ctx) return MCBA_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  { int r = check_pose_dims(ctx, C, F, B); if (r) return r; }
+  REQUIRE(poses && valid, MCBA_ERR_ARG, "null pose table");
+  REQUIRE(axis == 0 || axis == 2, MCBA_ERR_ARG, "axis must be 0 (cameras) or 2 (boards)");
+  REQUIRE(n_pairs >= 0, MCBA_ERR_ARG, "negative pair count");
+  REQUIRE(n_pairs == 0 || (pairs && t && inliers && n_inliers), MCBA_ERR_ARG, "null argument");
+  const int n = axis == 0 ? C : B;
+  const int64_t R = axis == 0 ? (int64_t)F * B : (int64_t)C * F;
+  REQUIRE((int64_t)n_pairs * R < ((int64_t)1 << 31), MCBA_ERR_UNSUPPORTED, "more than 2^31 rows");
+  for (int k = 0; k < n_pairs; k++)
+    REQUIRE(pairs[2 * k] >= 0 && pairs[2 * k] < n && pairs[2 * k + 1] >= 0 && pairs[2 * k + 1] < n && pairs[2 * k] != pairs[2 * k + 1],
+            MCBA_ERR_ARG, "pair index out of range");
+  if (n_pairs == 0) return MCBA_OK;
+  REQUIRE(all_finite(poses, 16 * (size_t)C * F * B), MCBA_ERR_NONFINITE, "non-finite pose in the table");
+  std::vector<PoseRow> rows((size_t)n_pairs * R);
+  std::vector<int64_t> start((size_t)n_pairs + 1);
+  for (int k = 0; k < n_pairs; k++) {
+    const int p = pairs[2 * k], q = pairs[2 * k + 1];
+    start[k] = k * R;
+    PoseRow* o = rows.data() + k * R;
+    if (axis == 0) {           // rows (f, b), f-major, of table[p] and table[q]
+      for (int64_t r = 0; r < R; r++) o[r] = PoseRow{PI_ROW_PAIR, (int32_t)(p * R + r), (int32_t)(q * R + r), 0};
+    } else {                   // rows (c, f), c-major, of the inverted table[:, :, p] and [:, :, q]
+      for (int64_t r = 0; r < R; r++) o[r] = PoseRow{PI_ROW_PAIR_INV, (int32_t)(r * B + p), (int32_t)(r * B + q), 0};
+    }
+  }
+  start[n_pairs] = (int64_t)n_pairs * R;
+  { int r = run_pose_align(ctx, C, F, B, poses, valid, nullptr, nullptr, rows, start, nullptr); if (r) return r; }
+  auto& pb = ctx->pinit;
+  cudaStream_t s = ctx->stream;
+  CK(cudaMemcpyAsync(t, pb.t.p, sizeof(double) * 16 * n_pairs, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(n_inliers, pb.n_inl.p, sizeof(int32_t) * n_pairs, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(inliers, pb.inl.p, (size_t)n_pairs * R, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  return MCBA_OK;
+}
+
+// Rig poses of initialise_poses (tables.py:370-375): per frame, align_transforms_robust over the (camera, board) rows, times = inv(t)
+int mcba_pose_times(mcba_ctx* ctx, int32_t C, int32_t F, int32_t B, const double* poses, const uint8_t* valid, const double* cam_poses,
+                    const uint8_t* cam_valid, const double* board_poses, const uint8_t* board_valid, double* times, uint8_t* times_valid) {
+  if (!ctx) return MCBA_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  { int r = check_pose_dims(ctx, C, F, B); if (r) return r; }
+  REQUIRE(poses && valid, MCBA_ERR_ARG, "null pose table");
+  REQUIRE(cam_poses && cam_valid && board_poses && board_valid && times && times_valid, MCBA_ERR_ARG, "null argument");
+  REQUIRE(all_finite(poses, 16 * (size_t)C * F * B) && all_finite(cam_poses, 16 * (size_t)C) && all_finite(board_poses, 16 * (size_t)B),
+          MCBA_ERR_NONFINITE, "non-finite pose");
+  std::vector<PoseRow> rows;
+  std::vector<int64_t> start(1, 0);
+  std::vector<int32_t> frame_of;
+  for (int f = 0; f < F; f++) {
+    const size_t r0 = rows.size();
+    for (int c = 0; c < C; c++) for (int b = 0; b < B; b++) {
+      const int v = (c * F + f) * B + b;
+      if (cam_valid[c] && valid[v] && board_valid[b]) rows.push_back(PoseRow{PI_ROW_FRAME, v, 0, 0});
+    }
+    if (rows.size() > r0) { start.push_back((int64_t)rows.size()); frame_of.push_back(f); }
+  }
+  for (int f = 0; f < F; f++) {
+    times_valid[f] = 0;
+    for (int k = 0; k < 16; k++) times[16 * (size_t)f + k] = (k % 5 == 0) ? 1.0 : 0.0;
+  }
+  if (frame_of.empty()) return MCBA_OK;
+  { int r = run_pose_align(ctx, C, F, B, poses, valid, cam_poses, board_poses, rows, start, nullptr); if (r) return r; }
+  std::vector<double> t(16 * frame_of.size());
+  CK(cudaMemcpyAsync(t.data(), ctx->pinit.t.p, sizeof(double) * t.size(), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  for (size_t k = 0; k < frame_of.size(); k++) {
+    double* o = times + 16 * (size_t)frame_of[k];
+    pi_inv34(t.data() + 16 * k, o);
+    o[12] = 0.0; o[13] = 0.0; o[14] = 0.0; o[15] = 1.0;
+    times_valid[frame_of[k]] = 1;
+  }
+  return MCBA_OK;
+}
+
+// mean_robust's cluster alone (transform/common.py:6-13): per set of 6-vectors, the mask of the largest Ward cluster
+int mcba_pose_cluster(mcba_ctx* ctx, int32_t n_sets, const int64_t* set_start, const double* vecs, uint8_t* mask) {
+  if (!ctx) return MCBA_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  REQUIRE(n_sets >= 0 && (n_sets == 0 || set_start), MCBA_ERR_ARG, "null set offsets");
+  if (n_sets == 0) return MCBA_OK;
+  REQUIRE(set_start[0] == 0, MCBA_ERR_ARG, "set offsets must start at 0");
+  for (int k = 0; k < n_sets; k++) REQUIRE(set_start[k + 1] >= set_start[k], MCBA_ERR_ARG, "set offsets must not decrease");
+  const int64_t N = set_start[n_sets];
+  REQUIRE(N < ((int64_t)1 << 31), MCBA_ERR_UNSUPPORTED, "more than 2^31 vectors");
+  REQUIRE(N == 0 || (vecs && mask), MCBA_ERR_ARG, "null argument");
+  if (N == 0) return MCBA_OK;
+  REQUIRE(all_finite(vecs, 6 * (size_t)N), MCBA_ERR_NONFINITE, "non-finite vector");
+  std::vector<int64_t> start(set_start, set_start + n_sets + 1);
+  { int r = run_pose_align(ctx, 1, 1, 1, nullptr, nullptr, nullptr, nullptr, {}, start, vecs); if (r) return r; }
+  CK(cudaMemcpyAsync(mask, ctx->pinit.inl.p, (size_t)N, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
   return MCBA_OK;
 }
 

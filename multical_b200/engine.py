@@ -202,6 +202,47 @@ class Engine:
                                           nat.dptr(poses), u8(ok)))
     return intr, poses[:nv].reshape(Cn, F, B, 4, 4), ok[:nv].reshape(Cn, F, B).astype(bool)
 
+  # ---- pose-graph initialisation (include/mcba.h mcba_pose_*) -------------------------------------------------------------------
+  @staticmethod
+  def _pose_table(poses, valid):
+    valid = np.ascontiguousarray(valid, dtype=np.uint8)
+    assert valid.ndim == 3, f"pose table valid must be [C, F, B], got {valid.shape}"
+    return nat.f64(poses).reshape(*valid.shape, 4, 4), valid
+
+  def pose_pairs(self, poses, valid, axis, pairs):
+    """estimate_transform for every (parent, child) of `pairs` along `axis` (0 cameras, 2 boards of the inverted table) ->
+    (t [n, 4, 4], inliers [n, rows], n_inliers [n])."""
+    poses, valid = self._pose_table(poses, valid)
+    Cn, F, B = valid.shape
+    pairs = np.ascontiguousarray(pairs, dtype=np.int32).reshape(-1, 2)
+    n, rows = len(pairs), (F * B if axis == 0 else Cn * F)
+    t, inl, cnt = np.zeros((max(n, 1), 4, 4)), np.zeros((max(n, 1), rows), np.uint8), np.zeros(max(n, 1), np.int32)
+    self._ck(self.lib.mcba_pose_pairs(self.h, Cn, F, B, nat.dptr(poses), valid.ctypes.data_as(C.POINTER(C.c_uint8)), int(axis),
+                                      nat.iptr(pairs), n, nat.dptr(t), inl.ctypes.data_as(C.POINTER(C.c_uint8)), nat.iptr(cnt)))
+    return t[:n], inl[:n].astype(bool), cnt[:n]
+
+  def pose_times(self, poses, valid, cam_poses, cam_valid, board_poses, board_valid):
+    """The rig poses of initialise_poses -> (times [F, 4, 4], valid [F])."""
+    poses, valid = self._pose_table(poses, valid)
+    Cn, F, B = valid.shape
+    cam, board = nat.f64(cam_poses).reshape(Cn, 4, 4), nat.f64(board_poses).reshape(B, 4, 4)
+    cv, bv = np.ascontiguousarray(cam_valid, np.uint8).reshape(Cn), np.ascontiguousarray(board_valid, np.uint8).reshape(B)
+    times, ok = np.zeros((F, 4, 4)), np.zeros(F, np.uint8)
+    u8 = lambda a: a.ctypes.data_as(C.POINTER(C.c_uint8))
+    self._ck(self.lib.mcba_pose_times(self.h, Cn, F, B, nat.dptr(poses), u8(valid), nat.dptr(cam), u8(cv), nat.dptr(board), u8(bv),
+                                      nat.dptr(times), u8(ok)))
+    return times, ok.astype(bool)
+
+  def pose_cluster(self, sets):
+    """mean_robust's clustering: for each array of 6-vectors, the mask of its largest Ward cluster."""
+    sets = [nat.f64(s).reshape(-1, 6) for s in sets]
+    start = np.concatenate([[0], np.cumsum([len(s) for s in sets])]).astype(np.int64)
+    vecs = np.ascontiguousarray(np.concatenate(sets) if sets else np.zeros((0, 6)))
+    mask = np.zeros(max(len(vecs), 1), np.uint8)
+    self._ck(self.lib.mcba_pose_cluster(self.h, len(sets), start.ctypes.data_as(C.POINTER(C.c_int64)), nat.dptr(vecs),
+                                        mask.ctypes.data_as(C.POINTER(C.c_uint8))))
+    return [mask[a:b].astype(bool) for a, b in zip(start[:-1], start[1:])]
+
   def view_errors(self):
     """Per-view sums of squared pixel errors and corner counts of the uploaded problem at the current parameters, both [C,F,B]
     (zero where there is no view): include/mcba.h mcba_view_errors."""

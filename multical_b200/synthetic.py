@@ -205,3 +205,28 @@ def make_scene(C=2, F=20, boards=("charuco", 16, 22, 0.025, 1), model="standard"
 def make_workload(name, seed=0, **overrides):
   cfg = dict(WORKLOADS[name]); cfg.update(overrides)
   return make_scene(seed=seed, **cfg)
+
+
+def make_pose_table_scene(C, F, B, p_valid, seed, outliers=0.0, cam_spread=0.3, dead_camera=None, empty_frame=None):
+  """A make_pose_table result without images, for the pose-graph initialisation: view (c, f, b) = cam[c] frame[f] board[b] times a
+  small perturbation; a fraction `outliers` of the views gets a large one; invalid views hold the identity.  dead_camera: a camera
+  that shares no view with the others; empty_frame: a frame without views.  -> (poses [C,F,B,4,4], valid, num_points, cam poses)."""
+  rng = np.random.default_rng(seed)
+  cam = to_matrix(np.hstack([rng.normal(0, cam_spread, (C, 3)), rng.normal(0, 0.3, (C, 3))]))
+  frm = to_matrix(np.hstack([rng.normal(0, 0.5, (F, 3)), rng.normal(0, 0.3, (F, 3)) + [0, 0, 1.0]]))
+  brd = to_matrix(np.hstack([rng.normal(0, 0.8, (B, 3)), rng.normal(0, 0.1, (B, 3))]))
+  T = cam[:, None, None] @ frm[None, :, None] @ brd[None, None, :]
+  noise = np.hstack([rng.normal(0, 0.003, (C * F * B, 3)), rng.normal(0, 0.002, (C * F * B, 3))])
+  bad = rng.random(C * F * B) < outliers
+  noise[bad] += np.hstack([rng.normal(0, 0.5, (bad.sum(), 3)), rng.normal(0, 0.3, (bad.sum(), 3))])
+  T = T @ to_matrix(noise).reshape(C, F, B, 4, 4)
+  valid = rng.random((C, F, B)) < p_valid
+  if dead_camera is not None:
+    mine = np.arange(F) % 4 == 0
+    valid[dead_camera] = mine[:, None] & valid[dead_camera]
+    valid[np.ix_(np.arange(C) != dead_camera, mine)] = False
+  if empty_frame is not None:
+    valid[:, empty_frame] = False
+  T = np.where(valid[..., None, None], T, np.eye(4))
+  npts = np.where(valid, rng.integers(20, 80, (C, F, B)), 0)
+  return T, valid, npts, cam

@@ -7,12 +7,19 @@
                                     loop around bundle_adjust with the quantile selectors the command line builds, config/workspace.py:47-58)
   pose_table(point_table, ...)   = the first statement of Workspace.initialise_poses   multical/workspace.py:196-198  (tables.make_pose_table:
                                     one board pose per view, here in one launch -- multical_b200/tables.py)
+  initialise_poses(point_table, ...) = Workspace.initialise_poses  multical/workspace.py:196-226 (pose table, pose graph, initial Calibration;
+                                    without the non-overlapping HandEye branch: pass its camera_poses)
 
 A `Workspace` keeps working unchanged when its module imports `Calibration`, `select_threshold` and `tables.make_pose_table` from this
 package (INTEGRATION.md A, D); these functions are the same steps for callers that do not carry a `Workspace` around (bench.py, tests)."""
+import numpy as np
+
 from .calibration import Calibration, select_threshold
 from .intrinsics import calibrate_cameras
-from .tables import make_pose_table
+from .log import info
+from .parameters import ParamList
+from .pose_set import PoseSet, StaticFrames
+from .tables import initialise_poses as _initialise_poses, make_pose_table
 
 
 def calibrate_single(boards, detected_points, image_sizes, camera_model, intrinsic_error_limit, fix_aspect=False, has_skew=False,
@@ -45,3 +52,31 @@ def optimize(calib: Calibration, iter=3, loss="linear", outlier_quantile=0.75, o
 def pose_table(point_table, boards, cameras, exclude_bad_poses=True, pose_error_limit=1.0):
   """workspace.py:196-198 (the defaults are initialise_poses' own: bad poses excluded, limit 1 px)."""
   return make_pose_table(point_table, boards, cameras, exclude_bad_poses, pose_error_limit)
+
+
+def table_info(valid, camera_names, board_names):
+  """tables.table_info (tables.py:190-204): view counts per camera and board."""
+  valid = np.asarray(valid)
+  info(f"Total: {int(valid.sum())}, cameras: {dict(zip(camera_names, valid.sum(axis=(1, 2)).tolist()))}, "
+       f"Boards: {dict(zip(board_names, valid.sum(axis=(0, 1)).tolist()))}")
+  if len(camera_names) > 1 and len(board_names) > 1:
+    info("Camera-board matrix")
+    info(valid.sum(axis=1))
+
+
+def initialise_poses(point_table, boards, cameras, motion_model=StaticFrames, camera_poses=None, exclude_bad_poses=True,
+                     pose_error_limit=1.0, camera_names=None, board_names=None, image_names=None):
+  """workspace.py:196-226: make_pose_table, initialise_poses, then the initial Calibration (reported as "Initialisation").
+  camera_poses: {camera name: 4x4} or a [C,4,4] array in camera order."""
+  camera_names = camera_names or [str(i) for i in range(len(cameras))]
+  board_names = board_names or [str(i) for i in range(len(boards))]
+  table = make_pose_table(point_table, boards, cameras, exclude_bad_poses, pose_error_limit)
+  info("Pose counts:")
+  table_info(table.valid, camera_names, board_names)
+  if isinstance(camera_poses, dict):
+    camera_poses = np.array([camera_poses[k] for k in camera_names])
+  init = _initialise_poses(table, camera_poses=camera_poses)
+  calib = Calibration(ParamList(cameras, camera_names), ParamList(boards, board_names), point_table, PoseSet(init.camera, camera_names), PoseSet(init.board, board_names),
+                      motion_model.init(init.times, image_names))
+  calib.report("Initialisation")
+  return calib
