@@ -30,7 +30,8 @@ extern "C" {
 typedef struct mcba_ctx mcba_ctx;
 
 enum { MCBA_OK = 0, MCBA_ERR_ARG = 1, MCBA_ERR_CUDA = 2, MCBA_ERR_STATE = 3, MCBA_ERR_NCCL = 4,
-       MCBA_ERR_NONFINITE = 5, MCBA_ERR_UNSUPPORTED = 6 };
+       MCBA_ERR_NONFINITE = 5, MCBA_ERR_UNSUPPORTED = 6,
+       MCBA_ERR_DEGENERATE = 7 /* input too degenerate for the estimate asked for (mcba_hand_eye_vote) */ };
 
 /* camera models: camera.py:43-48 (cv2.projectPoints, 5/8/12/14 coefficients) and
  * camera_fisheye.py:113-117 (cv2.fisheye.projectPoints, 4 coefficients) */
@@ -263,6 +264,21 @@ int  mcba_pose_pairs(mcba_ctx* ctx, int32_t C, int32_t F, int32_t B, const doubl
 int  mcba_pose_times(mcba_ctx* ctx, int32_t C, int32_t F, int32_t B, const double* poses, const uint8_t* valid, const double* cam_poses,
                      const uint8_t* cam_valid, const double* board_poses, const uint8_t* board_valid, double* times, uint8_t* times_valid);
 int  mcba_pose_cluster(mcba_ctx* ctx, int32_t n_sets, const int64_t* set_start, const double* vecs, uint8_t* mask);
+
+/* -- non-overlapping camera initialisation (HandEye.initialise_camera_poses, hand_eye/hand_eye.py:35-79) -------------------------------
+ * mcba_hand_eye_quads: one cv2.calibrateRobotWorldHandEye(..., CALIB_ROBOT_WORLD_HAND_EYE_SHAH) of master_slave_pair per quadruple
+ *   quads int32[n][4] = (master, slave, boardM, boardS) over the images where valid[master, :, boardM] & valid[slave, :, boardS], with
+ *   A_i = inv(poses[master, i, boardM]), B_i = inv(poses[slave, i, boardS]) and A X = Z B.  Out: X f64[n][4][4] (slaveCam_wrt_masterCam),
+ *   Z f64[n][4][4], n_images int32[n], ok uint8[n]: 0 for fewer than 3 images, for a rotation whose determinant OpenCV calls null, and
+ *   for a top singular value of sum kron(R_B, R_A) that is not separated from the second (relative gap below 1e-6: DESIGN.md §3f).
+ * mcba_hand_eye_vote: probabilistic_guess (hand_eye/helper.py:5-18) per set of points f64[N][3] (CSR offsets set_start int64[n_sets+1]):
+ *   scipy.stats.gaussian_kde densities at the points -> density f64[N], best int32[n_sets] = the argmax within the set (ties: the lowest
+ *   index within 1e-12 relative of the maximum).  A set of 3 points or fewer, or with a singular covariance, fails with
+ *   MCBA_ERR_DEGENERATE.
+ * Non-finite poses or points fail with MCBA_ERR_NONFINITE.  Neither touches the uploaded problem. */
+int  mcba_hand_eye_quads(mcba_ctx* ctx, int32_t C, int32_t F, int32_t B, const double* poses, const uint8_t* valid, int32_t n_quads,
+                         const int32_t* quads, double* X, double* Z, int32_t* n_images, uint8_t* ok);
+int  mcba_hand_eye_vote(mcba_ctx* ctx, int32_t n_sets, const int64_t* set_start, const double* points, double* density, int32_t* best);
 
 /* -- measurement hooks (bench.py): launch one kernel family on the context stream -------------- */
 enum { MCBA_BENCH_LINEARIZE = 0, MCBA_BENCH_RESIDUAL = 1, MCBA_BENCH_COST = 2,

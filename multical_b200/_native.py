@@ -29,7 +29,8 @@ EXPORTS = ["mcba_create", "mcba_destroy", "mcba_last_error", "mcba_set_stream", 
            "mcba_linearize", "mcba_reprojection_error", "mcba_solve", "mcba_bench_launch", "mcba_bench_info",
            "mcba_table_upload", "mcba_table_from_detections", "mcba_table_download", "mcba_table_set_inliers",
            "mcba_table_get_inliers", "mcba_table_select", "mcba_pnp_views", "mcba_table_errors", "mcba_table_error_ranks", "mcba_table_count_below", "mcba_table_reject",
-           "mcba_intrinsic_init", "mcba_view_errors", "mcba_pose_pairs", "mcba_pose_times", "mcba_pose_cluster"]
+           "mcba_intrinsic_init", "mcba_view_errors", "mcba_pose_pairs", "mcba_pose_times", "mcba_pose_cluster",
+           "mcba_hand_eye_quads", "mcba_hand_eye_vote"]
 TABLE_VALID, TABLE_INLIERS = 0, 1
 
 
@@ -126,6 +127,8 @@ def load():
   lib.mcba_pose_pairs.argtypes = [P, i32, i32, i32, D, U8, i32, I32, i32, D, U8, I32]
   lib.mcba_pose_times.argtypes = [P, i32, i32, i32, D, U8, D, U8, D, U8, D, U8]
   lib.mcba_pose_cluster.argtypes = [P, i32, I64, D, U8]
+  lib.mcba_hand_eye_quads.argtypes = [P, i32, i32, i32, D, U8, i32, I32, D, D, I32, U8]
+  lib.mcba_hand_eye_vote.argtypes = [P, i32, I64, D, D, I32]
   _lib = lib
   return lib
 

@@ -22,6 +22,7 @@
 #include "pnp_kernels.cuh"
 #include "intrinsics_kernels.cuh"
 #include "pose_init_kernels.cuh"
+#include "hand_eye_init_kernels.cuh"
 
 using namespace mcba;
 
@@ -143,6 +144,10 @@ struct mcba_ctx {
     DevBuf<double> poses, cam, board, m1, m2, vecs, t; DevBuf<uint8_t> valid, mask, inl; DevBuf<PoseRow> rows;
     DevBuf<int64_t> start; DevBuf<int32_t> items, n_inl; DevBuf<char> work;
   } pinit;
+  // non-overlapping camera initialisation (mcba_hand_eye_quads / mcba_hand_eye_vote)
+  struct HandEyeInitBuffers {
+    DevBuf<double> poses, X, Z, points, density; DevBuf<uint8_t> valid, ok; DevBuf<int32_t> quads, n_images, best; DevBuf<int64_t> start;
+  } heinit;
 };
 
 #define CK(call)                                                                                   \
@@ -1321,6 +1326,73 @@ int mcba_pose_cluster(mcba_ctx* ctx, int32_t n_sets, const int64_t* set_start, c
   { int r = run_pose_align(ctx, 1, 1, 1, nullptr, nullptr, nullptr, nullptr, {}, start, vecs); if (r) return r; }
   CK(cudaMemcpyAsync(mask, ctx->pinit.inl.p, (size_t)N, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
+  return MCBA_OK;
+}
+
+// One cv2.calibrateRobotWorldHandEye(SHAH) of HandEye.master_slave_pair (hand_eye/hand_eye.py:82-107) per quadruple, one CTA each
+int mcba_hand_eye_quads(mcba_ctx* ctx, int32_t C, int32_t F, int32_t B, const double* poses, const uint8_t* valid, int32_t n_quads,
+                        const int32_t* quads, double* X, double* Z, int32_t* n_images, uint8_t* ok) {
+  if (!ctx) return MCBA_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  { int r = check_pose_dims(ctx, C, F, B); if (r) return r; }
+  REQUIRE(poses && valid, MCBA_ERR_ARG, "null pose table");
+  REQUIRE(n_quads >= 0, MCBA_ERR_ARG, "negative quadruple count");
+  REQUIRE(n_quads == 0 || (quads && X && Z && n_images && ok), MCBA_ERR_ARG, "null argument");
+  for (int k = 0; k < n_quads; k++) {
+    const int32_t* q = quads + 4 * (size_t)k;
+    REQUIRE(q[0] >= 0 && q[0] < C && q[1] >= 0 && q[1] < C && q[2] >= 0 && q[2] < B && q[3] >= 0 && q[3] < B, MCBA_ERR_ARG,
+            "quadruple index out of range");
+    REQUIRE(q[0] != q[1], MCBA_ERR_ARG, "quadruple with master == slave");
+  }
+  if (n_quads == 0) return MCBA_OK;
+  REQUIRE(all_finite(poses, 16 * (size_t)C * F * B), MCBA_ERR_NONFINITE, "non-finite pose in the table");
+  auto& hb = ctx->heinit;
+  cudaStream_t s = ctx->stream;
+  const size_t nv = (size_t)C * F * B, nq = (size_t)n_quads;
+  CK(hb.poses.alloc(16 * nv)); CK(hb.valid.alloc(nv));
+  CK(hb.quads.alloc(4 * nq)); CK(hb.X.alloc(16 * nq)); CK(hb.Z.alloc(16 * nq)); CK(hb.n_images.alloc(nq)); CK(hb.ok.alloc(nq));
+  CK(cudaMemcpyAsync(hb.poses.p, poses, sizeof(double) * 16 * nv, cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(hb.valid.p, valid, nv, cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(hb.quads.p, quads, sizeof(int32_t) * 4 * nq, cudaMemcpyHostToDevice, s));
+  HandEyeArgs a{C, F, B, hb.poses.p, hb.valid.p, hb.quads.p, hb.X.p, hb.Z.p, hb.n_images.p, hb.ok.p};
+  k_he_quads<<<n_quads, HE_THREADS, 0, s>>>(a); CKL();
+  CK(cudaMemcpyAsync(X, hb.X.p, sizeof(double) * 16 * nq, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(Z, hb.Z.p, sizeof(double) * 16 * nq, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(n_images, hb.n_images.p, sizeof(int32_t) * nq, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(ok, hb.ok.p, nq, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  return MCBA_OK;
+}
+
+// probabilistic_guess (hand_eye/helper.py:5-18) for every set: gaussian_kde densities at the points, and the argmax
+int mcba_hand_eye_vote(mcba_ctx* ctx, int32_t n_sets, const int64_t* set_start, const double* points, double* density, int32_t* best) {
+  if (!ctx) return MCBA_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  REQUIRE(n_sets >= 0 && (n_sets == 0 || (set_start && best)), MCBA_ERR_ARG, "null set offsets");
+  if (n_sets == 0) return MCBA_OK;
+  REQUIRE(set_start[0] == 0, MCBA_ERR_ARG, "set offsets must start at 0");
+  for (int k = 0; k < n_sets; k++) REQUIRE(set_start[k + 1] >= set_start[k], MCBA_ERR_ARG, "set offsets must not decrease");
+  const int64_t N = set_start[n_sets];
+  REQUIRE(N < ((int64_t)1 << 31), MCBA_ERR_UNSUPPORTED, "more than 2^31 points");
+  REQUIRE(points && density, MCBA_ERR_ARG, "null argument");
+  for (int k = 0; k < n_sets; k++)
+    REQUIRE(set_start[k + 1] - set_start[k] > 3, MCBA_ERR_DEGENERATE,
+            "set " + std::to_string(k) + " has " + std::to_string(set_start[k + 1] - set_start[k]) +
+            " points: a 3-D kernel density estimate needs at least 4");
+  REQUIRE(all_finite(points, 3 * (size_t)N), MCBA_ERR_NONFINITE, "non-finite point");
+  auto& hb = ctx->heinit;
+  cudaStream_t s = ctx->stream;
+  CK(hb.start.alloc((size_t)n_sets + 1)); CK(hb.points.alloc(3 * (size_t)N)); CK(hb.density.alloc((size_t)N));
+  CK(hb.best.alloc((size_t)n_sets));
+  CK(cudaMemcpyAsync(hb.start.p, set_start, sizeof(int64_t) * (n_sets + 1), cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(hb.points.p, points, sizeof(double) * 3 * N, cudaMemcpyHostToDevice, s));
+  HandEyeVoteArgs a{n_sets, hb.start.p, hb.points.p, hb.density.p, hb.best.p};
+  k_he_vote<<<(n_sets + HE_VOTE_WARPS - 1) / HE_VOTE_WARPS, 32 * HE_VOTE_WARPS, 0, s>>>(a); CKL();
+  CK(cudaMemcpyAsync(density, hb.density.p, sizeof(double) * N, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(best, hb.best.p, sizeof(int32_t) * n_sets, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  for (int k = 0; k < n_sets; k++)
+    REQUIRE(best[k] >= 0, MCBA_ERR_DEGENERATE, "set " + std::to_string(k) + " has a singular covariance");
   return MCBA_OK;
 }
 

@@ -53,6 +53,7 @@ class Engine:
     if rc == 1: raise AssertionError(msg)            # reference uses `assert` for bad inputs (calibration.py:59-61)
     if rc == 5: raise ValueError(msg)                # scipy: "Residuals are not finite in the initial point."
     if rc == 6: raise NotImplementedError(msg)
+    if rc == 7: raise ValueError(msg)                # scipy.stats.gaussian_kde: too few points / singular covariance
     raise NativeError(f"libmcba error {rc}: {msg}")
 
   # ---- multi-GPU --------------------------------------------------------------------------------
@@ -242,6 +243,30 @@ class Engine:
     self._ck(self.lib.mcba_pose_cluster(self.h, len(sets), start.ctypes.data_as(C.POINTER(C.c_int64)), nat.dptr(vecs),
                                         mask.ctypes.data_as(C.POINTER(C.c_uint8))))
     return [mask[a:b].astype(bool) for a, b in zip(start[:-1], start[1:])]
+
+  # ---- non-overlapping camera initialisation (include/mcba.h mcba_hand_eye_*) ----------------------------------------------------
+  def hand_eye_quads(self, poses, valid, quads):
+    """cv2.calibrateRobotWorldHandEye(SHAH) of HandEye.master_slave_pair for every (master, slave, boardM, boardS) of `quads` ->
+    (X [n, 4, 4], Z [n, 4, 4], n_images [n], ok [n])."""
+    poses, valid = self._pose_table(poses, valid)
+    Cn, F, B = valid.shape
+    quads = np.ascontiguousarray(quads, dtype=np.int32).reshape(-1, 4)
+    n, k = len(quads), max(len(quads), 1)
+    X, Z, cnt, ok = np.zeros((k, 4, 4)), np.zeros((k, 4, 4)), np.zeros(k, np.int32), np.zeros(k, np.uint8)
+    u8 = lambda a: a.ctypes.data_as(C.POINTER(C.c_uint8))
+    self._ck(self.lib.mcba_hand_eye_quads(self.h, Cn, F, B, nat.dptr(poses), u8(valid), n, nat.iptr(quads), nat.dptr(X), nat.dptr(Z),
+                                          nat.iptr(cnt), u8(ok)))
+    return X[:n], Z[:n], cnt[:n], ok[:n].astype(bool)
+
+  def hand_eye_vote(self, sets):
+    """probabilistic_guess for each array of 3-D points: (gaussian_kde densities at the points, index of the densest) per set."""
+    sets = [nat.f64(s).reshape(-1, 3) for s in sets]
+    start = np.concatenate([[0], np.cumsum([len(s) for s in sets])]).astype(np.int64)
+    pts = np.ascontiguousarray(np.concatenate(sets) if sets else np.zeros((0, 3)))
+    dens, best = np.zeros(max(len(pts), 1)), np.zeros(max(len(sets), 1), np.int32)
+    self._ck(self.lib.mcba_hand_eye_vote(self.h, len(sets), start.ctypes.data_as(C.POINTER(C.c_int64)), nat.dptr(pts), nat.dptr(dens),
+                                         nat.iptr(best)))
+    return [dens[a:b] for a, b in zip(start[:-1], start[1:])], best[:len(sets)]
 
   def view_errors(self):
     """Per-view sums of squared pixel errors and corner counts of the uploaded problem at the current parameters, both [C,F,B]

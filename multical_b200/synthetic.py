@@ -207,10 +207,12 @@ def make_workload(name, seed=0, **overrides):
   return make_scene(seed=seed, **cfg)
 
 
-def make_pose_table_scene(C, F, B, p_valid, seed, outliers=0.0, cam_spread=0.3, dead_camera=None, empty_frame=None):
+def make_pose_table_scene(C, F, B, p_valid, seed, outliers=0.0, cam_spread=0.3, dead_camera=None, empty_frame=None, disjoint=False):
   """A make_pose_table result without images, for the pose-graph initialisation: view (c, f, b) = cam[c] frame[f] board[b] times a
   small perturbation; a fraction `outliers` of the views gets a large one; invalid views hold the identity.  dead_camera: a camera
-  that shares no view with the others; empty_frame: a frame without views.  -> (poses [C,F,B,4,4], valid, num_points, cam poses)."""
+  that shares no view with the others; empty_frame: a frame without views; disjoint: camera c sees only the boards b with
+  b % C == c (a non-overlapping rig: no two cameras see the same board, so the camera-overlap matrix is zero; B >= 3 C gives every
+  camera pair at least 9 hand-eye quadruples).  -> (poses [C,F,B,4,4], valid, num_points, cam poses)."""
   rng = np.random.default_rng(seed)
   cam = to_matrix(np.hstack([rng.normal(0, cam_spread, (C, 3)), rng.normal(0, 0.3, (C, 3))]))
   frm = to_matrix(np.hstack([rng.normal(0, 0.5, (F, 3)), rng.normal(0, 0.3, (F, 3)) + [0, 0, 1.0]]))
@@ -227,6 +229,8 @@ def make_pose_table_scene(C, F, B, p_valid, seed, outliers=0.0, cam_spread=0.3, 
     valid[np.ix_(np.arange(C) != dead_camera, mine)] = False
   if empty_frame is not None:
     valid[:, empty_frame] = False
+  if disjoint:
+    valid &= (np.arange(B)[None, :] % C == np.arange(C)[:, None])[:, None, :]
   T = np.where(valid[..., None, None], T, np.eye(4))
   npts = np.where(valid, rng.integers(20, 80, (C, F, B)), 0)
   return T, valid, npts, cam

@@ -8,7 +8,7 @@
   pose_table(point_table, ...)   = the first statement of Workspace.initialise_poses   multical/workspace.py:196-198  (tables.make_pose_table:
                                     one board pose per view, here in one launch -- multical_b200/tables.py)
   initialise_poses(point_table, ...) = Workspace.initialise_poses  multical/workspace.py:196-226 (pose table, pose graph, initial Calibration;
-                                    without the non-overlapping HandEye branch: pass its camera_poses)
+                                    is_non_overlapping: the camera poses of nonoverlap.HandEye, workspace.py:203-207)
 
 A `Workspace` keeps working unchanged when its module imports `Calibration`, `select_threshold` and `tables.make_pose_table` from this
 package (INTEGRATION.md A, D); these functions are the same steps for callers that do not carry a `Workspace` around (bench.py, tests)."""
@@ -17,6 +17,7 @@ import numpy as np
 from .calibration import Calibration, select_threshold
 from .intrinsics import calibrate_cameras
 from .log import info
+from .nonoverlap import HandEye
 from .parameters import ParamList
 from .pose_set import PoseSet, StaticFrames
 from .tables import initialise_poses as _initialise_poses, make_pose_table
@@ -65,14 +66,20 @@ def table_info(valid, camera_names, board_names):
 
 
 def initialise_poses(point_table, boards, cameras, motion_model=StaticFrames, camera_poses=None, exclude_bad_poses=True,
-                     pose_error_limit=1.0, camera_names=None, board_names=None, image_names=None):
+                     pose_error_limit=1.0, camera_names=None, board_names=None, image_names=None, is_non_overlapping=False,
+                     image_path=None):
   """workspace.py:196-226: make_pose_table, initialise_poses, then the initial Calibration (reported as "Initialisation").
-  camera_poses: {camera name: 4x4} or a [C,4,4] array in camera order."""
+  camera_poses: {camera name: 4x4} or a [C,4,4] array in camera order.  is_non_overlapping (used only without camera_poses): the
+  camera poses come from nonoverlap.HandEye, which writes camera_groups.pkl and initial_guess.json into image_path when it is given."""
   camera_names = camera_names or [str(i) for i in range(len(cameras))]
   board_names = board_names or [str(i) for i in range(len(boards))]
   table = make_pose_table(point_table, boards, cameras, exclude_bad_poses, pose_error_limit)
   info("Pose counts:")
   table_info(table.valid, camera_names, board_names)
+  if is_non_overlapping and camera_poses is None:
+    handeye = HandEye(table, camera_names, image_path)
+    handeye.initialise_camera_poses()
+    camera_poses = handeye.cam_init
   if isinstance(camera_poses, dict):
     camera_poses = np.array([camera_poses[k] for k in camera_names])
   init = _initialise_poses(table, camera_poses=camera_poses)
