@@ -233,10 +233,15 @@ int  mcba_pnp_views(mcba_ctx* ctx, const mcba_problem_desc* desc, const int64_t*
  * least squares over two vanishing-point rows per view; desc->optimize & MCBA_OPT_FIX_ASPECT gives fx = fy = their mean.
  * Out: intrinsics f64[C][5+nd] = [fx fy cx cy 0 | zeros] (NaN focal lengths for a camera without a usable view), poses f64[C*F*B][4][4]
  * (board wrt camera, k_pnp_views under K0 and zero distortion: OpenCV's findExtrinsicCameraParams2), ok uint8[C*F*B] (0 for unused views).
- * Boards with any z != 0 fail with MCBA_ERR_UNSUPPORTED, as OpenCV refuses non-planar rigs without an initial matrix; so does the
- * fisheye model.  Does not touch the uploaded problem.
+ * desc->model == MCBA_MODEL_FISHEYE (CameraFisheye.calibrate, camera_fisheye.py:70-94: cv2.fisheye.calibrate without an initial
+ * matrix) replaces the homographies and initIntrinsicParams2D by OpenCV's fisheye start, fx = fy = max(w, h) / 2 and principal point
+ * (w/2 - 0.5, h/2 - 0.5) whatever the views, and the poses by k_pnp_views<MCBA_MODEL_FISHEYE> under it (fisheye undistortion, exact at
+ * zero distortion, then the pinhole PnP); fix_aspect is ignored.
+ * Boards with any z != 0 fail with MCBA_ERR_UNSUPPORTED, as OpenCV refuses non-planar rigs without an initial matrix.  Does not touch
+ * the uploaded problem.
  * The solve itself is the engine's own: one camera, the used views as frames (frame pose = board wrt camera), camera and board poses at
- * identity and fixed, optimize = MCBA_OPT_MOTION | MCBA_OPT_CAMERAS [| MCBA_OPT_FIX_ASPECT].  It iterates to its own tolerances: the
+ * identity and fixed, optimize = MCBA_OPT_MOTION | MCBA_OPT_CAMERAS [| MCBA_OPT_FIX_ASPECT, never for fisheye: OpenCV's fisheye
+ * calibration has no aspect constraint].  It iterates to its own tolerances: the
  * minimum OpenCV's LM approaches, not the point where OpenCV's iteration limit stops it.
  * mcba_view_errors: per view of the packed problem at the current parameters, sumsq f64[C*F*B] = sum of squared pixel errors (u and v)
  * and count int64[C*F*B] = corners (both zero where there is no view): calibrateCameraExtended's perViewErrors = sqrt(sumsq / count). */

@@ -84,11 +84,25 @@ class CameraFisheye(Camera):
     self.fix_aspect = fix_aspect
     self.has_skew = has_skew
 
+  @staticmethod
+  def calibrate(boards, detections, image_size, max_iter=10, eps=1e-3, model="standard", fix_aspect=False, has_skew=False, flags=0,
+                max_images=None, **solve_opts):
+    """camera_fisheye.py:70-94 on the GPU (multical_b200/intrinsics.py): (CameraFisheye, err)."""
+    from .intrinsics import calibrate_fisheye
+    return calibrate_fisheye(boards, detections, image_size, max_iter=max_iter, eps=eps, model=model, fix_aspect=fix_aspect,
+                             has_skew=has_skew, flags=flags, max_images=max_images, **solve_opts)
+
 
 def calibrate_cameras(boards, points, image_sizes, intrinsic_error_limit, **kwargs):
   """camera.py:237-241 on the GPU (multical_b200/intrinsics.py): (cameras, errs)."""
   from .intrinsics import calibrate_cameras
   return calibrate_cameras(boards, points, image_sizes, intrinsic_error_limit, **kwargs)
+
+
+def calibrate_cameras_fisheye(boards, points, image_sizes, **kwargs):
+  """camera_fisheye.py:173-177 on the GPU (multical_b200/intrinsics.py): (cameras, errs)."""
+  from .intrinsics import calibrate_cameras_fisheye
+  return calibrate_cameras_fisheye(boards, points, image_sizes, **kwargs)
 
 
 def engine_model_of(camera):

@@ -6,6 +6,8 @@
 //                       Levenberg-Marquardt on its pixel reprojection error (what cv2.findHomography does)
 //   k_zhang_init        one CTA per camera: OpenCV's initIntrinsicParams2D (cv2.initCameraMatrix2D) from those homographies
 //   (the initial per-view poses are k_pnp_views, pnp_kernels.cuh, given K0 and zero distortion: OpenCV's findExtrinsicCameraParams2)
+//   k_fisheye_k0        one thread per camera: the start of cv2.fisheye.calibrate (CameraFisheye.calibrate, camera_fisheye.py:70-94),
+//                       whose initial per-view poses are k_pnp_views<MODEL_FISHEYE> under it (exact fisheye undistortion at k = 0)
 //   k_view_sumsq        per view of the packed problem: sum of squared pixel errors (k_views<MODE_COST>, kernels.cuh) and corner count
 //
 // K0 only seeds the trust-region solve, which iterates to its own tolerances.
@@ -258,6 +260,19 @@ k_zhang_init(ZhangArgs a) {
     k[0] = fx; k[1] = fy; k[2] = cx; k[3] = cy;
     for (int i = 4; i < a.kint; i++) k[i] = 0.0;
   }
+}
+
+// cv2.fisheye.calibrate's start without an initial matrix: fx = fy = max(w, h) / 2, principal point (w/2 - 0.5, h/2 - 0.5), zero skew
+// (CALIB_FIX_SKEW) and zero distortion -- what OpenCV 4.13 returns when its loop runs no iteration (DESIGN.md §3d).  It needs no view;
+// one thread per camera.
+__global__ void k_fisheye_k0(int C, int kint, const int32_t* image_size, double* intr) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  const int w = image_size[2 * c], h = image_size[2 * c + 1];
+  const double f = max(w, h) / 2.0;
+  double* k = intr + (size_t)c * kint;
+  k[0] = f; k[1] = f; k[2] = w / 2.0 - 0.5; k[3] = h / 2.0 - 0.5;
+  for (int i = 4; i < kint; i++) k[i] = 0.0;
 }
 
 // per-view sums of squared pixel errors (u and v) and corner counts, dense over (camera, frame, board), from the per-view costs of

@@ -1069,8 +1069,8 @@ int mcba_intrinsic_init(mcba_ctx* ctx, const mcba_problem_desc* desc, const int6
   CK(cudaSetDevice(ctx->device));
   { int r = check_desc(ctx, desc); if (r) return r; }
   REQUIRE(det_start && board_points && board_grid && image_sizes && view_use && intrinsics && poses && ok, MCBA_ERR_ARG, "null argument");
-  REQUIRE(desc->model != MODEL_FISHEYE, MCBA_ERR_UNSUPPORTED, "the intrinsic initialisation is for the pinhole camera models");
   const int C = desc->C, F = desc->F, B = desc->B, Pn = desc->P, nv = C * F * B;
+  const bool fisheye = desc->model == MODEL_FISHEYE;
   const int kint = 5 + model_nd(desc->model);
   { int r = check_detections(ctx, desc, det_start, det_ids, det_xy, board_grid); if (r) return r; }
   for (int c = 0; c < C; c++) REQUIRE(image_sizes[2 * c] > 0 && image_sizes[2 * c + 1] > 0, MCBA_ERR_ARG, "image sizes must be positive");
@@ -1102,18 +1102,23 @@ int mcba_intrinsic_init(mcba_ctx* ctx, const mcba_problem_desc* desc, const int6
   if (n_used) CK(cudaMemcpyAsync(ib.used.p, used.data(), sizeof(int32_t) * used.size(), cudaMemcpyHostToDevice, s));
   CK(cudaMemcpyAsync(ib.cam_start.p, cam_start.data(), sizeof(int32_t) * cam_start.size(), cudaMemcpyHostToDevice, s));
   CK(cudaMemcpyAsync(ib.size.p, image_sizes, sizeof(int32_t) * (size_t)C * 2, cudaMemcpyHostToDevice, s));
-  if (n_used) {
-    HomographyArgs h{};
-    h.n_used = n_used; h.B = B; h.P = Pn; h.used = ib.used.p; h.det_start = pb.start.p; h.det_ids = pb.ids.p; h.det_xy = pb.xy.p;
-    h.board_pts = pb.bp.p; h.H = ib.H.p; h.ok = ib.hok.p;
-    k_view_homography<<<(n_used + HOMOG_WARPS - 1) / HOMOG_WARPS, HOMOG_WARPS * 32, 0, s>>>(h); CKL();
+  if (fisheye) {
+    if (C) { k_fisheye_k0<<<(C + 127) / 128, 128, 0, s>>>(C, kint, ib.size.p, ib.k0.p); CKL(); }
+  } else {
+    if (n_used) {
+      HomographyArgs h{};
+      h.n_used = n_used; h.B = B; h.P = Pn; h.used = ib.used.p; h.det_start = pb.start.p; h.det_ids = pb.ids.p; h.det_xy = pb.xy.p;
+      h.board_pts = pb.bp.p; h.H = ib.H.p; h.ok = ib.hok.p;
+      k_view_homography<<<(n_used + HOMOG_WARPS - 1) / HOMOG_WARPS, HOMOG_WARPS * 32, 0, s>>>(h); CKL();
+    }
+    ZhangArgs z{};
+    z.kint = kint; z.fix_aspect = (desc->optimize & MCBA_OPT_FIX_ASPECT) ? 1 : 0; z.cam_start = ib.cam_start.p; z.image_size = ib.size.p;
+    z.H = ib.H.p; z.ok = ib.hok.p; z.intr = ib.k0.p;
+    k_zhang_init<<<C, ZHANG_THREADS, 0, s>>>(z); CKL();
   }
-  ZhangArgs z{};
-  z.kint = kint; z.fix_aspect = (desc->optimize & MCBA_OPT_FIX_ASPECT) ? 1 : 0; z.cam_start = ib.cam_start.p; z.image_size = ib.size.p;
-  z.H = ib.H.p; z.ok = ib.hok.p; z.intr = ib.k0.p;
-  k_zhang_init<<<C, ZHANG_THREADS, 0, s>>>(z); CKL();
   if (nv) {
-    { int r = launch_pnp(ctx, desc, MODEL_STANDARD, kint, ib.k0.p); if (r) return r; }      // zero distortion: the pinhole K0
+    // zero distortion: the pinhole K0, or the fisheye K0 whose undistortion is exact at k = 0
+    { int r = launch_pnp(ctx, desc, fisheye ? MODEL_FISHEYE : MODEL_STANDARD, kint, ib.k0.p); if (r) return r; }
     CK(cudaMemcpyAsync(poses, pb.pose.p, sizeof(double) * 16 * (size_t)nv, cudaMemcpyDeviceToHost, s));
     CK(cudaMemcpyAsync(ok, pb.ok.p, (size_t)nv, cudaMemcpyDeviceToHost, s));
   }

@@ -14,7 +14,11 @@ What stays on the host is the bookkeeping of the reference: the view set (calibr
 The solve iterates to its own tolerances (ftol = xtol = gtol = 1e-10, at most 100 evaluations): it reaches the minimum that OpenCV's
 Levenberg-Marquardt approaches, not the point where OpenCV's criteria (`max_iter`, `eps`: accepted for the reference's signature, unused)
 stop it -- with the reference's (10, 1e-3), OpenCV stops ~1e-5 relative away from it in fx.  The calibration runs on an engine of its own, so
-the process-wide bundle-adjustment engine keeps its problem."""
+the process-wide bundle-adjustment engine keeps its problem.
+
+The fisheye model (CameraFisheye.calibrate / calibrate_cameras_fisheye, camera_fisheye.py:70-94, 173-177: one cv2.fisheye.calibrate per
+camera, no loop) takes the same steps once: the same view set, OpenCV's fisheye start K0 with per-view poses by fisheye PnP under it
+(mcba_intrinsic_init), the same one-camera problem without an aspect constraint, and the total RMS as err."""
 import numpy as np
 
 from . import _native as nat
@@ -28,8 +32,11 @@ UNSUPPORTED = {
               "RMS OpenCV's LM settles at (50-view scenes, restarts do not help), so the result would not be OpenCV's minimum",
   "thin_prism": "under CALIB_THIN_PRISM_MODEL OpenCV keeps k4..k6 at zero, and the engine cannot fix single distortion coefficients",
   "tilted": "under CALIB_TILTED_MODEL OpenCV keeps k4..k6 and s1..s4 at zero, and the engine cannot fix single distortion coefficients",
-  "fisheye": "the reference's fisheye intrinsic calibration (camera_fisheye.py) is broken, and the engine cannot fix single coefficients",
+  "fisheye": "fisheye cameras calibrate with calibrate_cameras_fisheye / CameraFisheye.calibrate (the reference's camera_fisheye.py "
+             "signature: no intrinsic_error_limit, no rejection loop)",
 }
+# CameraFisheye.model (camera_fisheye.py:43-49): stored on the camera; the reference never passes them to OpenCV's flags
+FISHEYE_MODELS = ("standard", "fix_k1", "fix_k2", "fix_k3", "fix_k4")
 
 _engines = {}
 
@@ -104,13 +111,10 @@ def _solve_camera(eng, model, fix_aspect, views, k0, poses, board_points, solve_
                 solve=info)
 
 
-def calibrate_views(boards, cam_views, image_sizes, model="standard", fix_aspect=False, engine=None, camera_ids=None, **solve_opts):
-  """One calibrateCameraExtended for each camera's list of views (calibration_points entries, any order): returns per camera a struct of
-  the intrinsics [fx fy cx cy skew dist...], the views' rtvecs (board wrt camera), per-view RMS, total RMS, K0 and the solve summary.
-  camera_ids: how errors name the cameras (default: their position in cam_views)."""
+def init_views(boards, cam_views, image_sizes, model="standard", fix_aspect=False, engine=None):
+  """mcba_intrinsic_init for each camera's list of views: (K0 [C, 5+nd], initial board-wrt-camera poses [C,F,B,4,4], ok [C,F,B]),
+  indexed by the views' (frame, board)."""
   eng = engine or intrinsics_engine()
-  opts = dict(ftol=1e-10, xtol=1e-10, gtol=1e-10, max_nfev=100)
-  opts.update(solve_opts)
   board_points = stack_boards(boards)[0].astype(np.float32).astype(np.float64)
   F = max(max((v.frame for v in views), default=0) for views in cam_views) + 1
   B, P = board_points.shape[:2]
@@ -124,15 +128,27 @@ def calibrate_views(boards, cam_views, image_sizes, model="standard", fix_aspect
   det_xy = np.concatenate([t[3].corners.astype(np.float64) for t in order]) if order else np.zeros((0, 2))
   use = counts.reshape(Cn, F, B) > 0
   grid = np.array([[1, 1, 1, 0, 0]] * B, np.int32)              # the views are chosen already: no minimum-detections rule on the device
-  k0, poses, ok = eng.intrinsic_init(model, (Cn, F, B, P), det_start, det_ids, det_xy, board_points, grid, image_sizes, use, fix_aspect)
+  return eng.intrinsic_init(model, (Cn, F, B, P), det_start, det_ids, det_xy, board_points, grid, image_sizes, use, fix_aspect)
+
+
+def calibrate_views(boards, cam_views, image_sizes, model="standard", fix_aspect=False, engine=None, camera_ids=None, **solve_opts):
+  """One calibrateCameraExtended (model "fisheye": one cv2.fisheye.calibrate) for each camera's list of views (calibration_points
+  entries, any order): returns per camera a struct of the intrinsics [fx fy cx cy skew dist...], the views' rtvecs (board wrt camera),
+  per-view RMS, total RMS, K0 and the solve summary.  camera_ids: how errors name the cameras (default: their position in cam_views)."""
+  eng = engine or intrinsics_engine()
+  opts = dict(ftol=1e-10, xtol=1e-10, gtol=1e-10, max_nfev=100)
+  opts.update(solve_opts)
+  board_points = stack_boards(boards)[0].astype(np.float32).astype(np.float64)
+  k0, poses, ok = init_views(boards, cam_views, image_sizes, model, fix_aspect, eng)
   out = []
   names = list(range(len(cam_views))) if camera_ids is None else list(camera_ids)
   for c, views in enumerate(cam_views):
     if not np.isfinite(k0[c]).all():
       raise ValueError(f"camera {names[c]}: no initial camera matrix (degenerate homographies)")
     sel = [(v.frame, v.board) for v in views]
-    if not all(ok[c, f, b] for f, b in sel):
-      raise ValueError(f"camera {names[c]}: the initial pose of a view failed")
+    failed = [(f, b) for f, b in sel if not ok[c, f, b]]
+    if failed:
+      raise ValueError(f"camera {names[c]}: the initial pose of the view (frame {failed[0][0]}, board {failed[0][1]}) failed")
     res = _solve_camera(eng, model, fix_aspect, views, k0[c], np.stack([poses[c, f, b] for f, b in sel]), board_points, opts)
     res.k0 = k0[c]
     out.append(res)
@@ -190,4 +206,44 @@ def calibrate(boards, intrinsic_error_limit, detections, image_size, max_iter=10
   """Camera.calibrate (camera.py:68-105) for one camera's detections[frame][board]: (Camera, err)."""
   cams, errs = calibrate_cameras(boards, [detections], [image_size], intrinsic_error_limit, max_iter=max_iter, eps=eps, model=model,
                                  fix_aspect=fix_aspect, has_skew=has_skew, flags=flags, max_images=max_images, **solve_opts)
+  return cams[0], errs[0]
+
+
+def calibrate_cameras_fisheye(boards, points, image_sizes, max_iter=10, eps=1e-3, model="standard", fix_aspect=False, has_skew=False,
+                              flags=0, max_images=None, **solve_opts):
+  """camera_fisheye.py:173-177: (cameras, errs) for the nested detections points[camera][frame][board], one cv2.fisheye.calibrate per
+  camera (camera_fisheye.py:70-94) with CALIB_RECOMPUTE_EXTRINSIC | CALIB_FIX_SKEW: no rejection loop, no error limit.  The start is
+  OpenCV's (mcba_intrinsic_init with the fisheye model, one launch for all cameras), the solve the same engine problem as the pinhole
+  path's without an aspect constraint, err the total RMS sqrt(sum |e|^2 / corners).  `model` (fix_k1..fix_k4) and `fix_aspect` are only
+  stored on the cameras, as the reference never passes them to OpenCV; `max_iter` / `eps` are accepted for the signature (the device
+  solves to its own tolerances, module docstring).  With max_images, the np.random draws run camera by camera in order (the reference
+  draws them from a thread pool, in whatever order its threads run)."""
+  from .camera import CameraFisheye
+  del max_iter, eps
+  assert model in FISHEYE_MODELS, f"unknown camera model {model} options are {list(FISHEYE_MODELS)}"
+  if flags:
+    raise NotImplementedError(f"extra OpenCV calibration flags ({flags}) are not supported")
+  views = []
+  for c in range(len(points)):
+    v = calibration_points(boards, points[c])
+    if not v:
+      raise ValueError(f"camera {c}: no view with the minimum detections of its board")
+    if max_images is not None:
+      v = top_detection_coverage(v, max_images, image_sizes[c])
+    views.append(v)
+  res = calibrate_views(boards, views, image_sizes, model="fisheye", fix_aspect=False, **solve_opts)
+  cams = []
+  for r, size in zip(res, image_sizes):
+    x = r.intrinsics
+    K = np.array([[x[0], 0.0, x[2]], [0.0, x[1], x[3]], [0.0, 0.0, 1.0]])
+    cams.append(CameraFisheye(image_size=tuple(size), intrinsic=K, dist=x[5:9].reshape(4, 1).copy(), model=model, fix_aspect=fix_aspect,
+                              has_skew=has_skew))
+  return cams, [r.rms for r in res]
+
+
+def calibrate_fisheye(boards, detections, image_size, max_iter=10, eps=1e-3, model="standard", fix_aspect=False, has_skew=False, flags=0,
+                      max_images=None, **solve_opts):
+  """CameraFisheye.calibrate (camera_fisheye.py:70-94) for one camera's detections[frame][board]: (CameraFisheye, err)."""
+  cams, errs = calibrate_cameras_fisheye(boards, [detections], [image_size], max_iter=max_iter, eps=eps, model=model,
+                                         fix_aspect=fix_aspect, has_skew=has_skew, flags=flags, max_images=max_images, **solve_opts)
   return cams[0], errs[0]

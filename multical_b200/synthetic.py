@@ -118,8 +118,9 @@ def _boards(kind, w, h, square, count, rng):
 
 def make_scene(C=2, F=20, boards=("charuco", 16, 22, 0.025, 1), model="standard", vis=0.5,
                rig="arc", noise=0.3, seed=0, pose_jitter=0.01, intrinsic_jitter=0.0,
-               image_size=(1920, 1080), outlier_fraction=0.0, frame_chunk=64):
-  """Returns the scene dict described in the module docstring. Deterministic in `seed`."""
+               image_size=(1920, 1080), outlier_fraction=0.0, frame_chunk=64, focal=None):
+  """Returns the scene dict described in the module docstring. Deterministic in `seed`.  focal: the nominal focal length in pixels
+  (default 1200, fisheye 900)."""
   rng = np.random.default_rng(seed)
   kind, w, h, square, nb = boards
   board_points, board_poses, side = _boards(kind, w, h, square, nb, rng)
@@ -148,7 +149,7 @@ def make_scene(C=2, F=20, boards=("charuco", 16, 22, 0.025, 1), model="standard"
     cam_poses.append(look_at(eye, target + rng.normal(0, 0.02, 3)))
   cam_poses = np.stack(cam_poses)
 
-  f0 = 1200.0 if model != "fisheye" else 900.0
+  f0 = focal if focal is not None else 1200.0 if model != "fisheye" else 900.0
   K = np.tile(np.eye(3), (C, 1, 1))
   K[:, 0, 0] = f0 * (1 + rng.normal(0, 0.01, C)); K[:, 1, 1] = K[:, 0, 0] * (1 + rng.normal(0, 0.002, C))
   K[:, 0, 2] = W / 2 + rng.normal(0, 5, C); K[:, 1, 2] = H / 2 + rng.normal(0, 5, C)

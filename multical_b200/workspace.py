@@ -1,7 +1,7 @@
 """The `Workspace` methods around the hot path, as functions over a `Calibration` or the detections (the rest of the reference's
 `Workspace` -- image loading, detection, export -- is out of scope and stays the reference's own):
-  calibrate_single(boards, detected_points, ...)   = Workspace.calibrate_single   multical/workspace.py:165-194 (the pinhole branch:
-                                    every camera's intrinsics, multical_b200/intrinsics.py)
+  calibrate_single(boards, detected_points, ...)   = Workspace.calibrate_single   multical/workspace.py:165-194 (the pinhole and,
+                                    with isFisheye, the fisheye branch: every camera's intrinsics, multical_b200/intrinsics.py)
 
   calibrate(calib, ...)          = Workspace.calibrate          multical/workspace.py:228-247  (enable the chosen blocks, then the outlier
                                     loop around bundle_adjust with the quantile selectors the command line builds, config/workspace.py:47-58)
@@ -15,7 +15,7 @@ package (INTEGRATION.md A, D); these functions are the same steps for callers th
 import numpy as np
 
 from .calibration import Calibration, select_threshold
-from .intrinsics import calibrate_cameras
+from .intrinsics import calibrate_cameras, calibrate_cameras_fisheye
 from .log import info
 from .nonoverlap import HandEye
 from .parameters import ParamList
@@ -24,8 +24,12 @@ from .tables import initialise_poses as _initialise_poses, make_pose_table
 
 
 def calibrate_single(boards, detected_points, image_sizes, camera_model, intrinsic_error_limit, fix_aspect=False, has_skew=False,
-                     max_images=None):
-  """workspace.py:165-180 (the pinhole branch): every camera's intrinsics from its detections[frame][board] -> (cameras, errs)."""
+                     max_images=None, isFisheye=False):
+  """workspace.py:165-189: every camera's intrinsics from its detections[frame][board] -> (cameras, errs).  isFisheye routes to
+  calibrate_cameras_fisheye, which takes no error limit (CameraOpts.isFisheye, config/arguments.py:36)."""
+  if isFisheye:
+    return calibrate_cameras_fisheye(boards, detected_points, image_sizes, model=camera_model, fix_aspect=fix_aspect, has_skew=has_skew,
+                                     max_images=max_images)
   return calibrate_cameras(boards, detected_points, image_sizes, intrinsic_error_limit, model=camera_model, fix_aspect=fix_aspect,
                            has_skew=has_skew, max_images=max_images)
 
