@@ -30,7 +30,9 @@ EXPORTS = ["mcba_create", "mcba_destroy", "mcba_last_error", "mcba_set_stream", 
            "mcba_table_upload", "mcba_table_from_detections", "mcba_table_download", "mcba_table_set_inliers",
            "mcba_table_get_inliers", "mcba_table_select", "mcba_pnp_views", "mcba_table_errors", "mcba_table_error_ranks", "mcba_table_count_below", "mcba_table_reject",
            "mcba_intrinsic_init", "mcba_view_errors", "mcba_pose_pairs", "mcba_pose_times", "mcba_pose_cluster",
-           "mcba_hand_eye_quads", "mcba_hand_eye_vote"]
+           "mcba_hand_eye_quads", "mcba_hand_eye_vote", "mcba_undistort_map", "mcba_undistort_images", "mcba_project_points",
+           "mcba_undistort_points", "mcba_remap_cubic_table"]
+IMAGE_UINT8 = 0          # include/mcba.h MCBA_IMAGE_UINT8
 TABLE_VALID, TABLE_INLIERS = 0, 1
 
 
@@ -129,6 +131,12 @@ def load():
   lib.mcba_pose_cluster.argtypes = [P, i32, I64, D, U8]
   lib.mcba_hand_eye_quads.argtypes = [P, i32, i32, i32, D, U8, i32, I32, D, D, I32, U8]
   lib.mcba_hand_eye_vote.argtypes = [P, i32, I64, D, D, I32]
+  U8P = C.POINTER(U8)
+  lib.mcba_undistort_map.argtypes = [P, i32, D, i32, i32, C.POINTER(C.c_float)]
+  lib.mcba_undistort_images.argtypes = [P, i32, D, i32, i32, i32, i32, i32, i32, i32, U8P, U8P]
+  lib.mcba_project_points.argtypes = [P, i32, D, C.c_int64, D, D]
+  lib.mcba_undistort_points.argtypes = [P, i32, D, C.c_int64, D, D]
+  lib.mcba_remap_cubic_table.argtypes = [P, I32]
   _lib = lib
   return lib
 

@@ -59,6 +59,22 @@ class Camera(Parameters):
     K = np.array([[fx, skew, px], [0, fy, py], [0, 0, 1]], np.float64)
     return self.copy(intrinsic=K, dist=params["dist"])
 
+  @cached_property
+  def undistort_map(self):
+    """camera.py:113-117 on the GPU (multical_b200/undistort.py): float32 [h, w, 2] of cv2.initUndistortRectifyMap with R = I, newK = K."""
+    from .undistort import undistort_map
+    return undistort_map(self)
+
+  def undistort_points(self, points):
+    """camera.py:119-122 on the GPU: cv2.undistortPoints(points, K, dist, P=K) over any leading shape [..., 2]."""
+    from .undistort import undistort_points
+    return undistort_points(self, points)
+
+  def project(self, points):
+    """camera.py:124-128 on the GPU: cv2.projectPoints of camera-frame points [..., 3] with rvec = tvec = 0 -> pixels [..., 2]."""
+    from .undistort import project
+    return project(self, points)
+
   def approx_eq(self, other):
     return self.image_size == other.image_size and np.allclose(other.intrinsic, self.intrinsic) and np.allclose(other.dist, self.dist)
 
@@ -103,6 +119,12 @@ def calibrate_cameras_fisheye(boards, points, image_sizes, **kwargs):
   """camera_fisheye.py:173-177 on the GPU (multical_b200/intrinsics.py): (cameras, errs)."""
   from .intrinsics import calibrate_cameras_fisheye
   return calibrate_cameras_fisheye(boards, points, image_sizes, **kwargs)
+
+
+def undistort_images(images, cameras, j=None, chunksize=4):
+  """camera.py:247-258 on the GPU (multical_b200/undistort.py): per camera, its images remapped through its undistortion map."""
+  from .undistort import undistort_images
+  return undistort_images(images, cameras, j=j, chunksize=chunksize)
 
 
 def engine_model_of(camera):

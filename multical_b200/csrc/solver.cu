@@ -11,6 +11,7 @@
 #include <string>
 #include <chrono>
 #include <type_traits>
+#include <memory>
 #include <vector>
 
 #include "../../include/mcba.h"
@@ -23,6 +24,7 @@
 #include "intrinsics_kernels.cuh"
 #include "pose_init_kernels.cuh"
 #include "hand_eye_init_kernels.cuh"
+#include "undistort_kernels.cuh"
 
 using namespace mcba;
 
@@ -43,6 +45,24 @@ struct DevBuf {
     return cudaMalloc(&p, n * sizeof(T));
   }
 };
+
+// page-locked host staging (plain host memory on the test-suite's interpreter build, which has no pinned allocator)
+cudaError_t host_alloc(uint8_t** p, size_t bytes) {
+#ifdef MCBA_SIMT_BUILD
+  *p = (uint8_t*)malloc(bytes);
+  return *p ? cudaSuccess : cudaErrorMemoryAllocation;
+#else
+  return cudaMallocHost((void**)p, bytes);
+#endif
+}
+void host_free(uint8_t* p) {
+  if (!p) return;
+#ifdef MCBA_SIMT_BUILD
+  free(p);
+#else
+  cudaFreeHost(p);
+#endif
+}
 
 // The parameter state is one block of doubles, [cam_rt 6C | board_rt 6B | frame_rt F fbs | intr kint C | he_rt 12 | board_pts 3BP] with
 // fbs = max(fb, 6) doubles per frame: the current state (ctx->params) and the trial state (ctx->trial: what k_lm proposes, k_linearize
@@ -148,6 +168,20 @@ struct mcba_ctx {
   struct HandEyeInitBuffers {
     DevBuf<double> poses, X, Z, points, density; DevBuf<uint8_t> valid, ok; DevBuf<int32_t> quads, n_images, best; DevBuf<int64_t> start;
   } heinit;
+  // applying a calibration (mcba_undistort_* / mcba_project_points): the cubic weight table, the resident maps of recent cameras
+  // (fixed-point form, least recently used dropped first), the optional float map, points, and per-stream pinned staging for images
+  struct UndistortMap {
+    int model = -1, w = 0, h = 0; std::vector<double> cam; DevBuf<uint32_t> org; DevBuf<uint16_t> idx; uint64_t used = 0;
+  };
+  static constexpr int UND_STREAMS = 3, UND_MAX_MAPS = 64;
+  struct UndistortBuffers {
+    DevBuf<int32_t> tab; bool tab_ready = false;
+    std::vector<std::unique_ptr<UndistortMap>> maps; uint64_t tick = 0;
+    DevBuf<float2> fmap; DevBuf<double> pin, pout;
+    cudaStream_t st[UND_STREAMS] = {}; cudaEvent_t done[UND_STREAMS] = {}, map_ready = nullptr;
+    uint8_t* host_in[UND_STREAMS] = {}; uint8_t* host_out[UND_STREAMS] = {}; size_t host_in_cap = 0, host_out_cap = 0;
+    DevBuf<uint8_t> dev_in[UND_STREAMS], dev_out[UND_STREAMS];
+  } und;
 };
 
 #define CK(call)                                                                                   \
@@ -692,6 +726,13 @@ void mcba_destroy(mcba_ctx* ctx) {
   if (ctx->copy_done) cudaEventDestroy(ctx->copy_done);
   if (ctx->copy_go) cudaEventDestroy(ctx->copy_go);
   if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
+  for (int i = 0; i < mcba_ctx::UND_STREAMS; i++) {
+    auto& U = ctx->und;
+    if (U.st[i]) { cudaStreamSynchronize(U.st[i]); cudaStreamDestroy(U.st[i]); }
+    if (U.done[i]) cudaEventDestroy(U.done[i]);
+    host_free(U.host_in[i]); host_free(U.host_out[i]);
+  }
+  if (ctx->und.map_ready) cudaEventDestroy(ctx->und.map_ready);
   cudaStream_t own = ctx->own_stream;
   delete ctx;                            // device buffers are freed by their destructors
   if (own) cudaStreamDestroy(own);
@@ -1398,6 +1439,211 @@ int mcba_hand_eye_vote(mcba_ctx* ctx, int32_t n_sets, const int64_t* set_start, 
   CK(cudaStreamSynchronize(s));
   for (int k = 0; k < n_sets; k++)
     REQUIRE(best[k] >= 0, MCBA_ERR_DEGENERATE, "set " + std::to_string(k) + " has a singular covariance");
+  return MCBA_OK;
+}
+
+namespace {
+
+// the camera of the undistortion entries: [fx fy cx cy skew dist...] with 5 + nd values of `model`
+int check_camera(mcba_ctx* ctx, int32_t model, const double* camera) {
+  REQUIRE(model >= MODEL_STANDARD && model <= MODEL_TILTED, MCBA_ERR_ARG, "unknown camera model");
+  REQUIRE(camera, MCBA_ERR_ARG, "null camera");
+  REQUIRE(all_finite(camera, 5 + (size_t)model_nd(model)), MCBA_ERR_NONFINITE, "non-finite camera parameter");
+  REQUIRE(camera[0] != 0.0 && camera[1] != 0.0, MCBA_ERR_ARG, "zero focal length");
+  return MCBA_OK;
+}
+
+UndistortCamera make_camera(int model, const double* camera, int w, int h) {
+  UndistortCamera c{};
+  for (int i = 0; i < 5 + model_nd(model); i++) c.k[i] = camera[i];
+  for (int i = 0; i < 9; i++) c.tilt[i] = (i % 4 == 0) ? 1.0 : 0.0;
+  if (model == MODEL_TILTED) { double dMx[9], dMy[9]; tilt_matrices(camera[5 + 12], camera[5 + 13], c.tilt, dMx, dMy); }
+  c.w = w; c.h = h;
+  return c;
+}
+
+// the bicubic weight table, built on the context stream at first use
+int ensure_cubic_table(mcba_ctx* ctx) {
+  auto& U = ctx->und;
+  if (U.tab_ready) return MCBA_OK;
+  CK(U.tab.alloc(16 * (size_t)UND_TAB_ENTRIES));
+  k_cubic_table<<<(UND_TAB_ENTRIES + UND_THREADS - 1) / UND_THREADS, UND_THREADS, 0, ctx->stream>>>(U.tab.p); CKL();
+  U.tab_ready = true;
+  return MCBA_OK;
+}
+
+// the resident fixed-point map of a camera, computed on ctx->stream when it is not resident yet (or when the float map is asked for)
+int resident_map(mcba_ctx* ctx, int model, const double* camera, int w, int h, float* map_out, mcba_ctx::UndistortMap** out) {
+  auto& U = ctx->und;
+  cudaStream_t s = ctx->stream;
+  { int r = ensure_cubic_table(ctx); if (r) return r; }
+  const size_t nk = 5 + (size_t)model_nd(model), npx = (size_t)w * h;
+  mcba_ctx::UndistortMap* m = nullptr;
+  for (auto& e : U.maps)
+    if (e->model == model && e->w == w && e->h == h && std::memcmp(e->cam.data(), camera, nk * sizeof(double)) == 0) m = e.get();
+  if (!m || map_out) {
+    if (!m) {
+      if (U.maps.size() >= (size_t)mcba_ctx::UND_MAX_MAPS) {
+        auto lru = std::min_element(U.maps.begin(), U.maps.end(), [](const auto& a, const auto& b) { return a->used < b->used; });
+        CK(cudaStreamSynchronize(s));              // its buffers may still be read by work in flight
+        U.maps.erase(lru);
+      }
+      U.maps.emplace_back(new mcba_ctx::UndistortMap());
+      m = U.maps.back().get();
+      CK(m->org.alloc(npx)); CK(m->idx.alloc(npx));
+    }
+    float2* f = nullptr;
+    if (map_out) { CK(U.fmap.alloc(npx)); f = U.fmap.p; }
+    const UndistortCamera c = make_camera(model, camera, w, h);
+    const dim3 grid((w + UND_THREADS - 1) / UND_THREADS, h);
+    with_model(model, false, [&](auto M, auto) {
+      k_undistort_map<decltype(M)::value><<<grid, UND_THREADS, 0, s>>>(c, f, m->org.p, m->idx.p);
+    });
+    m->model = -1;                                 // not usable until the launch is known to have gone in
+    CKL();
+    m->model = model; m->w = w; m->h = h; m->cam.assign(camera, camera + nk);
+    if (map_out) {
+      CK(cudaMemcpyAsync(map_out, f, sizeof(float2) * npx, cudaMemcpyDeviceToHost, s));
+      CK(cudaStreamSynchronize(s));
+    }
+  }
+  m->used = ++U.tick;
+  *out = m;
+  return MCBA_OK;
+}
+
+// point entries: copy in, one thread per point, copy out
+int run_points(mcba_ctx* ctx, bool project, int32_t model, const double* camera, int64_t n, const double* in, double* out) {
+  if (!ctx) return MCBA_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  { int r = check_camera(ctx, model, camera); if (r) return r; }
+  REQUIRE(n >= 0, MCBA_ERR_ARG, "negative point count");
+  if (n == 0) return MCBA_OK;
+  REQUIRE(in && out, MCBA_ERR_ARG, "null argument");
+  auto& U = ctx->und;
+  cudaStream_t s = ctx->stream;
+  const size_t din = project ? 3 : 2;
+  CK(U.pin.alloc(din * n)); CK(U.pout.alloc(2 * (size_t)n));
+  CK(cudaMemcpyAsync(U.pin.p, in, sizeof(double) * din * n, cudaMemcpyHostToDevice, s));
+  const UndistortCamera c = make_camera(model, camera, 0, 0);
+  const unsigned blocks = (unsigned)((n + UND_THREADS - 1) / UND_THREADS);
+  with_model(model, false, [&](auto M, auto) {
+    constexpr int MODEL = decltype(M)::value;
+    if (project) k_project_points<MODEL><<<blocks, UND_THREADS, 0, s>>>(c, n, U.pin.p, U.pout.p);
+    else k_undistort_points<MODEL><<<blocks, UND_THREADS, 0, s>>>(c, n, U.pin.p, U.pout.p);
+  });
+  CKL();
+  CK(cudaMemcpyAsync(out, U.pout.p, sizeof(double) * 2 * n, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  return MCBA_OK;
+}
+
+}  // namespace
+
+// initUndistortRectifyMap(K, dist, None, K, (width, height)) of one camera, kept resident for mcba_undistort_images
+int mcba_undistort_map(mcba_ctx* ctx, int32_t model, const double* camera, int32_t width, int32_t height, float* map) {
+  if (!ctx) return MCBA_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  { int r = check_camera(ctx, model, camera); if (r) return r; }
+  REQUIRE(width > 0 && height > 0 && height <= 65535, MCBA_ERR_ARG, "map size out of range");
+  mcba_ctx::UndistortMap* m = nullptr;
+  int r = resident_map(ctx, model, camera, width, height, map, &m);
+  if (r) return r;
+  CK(cudaStreamSynchronize(ctx->stream));
+  return MCBA_OK;
+}
+
+// cv2.remap(src[i], map, None, INTER_CUBIC) for n images of one camera, host to host.  Chunks of images go through pinned staging
+// on UND_STREAMS streams in turn: while the host copies one chunk into its staging buffer, earlier chunks are in flight (copy in,
+// k_remap_cubic, copy out) on the other streams.
+int mcba_undistort_images(mcba_ctx* ctx, int32_t model, const double* camera, int32_t width, int32_t height, int32_t n,
+                          int32_t src_width, int32_t src_height, int32_t channels, int32_t dtype, const uint8_t* const* src,
+                          uint8_t* const* dst) {
+  if (!ctx) return MCBA_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  { int r = check_camera(ctx, model, camera); if (r) return r; }
+  REQUIRE(dtype == MCBA_IMAGE_UINT8, MCBA_ERR_ARG, "unsupported image dtype: only 8-bit unsigned images are remapped");
+  REQUIRE(channels == 1 || channels == 3, MCBA_ERR_ARG, "unsupported channel count: 1 or 3 channels are remapped");
+  REQUIRE(width > 0 && height > 0 && height <= 65535, MCBA_ERR_ARG, "map size out of range");
+  REQUIRE(src_width > 0 && src_height > 0, MCBA_ERR_ARG, "empty source image");
+  REQUIRE(n >= 0, MCBA_ERR_ARG, "negative image count");
+  if (n == 0) return MCBA_OK;
+  REQUIRE(src && dst, MCBA_ERR_ARG, "null image list");
+  for (int i = 0; i < n; i++) REQUIRE(src[i] && dst[i], MCBA_ERR_ARG, "null image " + std::to_string(i));
+  mcba_ctx::UndistortMap* m = nullptr;
+  { int r = resident_map(ctx, model, camera, width, height, nullptr, &m); if (r) return r; }
+  auto& U = ctx->und;
+  const size_t in_bytes = (size_t)src_width * src_height * channels, out_bytes = (size_t)width * height * channels;
+  const size_t chunk_bytes = (size_t)8 << 20;
+  const int per_chunk = (int)std::max<size_t>(1, std::min<size_t>((size_t)n, chunk_bytes / std::max(in_bytes, out_bytes)));
+  const int n_chunks = (n + per_chunk - 1) / per_chunk;
+  const int n_slots = std::min(mcba_ctx::UND_STREAMS, n_chunks);
+  if (!U.map_ready) CK(cudaEventCreateWithFlags(&U.map_ready, cudaEventDisableTiming));
+  if (U.host_in_cap < per_chunk * in_bytes || U.host_out_cap < per_chunk * out_bytes) {
+    for (int i = 0; i < mcba_ctx::UND_STREAMS; i++) {
+      if (U.st[i]) CK(cudaStreamSynchronize(U.st[i]));
+      host_free(U.host_in[i]); host_free(U.host_out[i]);
+      U.host_in[i] = U.host_out[i] = nullptr;
+    }
+    U.host_in_cap = std::max(U.host_in_cap, per_chunk * in_bytes);
+    U.host_out_cap = std::max(U.host_out_cap, per_chunk * out_bytes);
+  }
+  for (int i = 0; i < n_slots; i++) {
+    if (!U.st[i]) CK(cudaStreamCreateWithFlags(&U.st[i], cudaStreamNonBlocking));
+    if (!U.done[i]) CK(cudaEventCreateWithFlags(&U.done[i], cudaEventDisableTiming));
+    if (!U.host_in[i]) CK(host_alloc(&U.host_in[i], U.host_in_cap));
+    if (!U.host_out[i]) CK(host_alloc(&U.host_out[i], U.host_out_cap));
+    CK(U.dev_in[i].alloc(per_chunk * in_bytes)); CK(U.dev_out[i].alloc(per_chunk * out_bytes));
+  }
+  CK(cudaEventRecord(U.map_ready, ctx->stream));           // the map (and table) are written on the context stream
+  for (int i = 0; i < n_slots; i++) CK(cudaStreamWaitEvent(U.st[i], U.map_ready, 0));
+  RemapArgs a{};
+  a.org = m->org.p; a.idx = m->idx.p; a.tab = U.tab.p; a.ws = src_width; a.hs = src_height; a.wm = width; a.hm = height;
+  std::vector<int> pending(n_slots, -1);                    // chunk whose results a slot holds
+  auto drain = [&](int slot) -> int {
+    const int ck = pending[slot];
+    if (ck < 0) return MCBA_OK;
+    CK(cudaEventSynchronize(U.done[slot]));
+    const int first = ck * per_chunk, cnt = std::min(per_chunk, n - first);
+    for (int j = 0; j < cnt; j++) std::memcpy(dst[first + j], U.host_out[slot] + j * out_bytes, out_bytes);
+    pending[slot] = -1;
+    return MCBA_OK;
+  };
+  for (int ck = 0; ck < n_chunks; ck++) {
+    const int slot = ck % n_slots, first = ck * per_chunk, cnt = std::min(per_chunk, n - first);
+    { int r = drain(slot); if (r) return r; }
+    for (int j = 0; j < cnt; j++) std::memcpy(U.host_in[slot] + j * in_bytes, src[first + j], in_bytes);
+    cudaStream_t s = U.st[slot];
+    CK(cudaMemcpyAsync(U.dev_in[slot].p, U.host_in[slot], cnt * in_bytes, cudaMemcpyHostToDevice, s));
+    a.src = U.dev_in[slot].p; a.dst = U.dev_out[slot].p;
+    const dim3 grid((width + UND_THREADS - 1) / UND_THREADS, height, cnt);
+    if (channels == 1) k_remap_cubic<1><<<grid, UND_THREADS, 0, s>>>(a);
+    else k_remap_cubic<3><<<grid, UND_THREADS, 0, s>>>(a);
+    CKL();
+    CK(cudaMemcpyAsync(U.host_out[slot], U.dev_out[slot].p, cnt * out_bytes, cudaMemcpyDeviceToHost, s));
+    CK(cudaEventRecord(U.done[slot], s));
+    pending[slot] = ck;
+  }
+  for (int k = 0; k < n_slots; k++) { int r = drain((n_chunks + k) % n_slots); if (r) return r; }
+  return MCBA_OK;
+}
+
+int mcba_project_points(mcba_ctx* ctx, int32_t model, const double* camera, int64_t n, const double* points, double* pixels) {
+  return run_points(ctx, true, model, camera, n, points, pixels);
+}
+
+int mcba_undistort_points(mcba_ctx* ctx, int32_t model, const double* camera, int64_t n, const double* pixels, double* undistorted) {
+  return run_points(ctx, false, model, camera, n, pixels, undistorted);
+}
+
+// the fixed-point bicubic weights k_remap_cubic reads, int32[1024][16]
+int mcba_remap_cubic_table(mcba_ctx* ctx, int32_t* table) {
+  if (!ctx || !table) return MCBA_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  auto& U = ctx->und;
+  { int r = ensure_cubic_table(ctx); if (r) return r; }
+  CK(cudaMemcpyAsync(table, U.tab.p, sizeof(int32_t) * 16 * UND_TAB_ENTRIES, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
   return MCBA_OK;
 }
 

@@ -268,6 +268,62 @@ class Engine:
                                          nat.iptr(best)))
     return [dens[a:b] for a, b in zip(start[:-1], start[1:])], best[:len(sets)]
 
+  # ---- applying a calibration (include/mcba.h mcba_undistort_* / mcba_project_points) ---------------------------------------------
+  def _camera(self, model, camera):
+    cam = nat.f64(camera).reshape(-1)
+    assert cam.size == 5 + nat.DIST_SIZES[model], f"camera model {model} takes {5 + nat.DIST_SIZES[model]} parameters, got {cam.size}"
+    return nat.MODEL_IDS[model], cam
+
+  def undistort_map(self, model, camera, size, want_map=True):
+    """initUndistortRectifyMap(K, dist, None, K, size) of camera [fx fy cx cy skew dist...]: the map stays resident on the device;
+    returns it as float32 [h, w, 2] (None with want_map=False)."""
+    mid, cam = self._camera(model, camera)
+    w, h = (int(v) for v in size)
+    out = np.empty((h, w, 2), np.float32) if want_map else None
+    self._ck(self.lib.mcba_undistort_map(self.h, mid, nat.dptr(cam), w, h,
+                                         None if out is None else out.ctypes.data_as(C.POINTER(C.c_float))))
+    return out
+
+  def undistort_images(self, model, camera, size, images):
+    """cv2.remap(image, map, None, INTER_CUBIC) for a list of same-shape uint8 images [hs, ws] or [hs, ws, 3] of one camera, with the
+    camera's resident map of `size` = (w, h): a list of uint8 [h, w] or [h, w, 3] arrays."""
+    mid, cam = self._camera(model, camera)
+    w, h = (int(v) for v in size)
+    if len(images) == 0: return []
+    src = [np.ascontiguousarray(im) for im in images]
+    shape, dtype = src[0].shape, src[0].dtype
+    assert all(im.shape == shape and im.dtype == dtype for im in src), "images of one camera must share one shape and dtype"
+    channels = 1 if len(shape) == 2 else shape[2]
+    dt = nat.IMAGE_UINT8 if dtype == np.uint8 else -1
+    out_shape = (h, w) if len(shape) == 2 or channels == 1 else (h, w, channels)
+    dst = [np.empty(out_shape, np.uint8) for _ in src]
+    U8 = C.POINTER(C.c_uint8)
+    sp, dp = (U8 * len(src))(*[im.ctypes.data_as(U8) for im in src]), (U8 * len(dst))(*[im.ctypes.data_as(U8) for im in dst])
+    self._ck(self.lib.mcba_undistort_images(self.h, mid, nat.dptr(cam), w, h, len(src), shape[1], shape[0], channels, dt, sp, dp))
+    return dst
+
+  def project_points(self, model, camera, points):
+    """cv2.projectPoints(points, 0, 0, K, dist) (fisheye: cv2.fisheye.projectPoints): camera-frame f64 [n, 3] -> pixels f64 [n, 2]."""
+    mid, cam = self._camera(model, camera)
+    pts = nat.f64(points).reshape(-1, 3)
+    out = np.zeros((max(len(pts), 1), 2))
+    self._ck(self.lib.mcba_project_points(self.h, mid, nat.dptr(cam), len(pts), nat.dptr(pts), nat.dptr(out)))
+    return out[:len(pts)]
+
+  def undistort_points(self, model, camera, pixels):
+    """cv2.undistortPoints(pixels, K, dist, P=K) (fisheye: cv2.fisheye.undistortPoints): f64 [n, 2] -> f64 [n, 2]."""
+    mid, cam = self._camera(model, camera)
+    pts = nat.f64(pixels).reshape(-1, 2)
+    out = np.zeros((max(len(pts), 1), 2))
+    self._ck(self.lib.mcba_undistort_points(self.h, mid, nat.dptr(cam), len(pts), nat.dptr(pts), nat.dptr(out)))
+    return out[:len(pts)]
+
+  def remap_cubic_table(self):
+    """The fixed-point bicubic weights of the remap, int32 [1024, 16] (include/mcba.h mcba_remap_cubic_table)."""
+    tab = np.zeros((1024, 16), np.int32)
+    self._ck(self.lib.mcba_remap_cubic_table(self.h, nat.iptr(tab)))
+    return tab
+
   def view_errors(self):
     """Per-view sums of squared pixel errors and corner counts of the uploaded problem at the current parameters, both [C,F,B]
     (zero where there is no view): include/mcba.h mcba_view_errors."""
