@@ -27,6 +27,7 @@ constexpr int LIN_MAXB = 8;            // board pose tables staged per frame (mo
 constexpr int LIN_TSTR = 12;           // row stride of T^t in the epilogue (stride mod 16 == 12: conflict-free fragment loads)
 constexpr int LIN_VC = 44;             // per-warp view constants: 12 doubles per chain + the intrinsics
 constexpr int LIN_WB_FLAG = 0x4000;    // scatter-table entry: add the view's board offset (rows of W_f that belong to board b)
+constexpr int LIN_SMEM_MAX = 220 * 1024;   // dynamic shared memory of a CTA at most (bytes; the static part and the per-CTA reserve fit beside it)
 
 // compile-time shape of a residual row's local Jacobian [twist block(s) | fx fy cx cy dist | r]
 template <int MODEL, bool ROLL>
@@ -698,7 +699,9 @@ struct ReduceArgs {
   unsigned* cam_counter;                      // [C + 1]: slices done per camera | cameras done
 };
 __host__ __device__ inline int reduce_slices(int rec) { return (rec + RED_ENT - 1) / RED_ENT; }
-__host__ __device__ inline size_t reduce_smem_doubles(int T, int D, int B) { return (size_t)lin_record_doubles(T, D, B) + D * 6 + 36; }
+// the camera's moment sum | Um | Ac: the per-board parts of the record are read from `sred` where they are used, so that the CTA's
+// shared memory does not grow with the board count
+__host__ __device__ inline size_t reduce_smem_doubles(int T, int D) { return (size_t)T + D * 6 + 36; }
 
 template <int NP>
 __global__ void __launch_bounds__(RED_THREADS)
@@ -746,10 +749,10 @@ k_reduce_shared(DeviceProblem p, ReduceArgs a) {
   if (tid == 0) a.cam_counter[c] = 0;
   __threadfence();
   // ---- step 2: this camera's blocks
-  double* Msum = rsm;                         // [T] then per board [UB]
-  double* Um = rsm + rec;                     // [D][6]
+  double* Msum = rsm;                         // [T]
+  double* Um = rsm + T;                       // [D][6]
   double* Ac = Um + D * 6;                    // 36
-  for (int i = tid; i < rec; i += RED_THREADS) Msum[i] = __ldcg(&a.sred[(size_t)c * rec + i]);
+  for (int i = tid; i < T; i += RED_THREADS) Msum[i] = __ldcg(&a.sred[(size_t)c * rec + i]);
   if (tid == 0) { const PoseT& pc = p.cam_T[c]; const double I3[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1}; twist_map(I3, pc.JL, pc.t, Ac); }
   __syncthreads();
   for (int o = tid; o < D * 6; o += RED_THREADS) {       // Um = sum_a Msum[:, xi_a] Ac  (the camera's map is the same for every chain)
@@ -802,21 +805,21 @@ k_reduce_shared(DeviceProblem p, ReduceArgs a) {
   if (p.off_bp >= 0) {
     for (int b = 0; b < B; b++) {
       const int bp = p.off_bp + 6 * b;
-      const double* U = Msum + T + (size_t)b * UB;       // [D][6] | Hbb 36 | gb 6
+      const double* U = a.sred + (size_t)c * rec + T + (size_t)b * UB;      // [D][6] | Hbb 36 | gb 6 (summed by step 1 of this launch)
       if (cp >= 0)
         for (int o = tid; o < 36; o += RED_THREADS) {     // camera pose x board pose = sum_a Ac^T U_xi_a
           const int i = o / 6, j = o % 6; double acc = 0.0;
-          for (int kk = 0; kk < KO; kk++) acc += Ac[(kk % 6) * 6 + i] * U[kk * 6 + j];
+          for (int kk = 0; kk < KO; kk++) acc += Ac[(kk % 6) * 6 + i] * __ldcg(&U[kk * 6 + j]);
           put(cp + i, bp + j, acc);
         }
       if (in0 >= 0)
         for (int o = tid; o < p.kint * 6; o += RED_THREADS) { // intrinsics x board pose = U_kappa
           const int pi = o / 6, j = o % 6;
           double acc = 0.0;
-          for (int i = 0; i < nin; i++) if (intr_param_index(p, i) == pi) acc += U[(KO + i) * 6 + j];
+          for (int i = 0; i < nin; i++) if (intr_param_index(p, i) == pi) acc += __ldcg(&U[(KO + i) * 6 + j]);
           put(in0 + pi, bp + j, acc);
         }
-      for (int o = tid; o < 42; o += RED_THREADS) a.bpart[((size_t)c * B + b) * 42 + o] = U[D * 6 + o];
+      for (int o = tid; o < 42; o += RED_THREADS) a.bpart[((size_t)c * B + b) * 42 + o] = __ldcg(&U[D * 6 + o]);
     }
   }
   // ---- step 3 (last camera): board x board blocks, board gradients (camera order) and the cost (frame order)

@@ -274,7 +274,7 @@ int launch_linearize(mcba_ctx* ctx, const DeviceProblem& P, int loss, double f_s
 int launch_reduce_shared(mcba_ctx* ctx, const DeviceProblem& P) {
   ReduceArgs r{}; r.spart = ctx->spart.p; r.nparts = P.F > 0 ? ctx->lin_grid : 0; r.Hss = ctx->Hss.p; r.g = ctx->g.p; r.bpart = ctx->bpart.p;
   r.frame_cost = ctx->frame_cost.p; r.F = P.F; r.cost_out = ctx->lin_cost.p; r.cam_counter = ctx->cam_counter.p; r.sred = ctx->sred.p;
-  const size_t sm = sizeof(double) * reduce_smem_doubles(P.T, P.D, P.B);
+  const size_t sm = sizeof(double) * reduce_smem_doubles(P.T, P.D);
   const int grid = P.C * reduce_slices(lin_record_doubles(P.T, P.D, P.B));
   if (P.motion == MOTION_ROLLING) k_reduce_shared<2><<<grid, RED_THREADS, sm, ctx->stream>>>(P, r);
   else k_reduce_shared<1><<<grid, RED_THREADS, sm, ctx->stream>>>(P, r);
@@ -524,6 +524,7 @@ int setup_problem(mcba_ctx* ctx, const mcba_problem_desc* desc, int64_t N, int V
     if (split == 1) {
       double best = -1.0;
       for (int wc = LIN_WARPS; wc >= 2; wc /= 2) {
+        if (lin_smem_for(P, wc) > LIN_SMEM_MAX) continue;      // a CTA that large cannot be launched, even one per SM
         const size_t per_cta = lin_smem_for(P, wc) + 4 * 1024;
         const int occ = (int)std::min<size_t>((227 * 1024) / per_cta, (size_t)(16 / wc));
         if (occ < 1) continue;
@@ -540,7 +541,7 @@ int setup_problem(mcba_ctx* ctx, const mcba_problem_desc* desc, int64_t N, int V
       const int per = (std::max(F, 1) + max_grid - 1) / max_grid;
       ctx->lin_grid = std::max(1, (std::max(F, 1) + per - 1) / per);
     }
-    REQUIRE(lin_smem_for(P, warps) <= 220 * 1024, MCBA_ERR_UNSUPPORTED, "too many boards for the linearisation kernel's shared memory");
+    REQUIRE(lin_smem_for(P, warps) <= LIN_SMEM_MAX, MCBA_ERR_UNSUPPORTED, "too many boards for the linearisation kernel's shared memory");
     CK(ctx->spart.alloc((size_t)ctx->lin_grid * C * lin_record_doubles(P.T, P.D, B)));
     CK(ctx->bpart.alloc((size_t)C * B * 42));
     CK(ctx->sred.alloc((size_t)C * lin_record_doubles(P.T, P.D, B)));
@@ -702,7 +703,7 @@ int mcba_create(int device, mcba_ctx** out) {
   for (int model = MODEL_STANDARD; model <= MODEL_TILTED; model++)
     for (bool roll : {false, true})
       with_model(model, roll, [](auto M, auto R) {
-        cudaFuncSetAttribute(k_linearize<decltype(M)::value, decltype(R)::value>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
+        cudaFuncSetAttribute(k_linearize<decltype(M)::value, decltype(R)::value>, cudaFuncAttributeMaxDynamicSharedMemorySize, LIN_SMEM_MAX);
       });
   cudaFuncSetAttribute(k_reduce_shared<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
   cudaFuncSetAttribute(k_reduce_shared<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);

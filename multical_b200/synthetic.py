@@ -104,6 +104,13 @@ def _boards(kind, w, h, square, count, rng):
       T = np.eye(4); T[:3, 3] = [i * side * 1.1, 0, 0]
       poses.append(T)
     return boards, np.stack(poses), side
+  if kind == "tiles":     # `count` boards on a near-square grid in one plane: many boards, all in view of an arc rig
+    cols = int(np.ceil(np.sqrt(count)))
+    boards, poses = [pts.copy() for _ in range(count)], []
+    for i in range(count):
+      T = np.eye(4); T[:3, 3] = [(i % cols) * side * 1.1, (i // cols) * side * 1.1, 0]
+      poses.append(T)
+    return boards, np.stack(poses), side
   # cube: faces of a cube of side `side` centred at the origin, each board face-centred
   face_rot = [np.zeros(3), [0, np.pi / 2, 0], [-np.pi / 2, 0, 0], [0, -np.pi / 2, 0],
               [np.pi / 2, 0, 0], [0, np.pi, 0]]
@@ -133,7 +140,8 @@ def make_scene(C=2, F=20, boards=("charuco", 16, 22, 0.025, 1), model="standard"
   centre = np.mean([(T[:3, :3] @ p.T).T.mean(axis=0) + T[:3, 3] for T, p in zip(board_poses, board_points)], axis=0)
 
   # cameras (rig frame): arc of small baselines in front of the target, or inward-looking dome
-  dist_target = 1.1 if kind == "charuco" else 1.4
+  planar = kind in ("charuco", "tiles")
+  dist_target = 1.1 if planar else 1.4
   target = np.array([0.0, 0.0, dist_target])
   cam_poses = []
   for i in range(C):
@@ -156,7 +164,7 @@ def make_scene(C=2, F=20, boards=("charuco", 16, 22, 0.025, 1), model="standard"
   dist = DIST_GT[model][None, :] * (1 + rng.normal(0, 0.05, (C, nd)))
 
   # frame poses: world -> rig; board-set centre lands near the target with a random attitude
-  rot_sigma = 0.25 if kind == "charuco" else 0.6
+  rot_sigma = 0.25 if planar else 0.6
   rv = rng.normal(0, rot_sigma, (F, 3))
   Rf = Rotation.from_rotvec(rv).as_matrix()
   tf = target[None, :] + rng.normal(0, [0.08, 0.05, 0.08], (F, 3)) - np.einsum("fij,j->fi", Rf, centre)

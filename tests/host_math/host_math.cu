@@ -4,6 +4,7 @@
 // Not part of libmcba.so and never loaded by multical_b200.
 #include "solver_kernels.cuh"
 #include "pnp_kernels.cuh"
+#include "linearize.cuh"
 
 using namespace mcba;
 
@@ -26,6 +27,12 @@ static void project_all(int n, const double* X, const double* k, double* uv, dou
 template <int MODEL>
 static void undistort_all(int n, const double* uv, const double* k, double* out) {
   for (int i = 0; i < n; i++) undistort_pixel<MODEL>(k, uv[2 * i], uv[2 * i + 1], out[2 * i], out[2 * i + 1]);
+}
+
+template <int MODEL, bool ROLL>
+static size_t lin_smem_of(int B, int warps) {
+  using S = LinShape<MODEL, ROLL>;
+  return lin_smem_doubles(S::NC, S::T, S::D, S::FB, S::NIN, B, S::NP, warps);
 }
 
 extern "C" {
@@ -59,4 +66,15 @@ void hm_hand_eye_frame_map(const double* RG, const double* RA, const double* JLW
 }
 void hm_tr2d(double b11, double b12, double b22, double g1, double g2, double Delta, double* p) { solve_tr_2d(b11, b12, b22, g1, g2, Delta, p[0], p[1]); }
 void hm_loss(int loss, double z, double* r) { loss_rho(loss, z, r[0], r[1], r[2]); }
+// dynamic shared memory of a k_linearize CTA in doubles, as the host driver sizes the launch (lin_smem_for in csrc/solver.cu)
+size_t hm_lin_smem_doubles(int model, int roll, int B, int warps) {
+  switch (model) {
+    case MODEL_STANDARD: return roll ? lin_smem_of<MODEL_STANDARD, true>(B, warps) : lin_smem_of<MODEL_STANDARD, false>(B, warps);
+    case MODEL_RATIONAL: return roll ? lin_smem_of<MODEL_RATIONAL, true>(B, warps) : lin_smem_of<MODEL_RATIONAL, false>(B, warps);
+    case MODEL_THIN_PRISM: return roll ? lin_smem_of<MODEL_THIN_PRISM, true>(B, warps) : lin_smem_of<MODEL_THIN_PRISM, false>(B, warps);
+    case MODEL_FISHEYE: return roll ? lin_smem_of<MODEL_FISHEYE, true>(B, warps) : lin_smem_of<MODEL_FISHEYE, false>(B, warps);
+    case MODEL_TILTED: return roll ? lin_smem_of<MODEL_TILTED, true>(B, warps) : lin_smem_of<MODEL_TILTED, false>(B, warps);
+  }
+  return 0;
+}
 }

@@ -40,6 +40,8 @@ def hm():
   lib.hm_matrix_to_rtvec.argtypes = [D, D]
   lib.hm_tr2d.argtypes = [C.c_double] * 6 + [D]
   lib.hm_loss.argtypes = [C.c_int, C.c_double, D]
+  lib.hm_lin_smem_doubles.argtypes = [C.c_int] * 4
+  lib.hm_lin_smem_doubles.restype = C.c_size_t
   return lib
 
 

@@ -17,6 +17,7 @@ import test_gpu_table as gt
 import test_gpu_motion as gm
 import test_gpu_pnp as gn
 import test_gpu_step_parity as sp
+import test_gpu_linearize_shapes as lin_shapes
 from multical_b200 import _native, calibration
 
 
@@ -66,30 +67,10 @@ test_two_identical_solves_agree_bit_for_bit = gp.test_two_identical_solves_agree
 
 def test_more_views_per_frame_and_more_boards_than_the_staged_tables_hold():
   """k_linearize stages a frame's view records (up to 96) and the board pose tables (up to 8) in shared memory and reads them from
-  global memory beyond that (csrc/linearize.cuh LIN_MAXV, LIN_MAXB).  12 cameras x 9 boards: 108 views per frame, 9 board tables --
-  both fall-backs at once.  Residuals against the oracle, normal equations against finite differences of the oracle."""
-  import numpy as np
-  from scipy.optimize._numdiff import approx_derivative, group_columns
-  from multical_b200 import synthetic
-  from multical_b200.calibration import from_scene
-  from oracle.ba_oracle import Problem
-  scene = synthetic.make_scene(C=12, F=2, vis=0.9, seed=3, boards=("charuco", 5, 4, 0.03, 9))
-  assert (scene["valid"].any(axis=-1).sum(axis=(0, 2)) > 96).all() and scene["B"] == 9
-  calib = from_scene(scene).enable(cameras=True)
-  prob = Problem.from_scene(scene, optimize=dict(cameras=True))
-  eng = calib._upload(calib.inliers)
-  x = prob.param_vec
-  assert np.abs(eng.residuals(x) - prob.residuals(x)).max() < 1e-9
-  S = prob.sparsity_matrix()
-  J = approx_derivative(prob.residuals, x, method="3-point", sparsity=(S, group_columns(S))).toarray()
-  r = prob.residuals(x)
-  H, g = J.T @ J, J.T @ r
-  JtJ, Jtr, cost = eng.linearize(x)
-  nrm = np.sqrt(np.outer(np.diag(H), np.diag(H)))
-  live = nrm > 0
-  assert (np.abs(JtJ - H)[live] / nrm[live]).max() < 1e-6
-  assert np.abs(Jtr - g).max() < 1e-6 * np.abs(g).max()
-  assert abs(cost - 0.5 * r @ r) < 1e-12 * cost
+  global memory beyond that (csrc/linearize.cuh LIN_MAXV, LIN_MAXB).  12 cameras x 9 boards, frames of 96, 97 and 108 views: the step
+  from staged to global view lists inside one launch, with global board tables.  Residuals against the oracle, normal equations
+  against fourth-order differences of the oracle and the first step against the model (tests/test_gpu_linearize_shapes.py)."""
+  lin_shapes.run_shape("both unstaged, 96 / 97 / 108", 132)
 
 
 def test_rolling_frames_with_a_frame_count_that_ends_in_a_partial_syrk_step():
