@@ -10,11 +10,14 @@
 // Algorithmic bytes of one linearisation pass = 18 B / corner (+16 B / view).
 //
 // Kernel map (what each replaces in the reference is cited at the kernel):
-//   k_prepare          rtvec -> R,t,JL tables                     pose_set.py:55-57, rtvec.py:24-27
-//   k_views<MODE>      residual / cost / per-corner error          calibration.py:204-206
-//   k_point_blocks     board-point rows of the normal equations    (boards=True: calibration.py:188-190)
+//   k_prepare          rtvec -> R,t,JL tables of an unchanged state        pose_set.py:55-57, rtvec.py:24-27
+//   make_trial_item    x -> trial state + its tables (k_lm; the API hooks through k_trial_state, solver.cu)
+//   corner_loss        a corner's robust cost, row weights, scaled residual    common.py:720-731
+//   corner_row         a corner's weighted 2 x D local Jacobian rows
+//   k_views<MODE>      residual / cost / per-corner error                  calibration.py:204-206
+//   k_point_blocks     board-point rows of the normal equations            (boards=True: calibration.py:188-190)
 // The linearisation itself (residuals + analytic Jacobian + normal equations) is k_linearize (linearize.cuh), the trust-region loop
-// k_lm (lm_kernel.cuh).
+// k_lm (lm_kernel.cuh).  It, k_views and k_point_blocks share corner_point, project<>, corner_loss and corner_row.
 #pragma once
 #include <stdint.h>
 #include "geometry.cuh"
@@ -175,6 +178,7 @@ __global__ void k_state_to_matrices(int C, int B, int F, const double* cam_rt, c
 // trial parameter state = current state with the free blocks replaced by x (internal order), and the pose tables of that state (item i
 // of one pass of k_lm).  One item per pose, then one per camera (intrinsics), per board point, and one for the hand-eye pair (which
 // must be complete before the derived frame poses: those items recompute it themselves).  `trial` has the layout of the current state.
+// The only path from a parameter vector to a state: k_lm calls it for its trial states, set_state_from_x (solver.cu) for the API hooks.
 __device__ __forceinline__ void make_trial_item(const DeviceProblem& p, const double* x, double* trial, int i) {
   const int nfp = p.F * p.npf;
   const int np = p.C + p.B + nfp;
@@ -278,6 +282,61 @@ constexpr int VIEW_WARPS = 4;          // warps per CTA for k_views
 constexpr double SCIPY_EPS = 2.220446049250313e-16;
 constexpr double TRIGGS_FLOOR = 0.1;
 
+// robust loss per scalar residual (least_squares.py construct_loss_function, common.py:720-731) of a corner's residual pair (ru, rv):
+// adds its 0.5 sum rho to `cost` and returns the weights wu, wv of its u and v rows (Triggs' correction, floored) with the residuals
+// scaled to match.  loss == 0: cost 0.5 (ru^2 + rv^2), weights 1, residuals unchanged.  (Values in, a struct out: through references
+// the compiler orders k_linearize's instructions differently.)
+struct CornerLoss { double ru, rv, wu, wv; };
+__device__ __forceinline__ CornerLoss corner_loss(int loss, double f_scale, double ru, double rv, double& cost) {
+  double wu = 1.0, wv = 1.0;
+  if (loss == 0) {
+    cost += 0.5 * (ru * ru + rv * rv);
+  } else {
+    const double is = 1.0 / f_scale, fs2 = f_scale * f_scale;
+    double zu = ru * is, zv = rv * is;
+    zu *= zu; zv *= zv;
+    double r0u, r1u, r2u, r0v, r1v, r2v;
+    loss_rho(loss, zu, r0u, r1u, r2u);
+    loss_rho(loss, zv, r0v, r1v, r2v);
+    cost += 0.5 * fs2 * (r0u + r0v);
+    double ju = r1u + 2.0 * r2u * zu, jv = r1v + 2.0 * r2v * zv;
+    ju = fmax(fmax(ju, TRIGGS_FLOOR * r1u), SCIPY_EPS);
+    jv = fmax(fmax(jv, TRIGGS_FLOOR * r1v), SCIPY_EPS);
+    wu = sqrt(ju); wv = sqrt(jv);
+    ru *= r1u / wu; rv *= r1v / wv;
+  }
+  return {ru, rv, wu, wv};
+}
+
+// the weighted local Jacobian rows of a corner, columns [0, D): twist block(s) (6; rolling: start | end, 12) then [fx fy cx cy dist].
+// Xc = camera-frame point (rolling: Xs, Xe = the start / end chain's point, tau = the blend), Ju, Jv / ku, kv = d(u, v) / d(Xc) and
+// d(u, v) / d(intrinsics) from project<MODEL, true>.  The four structural zeros (fy, cy of the u row; fx, cx of the v row) are not
+// written: the caller zeroes the rows first (k_linearize needs zero rows for its idle lanes anyway, and stores of the zeros here would
+// change its instruction schedule).
+template <int MODEL, bool ROLL>
+__device__ __forceinline__ void corner_row(const double* Xc, const double* Xs, const double* Xe, double tau, const double* Ju, const double* Jv,
+                                           const double* ku, const double* kv, double wu, double wv, double* gu, double* gv) {
+  constexpr int ND = model_nd(MODEL), KO = ROLL ? 12 : 6;
+  if constexpr (!ROLL) {
+    gu[0] = (Xc[1] * Ju[2] - Xc[2] * Ju[1]) * wu; gu[1] = (Xc[2] * Ju[0] - Xc[0] * Ju[2]) * wu; gu[2] = (Xc[0] * Ju[1] - Xc[1] * Ju[0]) * wu;
+    gv[0] = (Xc[1] * Jv[2] - Xc[2] * Jv[1]) * wv; gv[1] = (Xc[2] * Jv[0] - Xc[0] * Jv[2]) * wv; gv[2] = (Xc[0] * Jv[1] - Xc[1] * Jv[0]) * wv;
+#pragma unroll
+    for (int i = 0; i < 3; i++) { gu[3 + i] = Ju[i] * wu; gv[3 + i] = Jv[i] * wv; }
+  } else {
+    const double su = (1.0 - tau) * wu, sv = (1.0 - tau) * wv, eu = tau * wu, ev = tau * wv;
+    gu[0] = (Xs[1] * Ju[2] - Xs[2] * Ju[1]) * su; gu[1] = (Xs[2] * Ju[0] - Xs[0] * Ju[2]) * su; gu[2] = (Xs[0] * Ju[1] - Xs[1] * Ju[0]) * su;
+    gv[0] = (Xs[1] * Jv[2] - Xs[2] * Jv[1]) * sv; gv[1] = (Xs[2] * Jv[0] - Xs[0] * Jv[2]) * sv; gv[2] = (Xs[0] * Jv[1] - Xs[1] * Jv[0]) * sv;
+    gu[6] = (Xe[1] * Ju[2] - Xe[2] * Ju[1]) * eu; gu[7] = (Xe[2] * Ju[0] - Xe[0] * Ju[2]) * eu; gu[8] = (Xe[0] * Ju[1] - Xe[1] * Ju[0]) * eu;
+    gv[6] = (Xe[1] * Jv[2] - Xe[2] * Jv[1]) * ev; gv[7] = (Xe[2] * Jv[0] - Xe[0] * Jv[2]) * ev; gv[8] = (Xe[0] * Jv[1] - Xe[1] * Jv[0]) * ev;
+#pragma unroll
+    for (int i = 0; i < 3; i++) { gu[3 + i] = Ju[i] * su; gv[3 + i] = Jv[i] * sv; gu[9 + i] = Ju[i] * eu; gv[9 + i] = Jv[i] * ev; }
+  }
+  gu[KO] = ku[0] * wu; gu[KO + 2] = wu;
+  gv[KO + 1] = kv[1] * wv; gv[KO + 3] = wv;
+#pragma unroll
+  for (int i = 0; i < ND; i++) { gu[KO + 4 + i] = ku[4 + i] * wu; gv[KO + 4 + i] = kv[4 + i] * wv; }
+}
+
 // k_views: one warp per view, lanes stride over the view's corners (one thread per corner per step).
 //   MODE_COST    -> 0.5*sum rho(f) per view               (cost hook of mcba_residuals)
 //   MODE_RESID   -> residual vector in canonical order     (calibration.py:204-206)
@@ -320,17 +379,7 @@ k_views(DeviceProblem p, ViewKernelArgs a) {
       } else if constexpr (MODE == MODE_ERROR) {
         a.err[p.orig[idx]] = sqrt(ru * ru + rv * rv);
       } else {
-        // robust loss per scalar residual (least_squares.py construct_loss_function, common.py:720-731)
-        if (a.loss == 0) acc += 0.5 * (ru * ru + rv * rv);
-        else {
-          const double is = 1.0 / a.f_scale, fs2 = a.f_scale * a.f_scale;
-          double zu = ru * is, zv = rv * is;
-          zu *= zu; zv *= zv;
-          double r0u, r1u, r2u, r0v, r1v, r2v;
-          loss_rho(a.loss, zu, r0u, r1u, r2u);
-          loss_rho(a.loss, zv, r0v, r1v, r2v);
-          acc += 0.5 * fs2 * (r0u + r0v);
-        }
+        corner_loss(a.loss, a.f_scale, ru, rv, acc);
       }
     }
     if constexpr (MODE == MODE_COST) {
@@ -429,41 +478,12 @@ k_point_blocks(DeviceProblem p, ViewKernelArgs a, double* Hss, double* W, double
       corner_point<ROLL>(vp, vpe, X, tau, Xc, Xs, Xe);
       double u, w_, Ju[3], Jv[3], ku[4 + ND], kv[4 + ND];
       project<MODEL, true>(Xc, k, u, w_, Ju, Jv, ku, kv);
-      double ru = u - ob.x, rv = w_ - ob.y, wu = 1.0, wv = 1.0;
-      if (a.loss != 0) {
-        const double is = 1.0 / a.f_scale;
-        double zu = ru * is, zv = rv * is;
-        zu *= zu; zv *= zv;
-        double r0u, r1u, r2u, r0v, r1v, r2v;
-        loss_rho(a.loss, zu, r0u, r1u, r2u);
-        loss_rho(a.loss, zv, r0v, r1v, r2v);
-        double ju = r1u + 2.0 * r2u * zu, jv = r1v + 2.0 * r2v * zv;
-        ju = fmax(fmax(ju, TRIGGS_FLOOR * r1u), SCIPY_EPS);
-        jv = fmax(fmax(jv, TRIGGS_FLOOR * r1v), SCIPY_EPS);
-        wu = sqrt(ju); wv = sqrt(jv);
-        ru *= r1u / wu; rv *= r1v / wv;
-      }
-      // local rows: twist block(s) (KO) then [fx fy cx cy dist] (NIN) -- the layout of k_linearize
-      double gu[KO + NIN], gv[KO + NIN];
-      if constexpr (!ROLL) {
-        gu[0] = (Xc[1] * Ju[2] - Xc[2] * Ju[1]) * wu; gu[1] = (Xc[2] * Ju[0] - Xc[0] * Ju[2]) * wu; gu[2] = (Xc[0] * Ju[1] - Xc[1] * Ju[0]) * wu;
-        gv[0] = (Xc[1] * Jv[2] - Xc[2] * Jv[1]) * wv; gv[1] = (Xc[2] * Jv[0] - Xc[0] * Jv[2]) * wv; gv[2] = (Xc[0] * Jv[1] - Xc[1] * Jv[0]) * wv;
-#pragma unroll
-        for (int i = 0; i < 3; i++) { gu[3 + i] = Ju[i] * wu; gv[3 + i] = Jv[i] * wv; }
-      } else {
-        const double su = (1.0 - tau) * wu, sv = (1.0 - tau) * wv, eu = tau * wu, ev = tau * wv;
-        gu[0] = (Xs[1] * Ju[2] - Xs[2] * Ju[1]) * su; gu[1] = (Xs[2] * Ju[0] - Xs[0] * Ju[2]) * su; gu[2] = (Xs[0] * Ju[1] - Xs[1] * Ju[0]) * su;
-        gv[0] = (Xs[1] * Jv[2] - Xs[2] * Jv[1]) * sv; gv[1] = (Xs[2] * Jv[0] - Xs[0] * Jv[2]) * sv; gv[2] = (Xs[0] * Jv[1] - Xs[1] * Jv[0]) * sv;
-        gu[6] = (Xe[1] * Ju[2] - Xe[2] * Ju[1]) * eu; gu[7] = (Xe[2] * Ju[0] - Xe[0] * Ju[2]) * eu; gu[8] = (Xe[0] * Ju[1] - Xe[1] * Ju[0]) * eu;
-        gv[6] = (Xe[1] * Jv[2] - Xe[2] * Jv[1]) * ev; gv[7] = (Xe[2] * Jv[0] - Xe[0] * Jv[2]) * ev; gv[8] = (Xe[0] * Jv[1] - Xe[1] * Jv[0]) * ev;
-#pragma unroll
-        for (int i = 0; i < 3; i++) { gu[3 + i] = Ju[i] * su; gv[3 + i] = Jv[i] * sv; gu[9 + i] = Ju[i] * eu; gv[9 + i] = Jv[i] * ev; }
-      }
-#pragma unroll
-      for (int i = 0; i < NIN; i++) { gu[KO + i] = 0.0; gv[KO + i] = 0.0; }
-      gu[KO] = ku[0] * wu; gu[KO + 2] = wu; gv[KO + 1] = kv[1] * wv; gv[KO + 3] = wv;
-#pragma unroll
-      for (int i = 0; i < ND; i++) { gu[KO + 4 + i] = ku[4 + i] * wu; gv[KO + 4 + i] = kv[4 + i] * wv; }
+      double cost = 0.0;         // unused: k_linearize sums the cost
+      const CornerLoss cl = corner_loss(a.loss, a.f_scale, u - ob.x, w_ - ob.y, cost);
+      const double ru = cl.ru, rv = cl.rv, wu = cl.wu, wv = cl.wv;
+      // local rows: twist block(s) (KO) then [fx fy cx cy dist] (NIN), as k_linearize stages them
+      double gu[KO + NIN] = {}, gv[KO + NIN] = {};
+      corner_row<MODEL, ROLL>(Xc, Xs, Xe, tau, Ju, Jv, ku, kv, wu, wv, gu, gv);
       // point rows: d r / d X_board = J_proj R_cfb  (rolling: R = (1 - tau) R_start + tau R_end)
       double xu[3], xv[3];
 #pragma unroll

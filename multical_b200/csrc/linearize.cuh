@@ -54,7 +54,7 @@ __device__ __forceinline__ void view_chunk(const DeviceProblem& p, int loss, dou
                                            const double* bp, double inv_h, int base, int end, int lane, double* stage,
                                            double (&acc)[LinShape<MODEL, ROLL>::NPAIR][2], double& cost_acc, double2 ob, int pi) {
   using S = LinShape<MODEL, ROLL>;
-  constexpr int ND = S::ND, KO = S::KO, D = S::D, NC = S::NC, NT = S::NT;
+  constexpr int ND = S::ND, D = S::D, NC = S::NC, NT = S::NT;
   const int grp = lane >> 2, tig = lane & 3;
   const int idx = base + lane;
   double gu[NC], gv[NC];
@@ -68,44 +68,9 @@ __device__ __forceinline__ void view_chunk(const DeviceProblem& p, int loss, dou
     double u, w_;
     double Ju[3], Jv[3], ku[4 + ND], kv[4 + ND];
     project<MODEL, true>(Xc, k, u, w_, Ju, Jv, ku, kv);
-    double ru = u - ob.x, rv = w_ - ob.y;              // projected - observed (calibration.py:206)
-    double wu = 1.0, wv = 1.0;
-    if (loss == 0) {
-      cost_acc += 0.5 * (ru * ru + rv * rv);
-    } else {
-      // robust loss per scalar residual (least_squares.py construct_loss_function, common.py:720-731)
-      const double is = 1.0 / f_scale, fs2 = f_scale * f_scale;
-      double zu = ru * is, zv = rv * is;
-      zu *= zu; zv *= zv;
-      double r0u, r1u, r2u, r0v, r1v, r2v;
-      loss_rho(loss, zu, r0u, r1u, r2u);
-      loss_rho(loss, zv, r0v, r1v, r2v);
-      cost_acc += 0.5 * fs2 * (r0u + r0v);
-      double ju = r1u + 2.0 * r2u * zu, jv = r1v + 2.0 * r2v * zv;
-      ju = fmax(fmax(ju, TRIGGS_FLOOR * r1u), SCIPY_EPS);
-      jv = fmax(fmax(jv, TRIGGS_FLOOR * r1v), SCIPY_EPS);
-      wu = sqrt(ju); wv = sqrt(jv);
-      ru *= r1u / wu; rv *= r1v / wv;
-    }
-    if constexpr (!ROLL) {
-      gu[0] = (Xc[1] * Ju[2] - Xc[2] * Ju[1]) * wu; gu[1] = (Xc[2] * Ju[0] - Xc[0] * Ju[2]) * wu; gu[2] = (Xc[0] * Ju[1] - Xc[1] * Ju[0]) * wu;
-      gv[0] = (Xc[1] * Jv[2] - Xc[2] * Jv[1]) * wv; gv[1] = (Xc[2] * Jv[0] - Xc[0] * Jv[2]) * wv; gv[2] = (Xc[0] * Jv[1] - Xc[1] * Jv[0]) * wv;
-#pragma unroll
-      for (int i = 0; i < 3; i++) { gu[3 + i] = Ju[i] * wu; gv[3 + i] = Jv[i] * wv; }
-    } else {
-      const double su = (1.0 - tau) * wu, sv = (1.0 - tau) * wv, eu = tau * wu, ev = tau * wv;
-      gu[0] = (Xs[1] * Ju[2] - Xs[2] * Ju[1]) * su; gu[1] = (Xs[2] * Ju[0] - Xs[0] * Ju[2]) * su; gu[2] = (Xs[0] * Ju[1] - Xs[1] * Ju[0]) * su;
-      gv[0] = (Xs[1] * Jv[2] - Xs[2] * Jv[1]) * sv; gv[1] = (Xs[2] * Jv[0] - Xs[0] * Jv[2]) * sv; gv[2] = (Xs[0] * Jv[1] - Xs[1] * Jv[0]) * sv;
-      gu[6] = (Xe[1] * Ju[2] - Xe[2] * Ju[1]) * eu; gu[7] = (Xe[2] * Ju[0] - Xe[0] * Ju[2]) * eu; gu[8] = (Xe[0] * Ju[1] - Xe[1] * Ju[0]) * eu;
-      gv[6] = (Xe[1] * Jv[2] - Xe[2] * Jv[1]) * ev; gv[7] = (Xe[2] * Jv[0] - Xe[0] * Jv[2]) * ev; gv[8] = (Xe[0] * Jv[1] - Xe[1] * Jv[0]) * ev;
-#pragma unroll
-      for (int i = 0; i < 3; i++) { gu[3 + i] = Ju[i] * su; gv[3 + i] = Jv[i] * sv; gu[9 + i] = Ju[i] * eu; gv[9 + i] = Jv[i] * ev; }
-    }
-    gu[KO] = ku[0] * wu; gu[KO + 2] = wu;
-    gv[KO + 1] = kv[1] * wv; gv[KO + 3] = wv;
-#pragma unroll
-    for (int i = 0; i < ND; i++) { gu[KO + 4 + i] = ku[4 + i] * wu; gv[KO + 4 + i] = kv[4 + i] * wv; }
-    gu[D] = ru; gv[D] = rv;                      // residual column: Gt^T Gt then carries G^T r as well
+    const CornerLoss cl = corner_loss(loss, f_scale, u - ob.x, w_ - ob.y, cost_acc);      // projected - observed (calibration.py:206)
+    corner_row<MODEL, ROLL>(Xc, Xs, Xe, tau, Ju, Jv, ku, kv, cl.wu, cl.wv, gu, gv);
+    gu[D] = cl.ru; gv[D] = cl.rv;                // residual column: Gt^T Gt then carries G^T r as well
   }
   // The 64 residual rows of the chunk go through the stage buffer in two halves of 32 (lanes 0-15, then lanes 16-31): half the shared
   // memory per warp, so that twice the warps fit an SM (the pass is latency-bound per warp: resident warps are what hides it).

@@ -203,18 +203,7 @@ struct mcba_ctx {
 
 namespace {
 
-// parameters of block-structured vector x (internal order) <-> full parameter state
-__global__ void k_scatter_params(DeviceProblem p, const double* x, double* cam_rt, double* board_rt, double* frame_rt, double* intr) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= p.n) return;
-  const double v = x[i];
-  if (i >= p.n_s) { frame_rt[i - p.n_s] = v; return; }
-  if (p.off_cp >= 0 && i >= p.off_cp && i < p.off_cp + 6 * p.C) { cam_rt[i - p.off_cp] = v; return; }
-  if (p.off_bp >= 0 && i >= p.off_bp && i < p.off_bp + 6 * p.B) { board_rt[i - p.off_bp] = v; return; }
-  if (p.off_in >= 0 && i >= p.off_in && i < p.off_in + p.kint * p.C) { intr[i - p.off_in] = v; return; }
-  if (p.off_pt >= 0 && i >= p.off_pt && i < p.off_pt + 3 * p.B * p.P) { p.board_pts[i - p.off_pt] = v; return; }
-  if (p.off_he >= 0 && i >= p.off_he && i < p.off_he + 12) p.he_rt[i - p.off_he] = v;
-}
+// full parameter state -> block-structured vector x (internal order)
 __global__ void k_gather_params(DeviceProblem p, double* x, const double* cam_rt, const double* board_rt, const double* frame_rt, const double* intr) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= p.n) return;
@@ -227,11 +216,13 @@ __global__ void k_gather_params(DeviceProblem p, double* x, const double* cam_rt
   else if (p.off_he >= 0 && i >= p.off_he && i < p.off_he + 12) v = p.he_rt[i - p.off_he];
   x[i] = v;
 }
-// copies the fixed blocks so that a trial state is complete; with fix_aspect fy follows fx (camera.py:159-160)
-__global__ void k_fix_aspect(DeviceProblem p, double* intr) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c < p.C && p.fix_aspect) intr[c * p.kint + 1] = intr[c * p.kint];
+// x (internal order) -> trial state and its pose tables, one thread per item of make_trial_item (p: the current state)
+__global__ void k_trial_state(DeviceProblem p, const double* x, double* trial, int n_items) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n_items) make_trial_item(p, x, trial, i);
 }
+// items of make_trial_item: poses, intrinsics per camera, padded board points, the hand-eye pair
+int trial_items(const DeviceProblem& P) { return P.C + P.B + P.F * P.npf + P.C + P.B * P.P + 2; }
 
 template <int MODE>
 int launch_views(mcba_ctx* ctx, const DeviceProblem& P, const ViewKernelArgs& a) {
@@ -296,17 +287,6 @@ int prepare(mcba_ctx* ctx, const DeviceProblem& P) {
   return MCBA_OK;
 }
 
-// push vector x (internal order) into the (trial or current) parameter state and rebuild the pose tables
-int set_state_from_x(mcba_ctx* ctx, const double* x, bool trial) {
-  DeviceProblem P = with_state(ctx, trial);
-  if (P.n > 0) {
-    k_scatter_params<<<(P.n + 255) / 256, 256, 0, ctx->stream>>>(P, x, P.cam_rt, P.board_rt, P.frame_rt, P.intr);
-    CKL();
-    if (P.fix_aspect && P.off_in >= 0) { k_fix_aspect<<<(P.C + 127) / 128, 128, 0, ctx->stream>>>(P, P.intr); CKL(); }
-  }
-  return prepare(ctx, P);
-}
-
 // The normal equations and the cost at the (trial or current) state, whose pose tables must already describe it: k_linearize, its per-CTA
 // records -> H_ss, g_s, cost (k_reduce_shared), then boards=True: the board-point blocks on top (k_point_blocks), then hand-eye: the
 // hand-eye rows and columns from the frame blocks (k_fold_hand_eye, last: it reads the point rows of W_f)
@@ -351,13 +331,27 @@ int copy_state_to_trial(mcba_ctx* ctx) {
   return MCBA_OK;
 }
 
+// push vector x (internal order) into the trial state and rebuild the pose tables, as k_lm builds its trial states; trial == false:
+// the trial state then becomes the current one.  The current state is only read, never updated in place: the derived hand-eye frame
+// poses read he_rt while other items write its new value.
+int set_state_from_x(mcba_ctx* ctx, const double* x, bool trial) {
+  // make_trial_item writes every entry but he_rt of a problem without hand-eye and frame_rt of a hand-eye problem (derived frames):
+  // those come from the copy
+  int r = copy_state_to_trial(ctx); if (r) return r;
+  const int items = trial_items(ctx->P);
+  k_trial_state<<<(items + 127) / 128, 128, 0, ctx->stream>>>(ctx->P, x, ctx->trial.p, items);
+  CKL();
+  if (!trial) CK(cudaMemcpyAsync(ctx->params.p, ctx->trial.p, sizeof(double) * ctx->layout.len, cudaMemcpyDeviceToDevice, ctx->stream));
+  return MCBA_OK;
+}
+
 LmArgs make_lm_args(mcba_ctx* ctx, int log_cap) {
   const DeviceProblem& P = ctx->P;
   LmArgs a{};
   a.P = P;
   a.trial = ctx->trial.p; a.state_len = (int)ctx->layout.len;
   a.n = P.n; a.n_s = P.n_s; a.F = P.F; a.fb = P.fb;
-  a.n_items = P.C + P.B + P.F * P.npf + P.C + P.B * P.P + 2;
+  a.n_items = trial_items(P);
   a.Hss = ctx->Hss.p; a.Hff = ctx->Hff.p; a.W = ctx->W.p; a.g = ctx->g.p;
   a.frame_cost = ctx->frame_cost.p; a.lin_cost = ctx->lin_cost.p;
   a.x = ctx->x.p; a.x_new = ctx->x_new.p; a.sinv = ctx->sinv.p; a.d = ctx->d.p; a.gh = ctx->gh.p; a.gn = ctx->gn.p;
@@ -1986,8 +1980,7 @@ int mcba_residuals(mcba_ctx* ctx, const double* x, double* r_out, double* cost) 
   bool trial = false;
   if (x) {
     // evaluate at x without disturbing the stored parameters: trial state = current state overwritten by x
-    int r = copy_state_to_trial(ctx); if (r) return r;
-    r = write_x_canonical(ctx, x, ctx->x_new.p); if (r) return r;
+    int r = write_x_canonical(ctx, x, ctx->x_new.p); if (r) return r;
     r = set_state_from_x(ctx, ctx->x_new.p, true); if (r) return r;
     trial = true;
   } else {
