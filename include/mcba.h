@@ -250,6 +250,22 @@ int  mcba_intrinsic_init(mcba_ctx* ctx, const mcba_problem_desc* desc, const int
                          const uint8_t* view_use, double* intrinsics, double* poses, uint8_t* ok);
 int  mcba_view_errors(mcba_ctx* ctx, double* sumsq, int64_t* count);
 
+/* -- stereo calibration of a camera pair (stereo_calibrate, camera.py:261-286: cv2.stereoCalibrate; stereo_calibrate_fisheye,
+ * camera_fisheye.py:180-205: cv2.fisheye.stereoCalibrate) ---------------------------------------------------------------------------
+ * mcba_stereo_init: OpenCV's start.  desc = {C = 2, F = views, B = 1, P, model}; detection lists as for mcba_pnp_views, list w = c*F + f
+ * (camera 0 the left one), with no minimum-detections rule; board_points f64[P][3] the pair's object points; intrinsics f64[2][5+nd]
+ * (Camera.params order) of both cameras.  Per view, k_pnp_views of both cameras under their intrinsics, then for every view where both
+ * poses are valid the relative pose R = R2 R1^T, T = T2 - R T1 (x_right = R x_left + T) and its rotation vector; rt0 f64[6] receives
+ * the median of each component over those views (the two middle values averaged for an even count; NaN without such a view).  fp64
+ * without floating-point sums: bit-reproducible.  Out: also left_poses f64[F][4][4] (board wrt the left camera) and ok uint8[F] (both
+ * poses valid).  Non-planar object points (z != 0) fail with MCBA_ERR_UNSUPPORTED, a view with fewer than 4 points in either camera
+ * with MCBA_ERR_DEGENERATE naming the view.  Does not touch the uploaded problem.
+ * The solve is the engine's own: C = 2, the views as frames, one board; cameras [I, rt0], frames at left_poses, the board at identity;
+ * optimize = MCBA_OPT_CAMERA_POSES | MCBA_OPT_MOTION [| MCBA_OPT_CAMERAS [| MCBA_OPT_FIX_ASPECT] with free intrinsics].  The pair's pose is
+ * read in gauge-invariant form, T_cam1 T_cam0^-1, and OpenCV's RMS is sqrt(sum of mcba_view_errors' sumsq / (2 x corners per camera)). */
+int  mcba_stereo_init(mcba_ctx* ctx, const mcba_problem_desc* desc, const int64_t* det_start, const int32_t* det_ids, const double* det_xy,
+                      const double* board_points, const double* intrinsics, double* rt0, double* left_poses, uint8_t* ok);
+
 /* -- pose-graph initialisation (tables.initialise_poses, tables.py:354-377) ---------------------------------------------------------
  * Every call of align_transforms_robust (transform/matrix.py:140-153) that initialise_poses makes, batched: mean_robust of the relative
  * poses (Ward clustering of their rtvecs, transform/common.py:6-19), the inlier test at 1.5 x the upper quartile of the errors over

@@ -31,7 +31,7 @@ EXPORTS = ["mcba_create", "mcba_destroy", "mcba_last_error", "mcba_set_stream", 
            "mcba_table_get_inliers", "mcba_table_select", "mcba_pnp_views", "mcba_table_errors", "mcba_table_error_ranks", "mcba_table_count_below", "mcba_table_reject",
            "mcba_intrinsic_init", "mcba_view_errors", "mcba_pose_pairs", "mcba_pose_times", "mcba_pose_cluster",
            "mcba_hand_eye_quads", "mcba_hand_eye_vote", "mcba_undistort_map", "mcba_undistort_images", "mcba_project_points",
-           "mcba_undistort_points", "mcba_remap_cubic_table"]
+           "mcba_undistort_points", "mcba_remap_cubic_table", "mcba_stereo_init"]
 IMAGE_UINT8 = 0          # include/mcba.h MCBA_IMAGE_UINT8
 TABLE_VALID, TABLE_INLIERS = 0, 1
 
@@ -125,6 +125,7 @@ def load():
   lib.mcba_table_reject.argtypes = [P, C.c_double, I64, I64]
   lib.mcba_intrinsic_init.argtypes = [P, C.POINTER(ProblemDesc), I64, I32, D, D, I32, I32, U8, D, D, U8]
   lib.mcba_view_errors.argtypes = [P, D, I64]
+  lib.mcba_stereo_init.argtypes = [P, C.POINTER(ProblemDesc), I64, I32, D, D, D, D, D, U8]
   i32 = C.c_int32
   lib.mcba_pose_pairs.argtypes = [P, i32, i32, i32, D, U8, i32, I32, i32, D, U8, I32]
   lib.mcba_pose_times.argtypes = [P, i32, i32, i32, D, U8, D, U8, D, U8, D, U8]

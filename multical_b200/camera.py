@@ -121,6 +121,19 @@ def calibrate_cameras_fisheye(boards, points, image_sizes, **kwargs):
   return calibrate_cameras_fisheye(boards, points, image_sizes, **kwargs)
 
 
+def stereo_calibrate(cameras, matches, max_iter=60, eps=1e-6, fix_aspect=False, fix_intrinsic=True, **solve_opts):
+  """camera.py:261-286 on the GPU (multical_b200/stereo.py): (left, right, 4x4 pose of the pair, err)."""
+  from .stereo import stereo_calibrate
+  return stereo_calibrate(cameras, matches, max_iter=max_iter, eps=eps, fix_aspect=fix_aspect, fix_intrinsic=fix_intrinsic, **solve_opts)
+
+
+def stereo_calibrate_fisheye(cameras, matches, max_iter=60, eps=1e-6, fix_aspect=False, fix_intrinsic=True, **solve_opts):
+  """camera_fisheye.py:180-205 on the GPU (multical_b200/stereo.py): (left, right, 4x4 pose of the pair, err)."""
+  from .stereo import stereo_calibrate_fisheye
+  return stereo_calibrate_fisheye(cameras, matches, max_iter=max_iter, eps=eps, fix_aspect=fix_aspect, fix_intrinsic=fix_intrinsic,
+                                  **solve_opts)
+
+
 def undistort_images(images, cameras, j=None, chunksize=4):
   """camera.py:247-258 on the GPU (multical_b200/undistort.py): per camera, its images remapped through its undistortion map."""
   from .undistort import undistort_images

@@ -25,6 +25,7 @@
 #include "pose_init_kernels.cuh"
 #include "hand_eye_init_kernels.cuh"
 #include "undistort_kernels.cuh"
+#include "stereo_kernels.cuh"
 
 using namespace mcba;
 
@@ -159,6 +160,10 @@ struct mcba_ctx {
   struct IntrinsicBuffers {
     DevBuf<int32_t> used, cam_start, size; DevBuf<double> H, k0; DevBuf<uint8_t> hok;
   } intrinsic;
+  // stereo initialisation (mcba_stereo_init): the intrinsics of the pair, relative poses, their sorted components, the start
+  struct StereoBuffers {
+    DevBuf<double> rel, sorted, rt0; DevBuf<uint8_t> both;
+  } stereo;
   // pose-graph initialisation (mcba_pose_pairs / mcba_pose_times / mcba_pose_cluster): the table, the gathered rows, per-item results
   struct PoseInitBuffers {
     DevBuf<double> poses, cam, board, m1, m2, vecs, t; DevBuf<uint8_t> valid, mask, inl; DevBuf<PoseRow> rows;
@@ -1016,6 +1021,11 @@ int mcba_table_from_detections(mcba_ctx* ctx, const mcba_problem_desc* desc, con
 
 namespace {
 
+bool all_finite(const double* p, size_t n) {
+  for (size_t i = 0; i < n; i++) if (!std::isfinite(p[i])) return false;
+  return true;
+}
+
 // The caller's detection lists: list w = (c*F+f)*B+b of the C*F*B views holds point ids det_ids[det_start[w]:det_start[w+1]] in [0, P) and
 // their pixel corners det_xy (a CSR layout); the boards' id grids are at most 64 x 64.
 int check_detections(mcba_ctx* ctx, const mcba_problem_desc* desc, const int64_t* det_start, const int32_t* det_ids, const double* det_xy,
@@ -1163,6 +1173,45 @@ int mcba_intrinsic_init(mcba_ctx* ctx, const mcba_problem_desc* desc, const int6
   return MCBA_OK;
 }
 
+// Initialisation of stereo calibration (stereo_kernels.cuh): per-view poses of both cameras by k_pnp_views under the given intrinsics,
+// then the median relative pose.  Independent of the uploaded problem.
+int mcba_stereo_init(mcba_ctx* ctx, const mcba_problem_desc* desc, const int64_t* det_start, const int32_t* det_ids, const double* det_xy,
+                     const double* board_points, const double* intrinsics, double* rt0, double* left_poses, uint8_t* ok) {
+  if (!ctx || !desc) return MCBA_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  { int r = check_desc(ctx, desc); if (r) return r; }
+  REQUIRE(desc->C == 2 && desc->B == 1 && desc->F > 0, MCBA_ERR_ARG, "a stereo pair is 2 cameras, 1 board and at least one view");
+  REQUIRE(det_start && board_points && intrinsics && rt0 && left_poses && ok, MCBA_ERR_ARG, "null argument");
+  const int F = desc->F, Pn = desc->P;
+  const int kint = 5 + model_nd(desc->model);
+  const int32_t grid[5] = {1, 1, 1, 0, 0};           // the views are chosen already: no minimum-detections rule on the device
+  { int r = check_detections(ctx, desc, det_start, det_ids, det_xy, grid); if (r) return r; }
+  REQUIRE(all_finite(intrinsics, 2 * (size_t)kint), MCBA_ERR_NONFINITE, "non-finite camera parameter");
+  // the per-view poses are the planar PnP of k_pnp_views
+  for (size_t i = 0; i < (size_t)Pn; i++)
+    REQUIRE(board_points[3 * i + 2] == 0.0, MCBA_ERR_UNSUPPORTED, "non-planar object points (z != 0): the initial view poses need planar targets");
+  for (int c = 0; c < 2; c++)
+    for (int f = 0; f < F; f++) {
+      const int64_t n = det_start[c * F + f + 1] - det_start[c * F + f];
+      REQUIRE(n >= 4, MCBA_ERR_DEGENERATE, "view " + std::to_string(f) + " has " + std::to_string(n) + " points: a view pose needs at least 4");
+    }
+  cudaStream_t s = ctx->stream;
+  auto& pb = ctx->pnp; auto& sb = ctx->stereo;
+  { int r = stage_detections(ctx, desc, det_start, det_ids, det_xy, grid, board_points); if (r) return r; }
+  CK(pb.in.alloc((size_t)2 * kint));
+  CK(cudaMemcpyAsync(pb.in.p, intrinsics, sizeof(double) * 2 * (size_t)kint, cudaMemcpyHostToDevice, s));
+  { int r = launch_pnp(ctx, desc, desc->model, kint, pb.in.p); if (r) return r; }
+  CK(sb.rel.alloc((size_t)6 * F)); CK(sb.sorted.alloc((size_t)6 * F)); CK(sb.rt0.alloc(6)); CK(sb.both.alloc((size_t)F));
+  StereoStartArgs a{};
+  a.F = F; a.poses = pb.pose.p; a.ok = pb.ok.p; a.rel = sb.rel.p; a.sorted = sb.sorted.p; a.rt0 = sb.rt0.p; a.both = sb.both.p;
+  k_stereo_start<<<1, STEREO_THREADS, 0, s>>>(a); CKL();
+  CK(cudaMemcpyAsync(rt0, sb.rt0.p, sizeof(double) * 6, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(left_poses, pb.pose.p, sizeof(double) * 16 * (size_t)F, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(ok, sb.both.p, (size_t)F, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  return MCBA_OK;
+}
+
 // Per-view sums of squared pixel errors and corner counts of the packed problem at the current parameters (intrinsics_kernels.cuh)
 int mcba_view_errors(mcba_ctx* ctx, double* sumsq, int64_t* count) {
   if (!ctx || !sumsq || !count) return MCBA_ERR_ARG;
@@ -1189,11 +1238,6 @@ int mcba_view_errors(mcba_ctx* ctx, double* sumsq, int64_t* count) {
 }
 
 namespace {
-
-bool all_finite(const double* p, size_t n) {
-  for (size_t i = 0; i < n; i++) if (!std::isfinite(p[i])) return false;
-  return true;
-}
 
 int check_pose_dims(mcba_ctx* ctx, int32_t C, int32_t F, int32_t B) {
   REQUIRE(C > 0 && F > 0 && B > 0, MCBA_ERR_ARG, "bad pose table dimensions");

@@ -203,6 +203,19 @@ class Engine:
                                           nat.dptr(poses), u8(ok)))
     return intr, poses[:nv].reshape(Cn, F, B, 4, 4), ok[:nv].reshape(Cn, F, B).astype(bool)
 
+  def stereo_init(self, model, F, P, det_start, det_ids, det_xy, board_points, intrinsics):
+    """Start of a stereo pair's calibration (include/mcba.h mcba_stereo_init): lists w = c*F + f of the two cameras' F views of board
+    points [P, 3], intrinsics [2, 5+nd] -> (rt0 [6], the median relative pose x_right = R x_left + T; left poses [F, 4, 4]; ok [F], both
+    poses valid)."""
+    (Cn, F, B, P), det_start, det_ids, det_xy, bp = self._detections((2, F, 1, P), det_start, det_ids, det_xy, board_points)
+    intr = nat.f64(intrinsics).reshape(2, 5 + nat.DIST_SIZES[model])
+    rt0, poses, ok = np.zeros(6), np.zeros((max(F, 1), 4, 4)), np.zeros(max(F, 1), np.uint8)
+    d = nat.ProblemDesc(Cn, F, B, P, nat.MODEL_IDS[model], 0, 0)
+    self._ck(self.lib.mcba_stereo_init(self.h, C.byref(d), det_start.ctypes.data_as(C.POINTER(C.c_int64)), nat.iptr(det_ids),
+                                       nat.dptr(det_xy), nat.dptr(bp), nat.dptr(intr), nat.dptr(rt0), nat.dptr(poses),
+                                       ok.ctypes.data_as(C.POINTER(C.c_uint8))))
+    return rt0, poses[:F], ok[:F].astype(bool)
+
   # ---- pose-graph initialisation (include/mcba.h mcba_pose_*) -------------------------------------------------------------------
   @staticmethod
   def _pose_table(poses, valid):
