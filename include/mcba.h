@@ -150,6 +150,13 @@ int  mcba_get_rolling(mcba_ctx* ctx, double* end_pose_matrices);
 int  mcba_set_hand_eye(mcba_ctx* ctx, const double* base_wrt_gripper, const double* world_wrt_base,
                        const double* gripper_wrt_camera);
 int  mcba_get_hand_eye(mcba_ctx* ctx, double* world_wrt_base, double* gripper_wrt_camera);
+/* single intrinsic parameters held fixed (OpenCV's CALIB_FIX_K1..K3, CALIB_ZERO_TANGENT_DIST, CALIB_FIX_PRINCIPAL_POINT, ...):
+ * fixed uint8[5+nd] in Camera.params order [fx fy cx cy skew dist...], 1 = fixed, the same for every camera (NULL = none).  A fixed
+ * parameter keeps its place in param_vec and its current value: its row and column of J^T J and its entry of J^T r are zero
+ * (mcba_linearize shows them), and mcba_solve / mcba_set_param_vec leave it bit for bit.  Harmless without MCBA_OPT_CAMERAS.
+ * Entries other than 0 / 1, or fx and fy fixed apart under MCBA_OPT_FIX_ASPECT (fy follows fx), fail with MCBA_ERR_ARG.  Every upload
+ * clears the mask. */
+int  mcba_set_fixed_intrinsics(mcba_ctx* ctx, const uint8_t* fixed);
 int  mcba_num_params(mcba_ctx* ctx, int64_t* n);      /* length of param_vec for the enabled blocks    */
 int  mcba_get_param_vec(mcba_ctx* ctx, double* x);    /* Parameters.param_vec (parameters.py:44-46)    */
 int  mcba_set_param_vec(mcba_ctx* ctx, const double* x);   /* with_param_vec (parameters.py:48-50)     */

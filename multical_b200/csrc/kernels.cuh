@@ -51,6 +51,8 @@ struct DeviceProblem {
   int n, n_s, n_f;
   int off_cp, off_bp, off_in, off_pt;   // offsets inside shared, -1 when the block is fixed (off_pt: 3 per padded board point)
   int motion_on, fix_aspect;            // motion_on: per-frame blocks are free (static / rolling frames)
+  uint32_t fixed_intr;                  // bit i: entry i of every camera's [fx fy cx cy skew dist...] is held at its current value
+                                        // (mcba_set_fixed_intrinsics): a dead column, like skew's
   int frame_blocks;                     // the linearisation emits H_ff, g_f (at g + n_s) and W_f: motion_on, or hand-eye with free
                                         // hand-eye parameters (k_fold_hand_eye folds the frame blocks into them)
   // motion model (the `motion` argument of Calibration, calibration.py:44-46)
@@ -212,6 +214,7 @@ __device__ __forceinline__ void make_trial_item(const DeviceProblem& p, const do
     for (int j = 0; j < p.kint; j++) {
       double v = __ldcg(&src[j]);
       if (j == 1 && p.fix_aspect && p.off_in >= 0) v = __ldcg(&src[0]);      // fy follows fx (camera.py:159-160)
+      if ((p.fixed_intr >> j) & 1u) v = __ldcg(&p.intr[p.kint * c + j]);     // held fixed: keeps the current value
       dst[j] = v;
     }
   } else if (i < np + p.C + p.B * p.P) {
@@ -401,9 +404,10 @@ __device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double
 __host__ __device__ constexpr int mma_nc(int model, bool roll = false) { return ((model_D(model) + (roll ? 6 : 0) + 1 + 7) / 8) * 8; }
 
 __device__ __forceinline__ int intr_param_index(const DeviceProblem& p, int local /*0..3+nd*/) {
-  // local [fx fy cx cy dist...] -> index in [fx fy cx cy skew dist...]; fix_aspect folds fy onto fx (camera.py:159-160)
-  if (local == 1 && p.fix_aspect) return 0;
-  return local < 4 ? local : local + 1;
+  // local [fx fy cx cy dist...] -> index in [fx fy cx cy skew dist...]; fix_aspect folds fy onto fx (camera.py:159-160); -1 for a
+  // parameter held fixed (DeviceProblem::fixed_intr): its column is zero, and every caller skips it
+  const int q = (local == 1 && p.fix_aspect) ? 0 : local < 4 ? local : local + 1;
+  return ((p.fixed_intr >> q) & 1u) ? -1 : q;
 }
 
 __device__ __forceinline__ void view_chain(const PoseT& pc, const PoseT& pf, double* Rcf, double* tcf) {
@@ -532,7 +536,8 @@ k_point_blocks(DeviceProblem p, ViewKernelArgs a, double* Hss, double* W, double
 #pragma unroll
           for (int i = 0; i < NIN; i++) {
             const double val = xu[r] * gu[KO + i] + xv[r] * gv[KO + i];
-            if (val != 0.0) addS(pt + r, in0 + intr_param_index(p, i), val);
+            const int q = intr_param_index(p, i);
+            if (val != 0.0 && q >= 0) addS(pt + r, in0 + q, val);
           }
         }
       }

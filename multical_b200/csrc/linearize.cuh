@@ -237,8 +237,10 @@ __device__ __forceinline__ void lin_flush_wacc(const DeviceProblem& p, const Lin
       const int i = o / FB, col = o % FB;
       const double val = wacc[(KO + i) * FB + col];
       if (p.fix_aspect && i == 1) { Wf[(size_t)(p.off_in + p.kint * cam + 1) * FB + col] = 0.0; continue; }      // fy follows fx (camera.py:159-160): folded onto fx, its own row is dead
+      const int q = intr_param_index(p, i);
+      if (q < 0) { Wf[(size_t)(p.off_in + p.kint * cam + (i < 4 ? i : i + 1)) * FB + col] = 0.0; continue; }      // held fixed: dead row
       const double v2 = (p.fix_aspect && i == 0) ? val + wacc[(KO + 1) * FB + col] : val;
-      Wf[(size_t)(p.off_in + p.kint * cam + intr_param_index(p, i)) * FB + col] = v2;
+      Wf[(size_t)(p.off_in + p.kint * cam + q) * FB + col] = v2;
     }
     for (int col = lane; col < FB; col += 32) Wf[(size_t)(p.off_in + p.kint * cam + 4) * FB + col] = 0.0;             // skew: ignored by cv2.projectPoints, dead column
   }
@@ -745,7 +747,8 @@ k_reduce_shared(DeviceProblem p, ReduceArgs a) {
     }
   }
   if (in0 >= 0) {
-    // one thread per TARGET parameter pair: rows folded onto one parameter (fix_aspect: fy onto fx, camera.py:159-160) are added in a fixed order
+    // one thread per TARGET parameter pair: rows folded onto one parameter (fix_aspect: fy onto fx, camera.py:159-160) are added in a fixed order;
+    // a parameter held fixed maps to -1, which no target matches: its row, column and gradient entry are written as zero
     const int kint = p.kint;
     if (cp >= 0)
       for (int o = tid; o < kint * 6; o += RED_THREADS) {

@@ -1959,6 +1959,23 @@ int mcba_get_hand_eye(mcba_ctx* ctx, double* world_wrt_base, double* gripper_wrt
   return MCBA_OK;
 }
 
+// OpenCV's CALIB_FIX_* flags: intrinsic parameters held at their current values.  The mask lives in the problem descriptor that every
+// launch takes by value (and so in the key of the solve's cached graph); setup_problem clears it on every upload.
+int mcba_set_fixed_intrinsics(mcba_ctx* ctx, const uint8_t* fixed) {
+  if (!ctx) return MCBA_ERR_ARG;
+  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "mcba_upload has not been called");
+  DeviceProblem& P = ctx->P;
+  uint32_t m = 0;
+  for (int i = 0; fixed && i < P.kint; i++) {
+    REQUIRE(fixed[i] <= 1, MCBA_ERR_ARG, "fixed intrinsics: every entry must be 0 or 1");
+    if (fixed[i]) m |= 1u << i;
+  }
+  REQUIRE(!P.fix_aspect || (m & 1u) == ((m >> 1) & 1u), MCBA_ERR_ARG,
+          "fixed intrinsics: under MCBA_OPT_FIX_ASPECT fy follows fx, so fx and fy are fixed together or not at all");
+  P.fixed_intr = m;
+  return MCBA_OK;
+}
+
 int mcba_get_params(mcba_ctx* ctx, double* cam_rt, double* board_rt, double* frame_rt, double* intrinsics) {
   if (!ctx) return MCBA_ERR_ARG;
   REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "mcba_upload has not been called");

@@ -457,6 +457,16 @@ class Engine:
     self._ck(self.lib.mcba_get_hand_eye(self.h, nat.dptr(w), nat.dptr(g)))
     return w, g
 
+  def set_fixed_intrinsics(self, fixed):
+    """Hold single intrinsic parameters at their current values (OpenCV's CALIB_FIX_* flags): fixed bool[5+nd] in Camera.params order
+    [fx fy cx cy skew dist...], shared by every camera; None = none.  The next upload clears it (include/mcba.h)."""
+    if fixed is None:
+      self._ck(self.lib.mcba_set_fixed_intrinsics(self.h, None))
+      return
+    m = np.ascontiguousarray(fixed, dtype=np.uint8)
+    assert m.shape == (self.kint,), f"fixed intrinsics: expected {self.kint} entries, got {m.shape}"
+    self._ck(self.lib.mcba_set_fixed_intrinsics(self.h, m.ctypes.data_as(C.POINTER(C.c_uint8))))
+
   def get_params(self):
     d = self.desc
     out = (np.zeros((d.C, 6)), np.zeros((d.B, 6)), np.zeros((max(d.F, 1), 6)), np.zeros((d.C, self.kint)))

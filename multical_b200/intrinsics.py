@@ -18,7 +18,10 @@ the process-wide bundle-adjustment engine keeps its problem.
 
 The fisheye model (CameraFisheye.calibrate / calibrate_cameras_fisheye, camera_fisheye.py:70-94, 173-177: one cv2.fisheye.calibrate per
 camera, no loop) takes the same steps once: the same view set, OpenCV's fisheye start K0 with per-view poses by fisheye PnP under it
-(mcba_intrinsic_init), the same one-camera problem without an aspect constraint, and the total RMS as err."""
+(mcba_intrinsic_init), the same one-camera problem without an aspect constraint, and the total RMS as err.
+
+Both paths take OpenCV's fixed-parameter `flags` (CALIB_FIX_K1.., CALIB_FIX_PRINCIPAL_POINT, ...; pinhole_flags, fisheye_flags) as the
+engine's fixed-intrinsics mask: the parameters they name keep K0's values, which are OpenCV's without an intrinsic guess."""
 import numpy as np
 
 from . import _native as nat
@@ -30,13 +33,46 @@ SUPPORTED_MODELS = ("standard",)
 UNSUPPORTED = {
   "rational": "k1..k3 and k4..k6 are nearly degenerate; in that valley the engine's trust region stops on xtol 1.7e-4 - 1.8e-4 above the "
               "RMS OpenCV's LM settles at (50-view scenes, restarts do not help), so the result would not be OpenCV's minimum",
-  "thin_prism": "under CALIB_THIN_PRISM_MODEL OpenCV keeps k4..k6 at zero, and the engine cannot fix single distortion coefficients",
-  "tilted": "under CALIB_TILTED_MODEL OpenCV keeps k4..k6 and s1..s4 at zero, and the engine cannot fix single distortion coefficients",
+  "thin_prism": "under CALIB_THIN_PRISM_MODEL OpenCV keeps k4..k6 at zero; the engine's fixed-intrinsics mask can hold them, but this "
+                "model's free-intrinsics solve is not checked against OpenCV yet",
+  "tilted": "under CALIB_TILTED_MODEL OpenCV keeps k4..k6 and s1..s4 at zero; the engine's fixed-intrinsics mask can hold them, but this "
+            "model's free-intrinsics solve is not checked against OpenCV yet",
   "fisheye": "fisheye cameras calibrate with calibrate_cameras_fisheye / CameraFisheye.calibrate (the reference's camera_fisheye.py "
              "signature: no intrinsic_error_limit, no rejection loop)",
 }
 # CameraFisheye.model (camera_fisheye.py:43-49): stored on the camera; the reference never passes them to OpenCV's flags
 FISHEYE_MODELS = ("standard", "fix_k1", "fix_k2", "fix_k3", "fix_k4")
+
+# The `flags` the reference ORs into OpenCV's (camera.py:81, camera_fisheye.py:80), as the engine's fixed-intrinsics mask
+# (mcba_set_fixed_intrinsics): flag bit -> (OpenCV's name, indices into Camera.params [fx fy cx cy skew dist...]).  Without an intrinsic
+# guess OpenCV holds a fixed distortion coefficient at 0 and a fixed principal point at its start, which are K0's values; the fisheye
+# focal lengths' start max(w, h) / 2 is K0's too.
+PINHOLE_FIXED = {
+  4: ("CALIB_FIX_PRINCIPAL_POINT", (2, 3)), 8: ("CALIB_ZERO_TANGENT_DIST", (7, 8)), 32: ("CALIB_FIX_K1", (5,)),
+  64: ("CALIB_FIX_K2", (6,)), 128: ("CALIB_FIX_K3", (9,)),
+  1 << 21: ("CALIB_FIX_TANGENT_DIST", (7, 8)),       # holds p1, p2 at their start, 0 without a guess: ZERO_TANGENT_DIST (OpenCV 4.13)
+}
+PINHOLE_FIX_ASPECT_RATIO = 2                          # the same as fix_aspect=True
+PINHOLE_NO_EFFECT = {2048: "CALIB_FIX_K4", 4096: "CALIB_FIX_K5", 8192: "CALIB_FIX_K6", 65536: "CALIB_FIX_S1_S2_S3_S4",
+                     524288: "CALIB_FIX_TAUX_TAUY"}     # coefficients the standard model does not have
+FISHEYE_FIXED = {
+  16: ("CALIB_FIX_K1", (5,)), 32: ("CALIB_FIX_K2", (6,)), 64: ("CALIB_FIX_K3", (7,)), 128: ("CALIB_FIX_K4", (8,)),
+  512: ("CALIB_FIX_PRINCIPAL_POINT", (2, 3)), 2048: ("CALIB_FIX_FOCAL_LENGTH", (0, 1)),
+}
+FISHEYE_NO_EFFECT = {2: "CALIB_RECOMPUTE_EXTRINSIC", 8: "CALIB_FIX_SKEW"}      # the reference sets both itself
+_NO_GUESS = "the reference passes no initial camera matrix (camera.py:86-88, camera_fisheye.py:91-92), so there is no guess to use"
+PINHOLE_REFUSED = {
+  1: ("CALIB_USE_INTRINSIC_GUESS", _NO_GUESS),
+  16: ("CALIB_FIX_FOCAL_LENGTH", "OpenCV holds fx, fy at its own initCameraMatrix2D start, which K0 matches only to 1e-3 relative, so "
+                                 "the held focal lengths and the whole fit would differ from OpenCV's"),
+  16384: ("CALIB_RATIONAL_MODEL", "the camera model comes from `model`; this flag contradicts model='standard'"),
+  32768: ("CALIB_THIN_PRISM_MODEL", "the camera model comes from `model`; this flag contradicts model='standard'"),
+  262144: ("CALIB_TILTED_MODEL", "the camera model comes from `model`; this flag contradicts model='standard'"),
+}
+FISHEYE_REFUSED = {
+  1: ("CALIB_USE_INTRINSIC_GUESS", _NO_GUESS),
+  4: ("CALIB_CHECK_COND", "OpenCV's condition-number check of every view's extrinsic Jacobian is not implemented"),
+}
 
 _engines = {}
 
@@ -83,15 +119,41 @@ def calibration_points(boards, detections):
   return views
 
 
-def _check_model(model, flags):
+def _check_model(model):
   if model in UNSUPPORTED:
     raise NotImplementedError(f"intrinsic calibration of the {model} model: {UNSUPPORTED[model]}")
   assert model in SUPPORTED_MODELS, f"unknown camera model {model}"
-  if flags:
-    raise NotImplementedError(f"extra OpenCV calibration flags ({flags}) are not supported")
 
 
-def _solve_camera(eng, model, fix_aspect, views, k0, poses, board_points, solve_opts):
+def fixed_of_flags(flags, kint, fixed_bits, no_effect, refused, what):
+  """OpenCV calibration flags -> the fixed-intrinsics mask bool[kint] (None when nothing is fixed).  A refused, unknown or unsupported
+  bit raises NotImplementedError naming it."""
+  flags = int(flags)
+  for bit, (name, reason) in refused.items():
+    if flags & bit: raise NotImplementedError(f"{what} flag {name} ({bit}) is not supported: {reason}")
+  fixed = np.zeros(kint, bool)
+  rest = flags
+  for bit, (_, idx) in fixed_bits.items():
+    if flags & bit: fixed[list(idx)] = True
+    rest &= ~bit
+  for bit in no_effect: rest &= ~bit
+  if rest: raise NotImplementedError(f"{what} flag bits {rest} ({rest:#x}) are not supported flags of this calibration")
+  return fixed if fixed.any() else None
+
+
+def pinhole_flags(flags, model="standard"):
+  """calibrateCamera flags -> (fixed-intrinsics mask or None, whether they fix the aspect ratio)."""
+  fixed = fixed_of_flags(flags, 5 + nat.DIST_SIZES[model], PINHOLE_FIXED, set(PINHOLE_NO_EFFECT) | {PINHOLE_FIX_ASPECT_RATIO},
+                         PINHOLE_REFUSED, "calibrateCamera")
+  return fixed, bool(int(flags) & PINHOLE_FIX_ASPECT_RATIO)
+
+
+def fisheye_flags(flags):
+  """cv2.fisheye.calibrate flags -> fixed-intrinsics mask or None."""
+  return fixed_of_flags(flags, 5 + nat.DIST_SIZES["fisheye"], FISHEYE_FIXED, FISHEYE_NO_EFFECT, FISHEYE_REFUSED, "cv2.fisheye.calibrate")
+
+
+def _solve_camera(eng, model, fix_aspect, views, k0, poses, board_points, solve_opts, fixed=None):
   """One calibrateCameraExtended: the views as frames of a one-camera problem, started from K0 and the PnP poses."""
   nv = len(views)
   B, P = board_points.shape[:2]
@@ -101,7 +163,8 @@ def _solve_camera(eng, model, fix_aspect, views, k0, poses, board_points, solve_
   bits = nat.OPT_BITS["motion"] | nat.OPT_BITS["cameras"] | (nat.OPT_FIX_ASPECT if fix_aspect else 0)
   eng.upload(model, bits, (1, nv, B, P), rows, obs, board_points)
   mats = np.concatenate([np.eye(4)[None], np.tile(np.eye(4), (B, 1, 1)), poses])
-  eng.set_state_matrices(mats, k0[None])
+  eng.set_state_matrices(mats, k0[None])          # K0: zero distortion, and the principal point OpenCV holds fixed
+  if fixed is not None: eng.set_fixed_intrinsics(fixed)
   info = eng.solve(**solve_opts)
   sumsq, count = eng.view_errors()
   per_view = np.array([sumsq[0, i, v.board] for i, v in enumerate(views)])
@@ -131,10 +194,12 @@ def init_views(boards, cam_views, image_sizes, model="standard", fix_aspect=Fals
   return eng.intrinsic_init(model, (Cn, F, B, P), det_start, det_ids, det_xy, board_points, grid, image_sizes, use, fix_aspect)
 
 
-def calibrate_views(boards, cam_views, image_sizes, model="standard", fix_aspect=False, engine=None, camera_ids=None, **solve_opts):
+def calibrate_views(boards, cam_views, image_sizes, model="standard", fix_aspect=False, engine=None, camera_ids=None, fixed=None,
+                    **solve_opts):
   """One calibrateCameraExtended (model "fisheye": one cv2.fisheye.calibrate) for each camera's list of views (calibration_points
   entries, any order): returns per camera a struct of the intrinsics [fx fy cx cy skew dist...], the views' rtvecs (board wrt camera),
-  per-view RMS, total RMS, K0 and the solve summary.  camera_ids: how errors name the cameras (default: their position in cam_views)."""
+  per-view RMS, total RMS, K0 and the solve summary.  camera_ids: how errors name the cameras (default: their position in cam_views).
+  fixed: bool[5+nd], the intrinsics held at K0's values (fixed_of_flags; None: all free)."""
   eng = engine or intrinsics_engine()
   opts = dict(ftol=1e-10, xtol=1e-10, gtol=1e-10, max_nfev=100)
   opts.update(solve_opts)
@@ -149,7 +214,8 @@ def calibrate_views(boards, cam_views, image_sizes, model="standard", fix_aspect
     failed = [(f, b) for f, b in sel if not ok[c, f, b]]
     if failed:
       raise ValueError(f"camera {names[c]}: the initial pose of the view (frame {failed[0][0]}, board {failed[0][1]}) failed")
-    res = _solve_camera(eng, model, fix_aspect, views, k0[c], np.stack([poses[c, f, b] for f, b in sel]), board_points, opts)
+    res = _solve_camera(eng, model, fix_aspect, views, k0[c], np.stack([poses[c, f, b] for f, b in sel]), board_points, opts,
+                       fixed)
     res.k0 = k0[c]
     out.append(res)
   return out
@@ -170,7 +236,9 @@ def calibrate_cameras(boards, points, image_sizes, intrinsic_error_limit, max_it
   `max_iter` / `eps` are accepted for the reference's signature: the device solves to its own tolerances (module docstring); the keyword
   arguments ftol, xtol, gtol, max_nfev go to the solve."""
   del max_iter, eps
-  _check_model(model, flags)
+  _check_model(model)
+  fixed, flag_aspect = pinhole_flags(flags, model)
+  aspect = fix_aspect or flag_aspect          # the returned Camera keeps the fix_aspect it was given, as the reference's does
   Cn = len(points)
   views, err, result, per_view = [], [None] * Cn, [None] * Cn, [None] * Cn
   for c in range(Cn):
@@ -182,8 +250,8 @@ def calibrate_cameras(boards, points, image_sizes, intrinsic_error_limit, max_it
     views.append(v)
   active = list(range(Cn))
   while active:
-    res = calibrate_views(boards, [views[c] for c in active], [image_sizes[c] for c in active], model, fix_aspect, camera_ids=active,
-                          **solve_opts)
+    res = calibrate_views(boards, [views[c] for c in active], [image_sizes[c] for c in active], model, aspect, camera_ids=active,
+                          fixed=fixed, **solve_opts)
     still = []
     for c, r in zip(active, res):
       result[c], per_view[c] = r, r.per_view
@@ -221,8 +289,7 @@ def calibrate_cameras_fisheye(boards, points, image_sizes, max_iter=10, eps=1e-3
   from .camera import CameraFisheye
   del max_iter, eps
   assert model in FISHEYE_MODELS, f"unknown camera model {model} options are {list(FISHEYE_MODELS)}"
-  if flags:
-    raise NotImplementedError(f"extra OpenCV calibration flags ({flags}) are not supported")
+  fixed = fisheye_flags(flags)
   views = []
   for c in range(len(points)):
     v = calibration_points(boards, points[c])
@@ -231,7 +298,7 @@ def calibrate_cameras_fisheye(boards, points, image_sizes, max_iter=10, eps=1e-3
     if max_images is not None:
       v = top_detection_coverage(v, max_images, image_sizes[c])
     views.append(v)
-  res = calibrate_views(boards, views, image_sizes, model="fisheye", fix_aspect=False, **solve_opts)
+  res = calibrate_views(boards, views, image_sizes, model="fisheye", fix_aspect=False, fixed=fixed, **solve_opts)
   cams = []
   for r, size in zip(res, image_sizes):
     x = r.intrinsics

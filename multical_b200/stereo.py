@@ -24,8 +24,10 @@ from .structs import struct
 FREE_INTRINSIC_MODELS = ("standard", "fisheye")
 UNSUPPORTED_FREE = {
   "rational": "k1..k3 and k4..k6 are nearly degenerate, and the engine's trust region stops short of OpenCV's minimum (DESIGN.md §3d)",
-  "thin_prism": "under CALIB_THIN_PRISM_MODEL OpenCV keeps k4..k6 at zero, and the engine cannot fix single distortion coefficients",
-  "tilted": "under CALIB_TILTED_MODEL OpenCV keeps k4..k6 and s1..s4 at zero, and the engine cannot fix single distortion coefficients",
+  "thin_prism": "under CALIB_THIN_PRISM_MODEL OpenCV keeps k4..k6 at zero; the engine's fixed-intrinsics mask can hold them, but this "
+                "model's free-intrinsics solve is not checked against OpenCV yet",
+  "tilted": "under CALIB_TILTED_MODEL OpenCV keeps k4..k6 and s1..s4 at zero; the engine's fixed-intrinsics mask can hold them, but this "
+            "model's free-intrinsics solve is not checked against OpenCV yet",
 }
 
 
