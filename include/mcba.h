@@ -335,6 +335,27 @@ int  mcba_project_points(mcba_ctx* ctx, int32_t model, const double* camera, int
 int  mcba_undistort_points(mcba_ctx* ctx, int32_t model, const double* camera, int64_t n, const double* pixels, double* undistorted);
 int  mcba_remap_cubic_table(mcba_ctx* ctx, int32_t* table);
 
+/* -- rectifying a calibrated pair (cv2.initUndistortRectifyMap / cv2.undistortPoints with R and P, after cv2.stereoRectify) ---------------
+ * camera as above; R f64[9] (the rectifying rotation, row-major) and P f64[9] (the left 3x3 of the new projection matrix, row-major).
+ * mcba_rectify_map: cv2.initUndistortRectifyMap(K, dist, R, P, (width, height), CV_32FC2) (cv2.fisheye.initUndistortRectifyMap for
+ *   MCBA_MODEL_FISHEYE; its two CV_32F maps interleaved).  The normalised point of pixel (u, v) of row v is OpenCV's walk along the row
+ *   from (P R)^-1 (0, v, 1) in steps of (P R)^-1 (1, 0, 0): blocks of 8 pixels for the pinhole models, one pixel at a time for the
+ *   fisheye, as OpenCV's own loops round it.  (width, height) is the rectified image's size, which need not be the camera's.  The map
+ *   stays resident like an undistortion map, keyed by the camera, R, P and the size; map receives the float map when not NULL.  Fisheye
+ *   maps may be at most 8533 pixels wide, pinhole maps about 68000.
+ * mcba_rectify_images: mcba_undistort_images through the rectification map of (R, P, width, height).
+ * mcba_rectify_points: cv2.undistortPoints(pixels, K, dist, R = R, P = P) (cv2.fisheye.undistortPoints(pixels, K, dist, R, P)):
+ *   f64[n][2] -> f64[n][2].  P = I gives normalised coordinates in the rectified frame.
+ * (P R)^-1 comes from 3x3 Gaussian elimination with partial pivoting on the host: a singular P R fails with MCBA_ERR_ARG.  Non-finite
+ * camera parameters, R or P fail with MCBA_ERR_NONFINITE.  None of these touches the uploaded problem. */
+int  mcba_rectify_map(mcba_ctx* ctx, int32_t model, const double* camera, const double* R, const double* P, int32_t width,
+                      int32_t height, float* map);
+int  mcba_rectify_images(mcba_ctx* ctx, int32_t model, const double* camera, const double* R, const double* P, int32_t width,
+                         int32_t height, int32_t n, int32_t src_width, int32_t src_height, int32_t channels, int32_t dtype,
+                         const uint8_t* const* src, uint8_t* const* dst);
+int  mcba_rectify_points(mcba_ctx* ctx, int32_t model, const double* camera, const double* R, const double* P, int64_t n,
+                         const double* pixels, double* rectified);
+
 /* -- measurement hooks (bench.py): launch one kernel family on the context stream -------------- */
 enum { MCBA_BENCH_LINEARIZE = 0, MCBA_BENCH_RESIDUAL = 1, MCBA_BENCH_COST = 2,
        MCBA_BENCH_NO_PREPARE = 256 /* or-ed in: reuse the pose tables of the previous call (times the kernel alone) */ };

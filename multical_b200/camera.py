@@ -75,6 +75,17 @@ class Camera(Parameters):
     from .undistort import project
     return project(self, points)
 
+  def rectify_map(self, R, P, size=None):
+    """float32 [h, w, 2] of cv2.initUndistortRectifyMap(K, dist, R, P, size) on the GPU (multical_b200/rectify.py); size defaults to
+    image_size."""
+    from .rectify import rectify_map
+    return rectify_map(self, R, P, size)
+
+  def rectify_points(self, points, R, P):
+    """cv2.undistortPoints(points, K, dist, R=R, P=P) on the GPU over any leading shape [..., 2]."""
+    from .rectify import rectify_points
+    return rectify_points(self, points, R, P)
+
   def approx_eq(self, other):
     return self.image_size == other.image_size and np.allclose(other.intrinsic, self.intrinsic) and np.allclose(other.dist, self.dist)
 
@@ -138,6 +149,24 @@ def undistort_images(images, cameras, j=None, chunksize=4):
   """camera.py:247-258 on the GPU (multical_b200/undistort.py): per camera, its images remapped through its undistortion map."""
   from .undistort import undistort_images
   return undistort_images(images, cameras, j=j, chunksize=chunksize)
+
+
+def stereo_rectify(left, right, pose, alpha=-1, new_size=None, zero_disparity=True):
+  """cv2.stereoRectify of a calibrated pinhole pair on the GPU (multical_b200/rectify.py): struct(R1, R2, P1, P2, Q, roi1, roi2)."""
+  from .rectify import stereo_rectify
+  return stereo_rectify(left, right, pose, alpha=alpha, new_size=new_size, zero_disparity=zero_disparity)
+
+
+def stereo_rectify_fisheye(left, right, pose, zero_disparity=True, new_size=None, balance=0.0, fov_scale=1.0):
+  """cv2.fisheye.stereoRectify of a calibrated fisheye pair on the GPU (multical_b200/rectify.py): struct(R1, R2, P1, P2, Q)."""
+  from .rectify import stereo_rectify_fisheye
+  return stereo_rectify_fisheye(left, right, pose, zero_disparity=zero_disparity, new_size=new_size, balance=balance, fov_scale=fov_scale)
+
+
+def rectify_images(images, cameras, rectifications, size=None):
+  """Per camera, its images remapped through its rectification map under rectifications[k] = (R, P) (multical_b200/rectify.py)."""
+  from .rectify import rectify_images
+  return rectify_images(images, cameras, rectifications, size=size)
 
 
 def engine_model_of(camera):

@@ -10,6 +10,7 @@
 #include <cstdlib>
 #include <string>
 #include <chrono>
+#include <functional>
 #include <type_traits>
 #include <memory>
 #include <vector>
@@ -709,6 +710,10 @@ int mcba_create(int device, mcba_ctx** out) {
   cudaFuncSetAttribute(k_lm<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
   cudaFuncSetAttribute(k_lm<12>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
   cudaFuncSetAttribute(k_pose_align<PI_SMALL_THREADS, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, PI_SMALL_MAX * PI_ROW_BYTES);
+  for (int model = MODEL_STANDARD; model <= MODEL_TILTED; model++)
+    with_model(model, false, [](auto M, auto) {
+      cudaFuncSetAttribute(k_rectify_map<decltype(M)::value>, cudaFuncAttributeMaxDynamicSharedMemorySize, RECT_SMEM_MAX);
+    });
   *out = ctx;
   return MCBA_OK;
 }
@@ -1511,15 +1516,19 @@ int ensure_cubic_table(mcba_ctx* ctx) {
   return MCBA_OK;
 }
 
-// the resident fixed-point map of a camera, computed on ctx->stream when it is not resident yet (or when the float map is asked for)
-int resident_map(mcba_ctx* ctx, int model, const double* camera, int w, int h, float* map_out, mcba_ctx::UndistortMap** out) {
+// the resident fixed-point map of a key, computed on ctx->stream by launch(float map or null, org, idx) when it is not resident yet (or
+// when the float map is asked for).  The key is the camera vector for an undistortion map, the camera vector followed by R and P for a
+// rectification map: its length tells the two apart.
+int resident_map(mcba_ctx* ctx, int model, const double* key, size_t nk, int w, int h, float* map_out,
+                 const std::function<void(float2*, uint32_t*, uint16_t*)>& launch, mcba_ctx::UndistortMap** out) {
   auto& U = ctx->und;
   cudaStream_t s = ctx->stream;
   { int r = ensure_cubic_table(ctx); if (r) return r; }
-  const size_t nk = 5 + (size_t)model_nd(model), npx = (size_t)w * h;
+  const size_t npx = (size_t)w * h;
   mcba_ctx::UndistortMap* m = nullptr;
   for (auto& e : U.maps)
-    if (e->model == model && e->w == w && e->h == h && std::memcmp(e->cam.data(), camera, nk * sizeof(double)) == 0) m = e.get();
+    if (e->model == model && e->w == w && e->h == h && e->cam.size() == nk && std::memcmp(e->cam.data(), key, nk * sizeof(double)) == 0)
+      m = e.get();
   if (!m || map_out) {
     if (!m) {
       if (U.maps.size() >= (size_t)mcba_ctx::UND_MAX_MAPS) {
@@ -1533,14 +1542,10 @@ int resident_map(mcba_ctx* ctx, int model, const double* camera, int w, int h, f
     }
     float2* f = nullptr;
     if (map_out) { CK(U.fmap.alloc(npx)); f = U.fmap.p; }
-    const UndistortCamera c = make_camera(model, camera, w, h);
-    const dim3 grid((w + UND_THREADS - 1) / UND_THREADS, h);
-    with_model(model, false, [&](auto M, auto) {
-      k_undistort_map<decltype(M)::value><<<grid, UND_THREADS, 0, s>>>(c, f, m->org.p, m->idx.p);
-    });
+    launch(f, m->org.p, m->idx.p);
     m->model = -1;                                 // not usable until the launch is known to have gone in
     CKL();
-    m->model = model; m->w = w; m->h = h; m->cam.assign(camera, camera + nk);
+    m->model = model; m->w = w; m->h = h; m->cam.assign(key, key + nk);
     if (map_out) {
       CK(cudaMemcpyAsync(map_out, f, sizeof(float2) * npx, cudaMemcpyDeviceToHost, s));
       CK(cudaStreamSynchronize(s));
@@ -1551,66 +1556,68 @@ int resident_map(mcba_ctx* ctx, int model, const double* camera, int w, int h, f
   return MCBA_OK;
 }
 
-// point entries: copy in, one thread per point, copy out
-int run_points(mcba_ctx* ctx, bool project, int32_t model, const double* camera, int64_t n, const double* in, double* out) {
-  if (!ctx) return MCBA_ERR_ARG;
-  CK(cudaSetDevice(ctx->device));
-  { int r = check_camera(ctx, model, camera); if (r) return r; }
-  REQUIRE(n >= 0, MCBA_ERR_ARG, "negative point count");
-  if (n == 0) return MCBA_OK;
-  REQUIRE(in && out, MCBA_ERR_ARG, "null argument");
-  auto& U = ctx->und;
+// the resident undistortion map of a camera (k_undistort_map)
+int undistortion_map(mcba_ctx* ctx, int model, const double* camera, int w, int h, float* map_out, mcba_ctx::UndistortMap** out) {
+  const UndistortCamera c = make_camera(model, camera, w, h);
+  const dim3 grid((w + UND_THREADS - 1) / UND_THREADS, h);
   cudaStream_t s = ctx->stream;
-  const size_t din = project ? 3 : 2;
-  CK(U.pin.alloc(din * n)); CK(U.pout.alloc(2 * (size_t)n));
-  CK(cudaMemcpyAsync(U.pin.p, in, sizeof(double) * din * n, cudaMemcpyHostToDevice, s));
-  const UndistortCamera c = make_camera(model, camera, 0, 0);
-  const unsigned blocks = (unsigned)((n + UND_THREADS - 1) / UND_THREADS);
-  with_model(model, false, [&](auto M, auto) {
-    constexpr int MODEL = decltype(M)::value;
-    if (project) k_project_points<MODEL><<<blocks, UND_THREADS, 0, s>>>(c, n, U.pin.p, U.pout.p);
-    else k_undistort_points<MODEL><<<blocks, UND_THREADS, 0, s>>>(c, n, U.pin.p, U.pout.p);
-  });
-  CKL();
-  CK(cudaMemcpyAsync(out, U.pout.p, sizeof(double) * 2 * n, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
+  return resident_map(ctx, model, camera, 5 + (size_t)model_nd(model), w, h, map_out, [&](float2* f, uint32_t* org, uint16_t* idx) {
+    with_model(model, false, [&](auto M, auto) { k_undistort_map<decltype(M)::value><<<grid, UND_THREADS, 0, s>>>(c, f, org, idx); });
+  }, out);
+}
+
+// rr = P R and ir = rr^-1 (row-major 3x3) for the rectification entries; a singular or non-finite P R fails with MCBA_ERR_ARG
+int make_rectify_camera(mcba_ctx* ctx, int model, const double* camera, const double* R, const double* P, int w, int h, RectifyCamera& rc) {
+  REQUIRE(R && P, MCBA_ERR_ARG, "null R or P");
+  REQUIRE(all_finite(R, 9) && all_finite(P, 9), MCBA_ERR_NONFINITE, "non-finite R or P");
+  rc.cam = make_camera(model, camera, w, h);
+  for (int i = 0; i < 3; i++)
+    for (int j = 0; j < 3; j++) rc.rr[3 * i + j] = P[3 * i] * R[j] + P[3 * i + 1] * R[3 + j] + P[3 * i + 2] * R[6 + j];
+  // Gauss-Jordan elimination with partial pivoting on [rr | I]
+  double A[3][3], I[3][3];
+  for (int i = 0; i < 3; i++)
+    for (int j = 0; j < 3; j++) { A[i][j] = rc.rr[3 * i + j]; I[i][j] = i == j ? 1.0 : 0.0; }
+  for (int c = 0; c < 3; c++) {
+    int p = c;
+    for (int r = c + 1; r < 3; r++) if (std::fabs(A[r][c]) > std::fabs(A[p][c])) p = r;
+    REQUIRE(A[p][c] != 0.0, MCBA_ERR_ARG, "P R is singular");
+    for (int j = 0; j < 3; j++) { std::swap(A[c][j], A[p][j]); std::swap(I[c][j], I[p][j]); }
+    for (int r = 0; r < 3; r++) {
+      if (r == c) continue;
+      const double f = A[r][c] / A[c][c];
+      for (int j = 0; j < 3; j++) { A[r][j] -= f * A[c][j]; I[r][j] -= f * I[c][j]; }
+    }
+  }
+  for (int i = 0; i < 3; i++)
+    for (int j = 0; j < 3; j++) rc.ir[3 * i + j] = I[i][j] / A[i][i];
+  REQUIRE(all_finite(rc.ir, 9), MCBA_ERR_ARG, "P R is singular");
   return MCBA_OK;
 }
 
-}  // namespace
+// shared memory of a k_rectify_map CTA
+size_t rectify_smem(int model, int w) { return 3 * sizeof(double) * (size_t)rectify_walk_len(model, w); }
 
-// initUndistortRectifyMap(K, dist, None, K, (width, height)) of one camera, kept resident for mcba_undistort_images
-int mcba_undistort_map(mcba_ctx* ctx, int32_t model, const double* camera, int32_t width, int32_t height, float* map) {
-  if (!ctx) return MCBA_ERR_ARG;
-  CK(cudaSetDevice(ctx->device));
-  { int r = check_camera(ctx, model, camera); if (r) return r; }
-  REQUIRE(width > 0 && height > 0 && height <= 65535, MCBA_ERR_ARG, "map size out of range");
-  mcba_ctx::UndistortMap* m = nullptr;
-  int r = resident_map(ctx, model, camera, width, height, map, &m);
-  if (r) return r;
-  CK(cudaStreamSynchronize(ctx->stream));
-  return MCBA_OK;
+// the resident rectification map of a camera under (R, P) (k_rectify_map)
+int rectification_map(mcba_ctx* ctx, int model, const double* camera, const double* R, const double* P, int w, int h, float* map_out,
+                      mcba_ctx::UndistortMap** out) {
+  RectifyCamera rc;
+  { int r = make_rectify_camera(ctx, model, camera, R, P, w, h, rc); if (r) return r; }
+  const size_t smem = rectify_smem(model, w);
+  REQUIRE(smem <= (size_t)RECT_SMEM_MAX, MCBA_ERR_ARG, "map too wide for one row's walk in shared memory");
+  const size_t nk = 5 + (size_t)model_nd(model);
+  std::vector<double> key(camera, camera + nk);
+  key.insert(key.end(), R, R + 9); key.insert(key.end(), P, P + 9);
+  cudaStream_t s = ctx->stream;
+  return resident_map(ctx, model, key.data(), key.size(), w, h, map_out, [&](float2* f, uint32_t* org, uint16_t* idx) {
+    with_model(model, false, [&](auto M, auto) { k_rectify_map<decltype(M)::value><<<h, UND_THREADS, smem, s>>>(rc, f, org, idx); });
+  }, out);
 }
 
-// cv2.remap(src[i], map, None, INTER_CUBIC) for n images of one camera, host to host.  Chunks of images go through pinned staging
-// on UND_STREAMS streams in turn: while the host copies one chunk into its staging buffer, earlier chunks are in flight (copy in,
-// k_remap_cubic, copy out) on the other streams.
-int mcba_undistort_images(mcba_ctx* ctx, int32_t model, const double* camera, int32_t width, int32_t height, int32_t n,
-                          int32_t src_width, int32_t src_height, int32_t channels, int32_t dtype, const uint8_t* const* src,
-                          uint8_t* const* dst) {
-  if (!ctx) return MCBA_ERR_ARG;
-  CK(cudaSetDevice(ctx->device));
-  { int r = check_camera(ctx, model, camera); if (r) return r; }
-  REQUIRE(dtype == MCBA_IMAGE_UINT8, MCBA_ERR_ARG, "unsupported image dtype: only 8-bit unsigned images are remapped");
-  REQUIRE(channels == 1 || channels == 3, MCBA_ERR_ARG, "unsupported channel count: 1 or 3 channels are remapped");
-  REQUIRE(width > 0 && height > 0 && height <= 65535, MCBA_ERR_ARG, "map size out of range");
-  REQUIRE(src_width > 0 && src_height > 0, MCBA_ERR_ARG, "empty source image");
-  REQUIRE(n >= 0, MCBA_ERR_ARG, "negative image count");
-  if (n == 0) return MCBA_OK;
-  REQUIRE(src && dst, MCBA_ERR_ARG, "null image list");
-  for (int i = 0; i < n; i++) REQUIRE(src[i] && dst[i], MCBA_ERR_ARG, "null image " + std::to_string(i));
-  mcba_ctx::UndistortMap* m = nullptr;
-  { int r = resident_map(ctx, model, camera, width, height, nullptr, &m); if (r) return r; }
+// cv2.remap(src[i], map, None, INTER_CUBIC) for n images through the resident map m of (width, height), host to host.  Chunks of images
+// go through pinned staging on UND_STREAMS streams in turn: while the host copies one chunk into its staging buffer, earlier chunks are
+// in flight (copy in, k_remap_cubic, copy out) on the other streams.
+int remap_images(mcba_ctx* ctx, const mcba_ctx::UndistortMap* m, int32_t width, int32_t height, int32_t n, int32_t src_width,
+                 int32_t src_height, int32_t channels, const uint8_t* const* src, uint8_t* const* dst) {
   auto& U = ctx->und;
   const size_t in_bytes = (size_t)src_width * src_height * channels, out_bytes = (size_t)width * height * channels;
   const size_t chunk_bytes = (size_t)8 << 20;
@@ -1665,6 +1672,113 @@ int mcba_undistort_images(mcba_ctx* ctx, int32_t model, const double* camera, in
   }
   for (int k = 0; k < n_slots; k++) { int r = drain((n_chunks + k) % n_slots); if (r) return r; }
   return MCBA_OK;
+}
+
+// the checks every image entry makes before its map is looked up
+int check_images(mcba_ctx* ctx, int32_t width, int32_t height, int32_t n, int32_t src_width, int32_t src_height, int32_t channels,
+                 int32_t dtype, const uint8_t* const* src, uint8_t* const* dst) {
+  REQUIRE(dtype == MCBA_IMAGE_UINT8, MCBA_ERR_ARG, "unsupported image dtype: only 8-bit unsigned images are remapped");
+  REQUIRE(channels == 1 || channels == 3, MCBA_ERR_ARG, "unsupported channel count: 1 or 3 channels are remapped");
+  REQUIRE(width > 0 && height > 0 && height <= 65535, MCBA_ERR_ARG, "map size out of range");
+  REQUIRE(src_width > 0 && src_height > 0, MCBA_ERR_ARG, "empty source image");
+  REQUIRE(n >= 0, MCBA_ERR_ARG, "negative image count");
+  if (n == 0) return MCBA_OK;
+  REQUIRE(src && dst, MCBA_ERR_ARG, "null image list");
+  for (int i = 0; i < n; i++) REQUIRE(src[i] && dst[i], MCBA_ERR_ARG, "null image " + std::to_string(i));
+  return MCBA_OK;
+}
+
+// point entries: copy in, one thread per point, copy out.  R and P (both or neither) make it the rectification of the points.
+int run_points(mcba_ctx* ctx, bool project, int32_t model, const double* camera, int64_t n, const double* in, double* out,
+               const double* R = nullptr, const double* P = nullptr) {
+  if (!ctx) return MCBA_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  { int r = check_camera(ctx, model, camera); if (r) return r; }
+  const bool rectify = R || P;
+  RectifyCamera rc;
+  if (rectify) { int r = make_rectify_camera(ctx, model, camera, R, P, 0, 0, rc); if (r) return r; }
+  REQUIRE(n >= 0, MCBA_ERR_ARG, "negative point count");
+  if (n == 0) return MCBA_OK;
+  REQUIRE(in && out, MCBA_ERR_ARG, "null argument");
+  auto& U = ctx->und;
+  cudaStream_t s = ctx->stream;
+  const size_t din = project ? 3 : 2;
+  CK(U.pin.alloc(din * n)); CK(U.pout.alloc(2 * (size_t)n));
+  CK(cudaMemcpyAsync(U.pin.p, in, sizeof(double) * din * n, cudaMemcpyHostToDevice, s));
+  const UndistortCamera c = make_camera(model, camera, 0, 0);
+  const unsigned blocks = (unsigned)((n + UND_THREADS - 1) / UND_THREADS);
+  with_model(model, false, [&](auto M, auto) {
+    constexpr int MODEL = decltype(M)::value;
+    if (project) k_project_points<MODEL><<<blocks, UND_THREADS, 0, s>>>(c, n, U.pin.p, U.pout.p);
+    else if (rectify) k_rectify_points<MODEL><<<blocks, UND_THREADS, 0, s>>>(rc, n, U.pin.p, U.pout.p);
+    else k_undistort_points<MODEL><<<blocks, UND_THREADS, 0, s>>>(c, n, U.pin.p, U.pout.p);
+  });
+  CKL();
+  CK(cudaMemcpyAsync(out, U.pout.p, sizeof(double) * 2 * n, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  return MCBA_OK;
+}
+
+}  // namespace
+
+// initUndistortRectifyMap(K, dist, None, K, (width, height)) of one camera, kept resident for mcba_undistort_images
+int mcba_undistort_map(mcba_ctx* ctx, int32_t model, const double* camera, int32_t width, int32_t height, float* map) {
+  if (!ctx) return MCBA_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  { int r = check_camera(ctx, model, camera); if (r) return r; }
+  REQUIRE(width > 0 && height > 0 && height <= 65535, MCBA_ERR_ARG, "map size out of range");
+  mcba_ctx::UndistortMap* m = nullptr;
+  int r = undistortion_map(ctx, model, camera, width, height, map, &m);
+  if (r) return r;
+  CK(cudaStreamSynchronize(ctx->stream));
+  return MCBA_OK;
+}
+
+// cv2.remap(src[i], map, None, INTER_CUBIC) for n images of one camera through its undistortion map, host to host (remap_images)
+int mcba_undistort_images(mcba_ctx* ctx, int32_t model, const double* camera, int32_t width, int32_t height, int32_t n,
+                          int32_t src_width, int32_t src_height, int32_t channels, int32_t dtype, const uint8_t* const* src,
+                          uint8_t* const* dst) {
+  if (!ctx) return MCBA_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  { int r = check_camera(ctx, model, camera); if (r) return r; }
+  { int r = check_images(ctx, width, height, n, src_width, src_height, channels, dtype, src, dst); if (r || n == 0) return r; }
+  mcba_ctx::UndistortMap* m = nullptr;
+  { int r = undistortion_map(ctx, model, camera, width, height, nullptr, &m); if (r) return r; }
+  return remap_images(ctx, m, width, height, n, src_width, src_height, channels, src, dst);
+}
+
+// initUndistortRectifyMap(K, dist, R, P, (width, height)) of one camera, kept resident for mcba_rectify_images
+int mcba_rectify_map(mcba_ctx* ctx, int32_t model, const double* camera, const double* R, const double* P, int32_t width, int32_t height,
+                     float* map) {
+  if (!ctx) return MCBA_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  { int r = check_camera(ctx, model, camera); if (r) return r; }
+  REQUIRE(width > 0 && height > 0 && height <= 65535, MCBA_ERR_ARG, "map size out of range");
+  mcba_ctx::UndistortMap* m = nullptr;
+  int r = rectification_map(ctx, model, camera, R, P, width, height, map, &m);
+  if (r) return r;
+  CK(cudaStreamSynchronize(ctx->stream));
+  return MCBA_OK;
+}
+
+// cv2.remap(src[i], map, None, INTER_CUBIC) for n images of one camera through its rectification map, host to host (remap_images)
+int mcba_rectify_images(mcba_ctx* ctx, int32_t model, const double* camera, const double* R, const double* P, int32_t width,
+                        int32_t height, int32_t n, int32_t src_width, int32_t src_height, int32_t channels, int32_t dtype,
+                        const uint8_t* const* src, uint8_t* const* dst) {
+  if (!ctx) return MCBA_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  { int r = check_camera(ctx, model, camera); if (r) return r; }
+  { int r = check_images(ctx, width, height, n, src_width, src_height, channels, dtype, src, dst); if (r || n == 0) return r; }
+  mcba_ctx::UndistortMap* m = nullptr;
+  { int r = rectification_map(ctx, model, camera, R, P, width, height, nullptr, &m); if (r) return r; }
+  return remap_images(ctx, m, width, height, n, src_width, src_height, channels, src, dst);
+}
+
+int mcba_rectify_points(mcba_ctx* ctx, int32_t model, const double* camera, const double* R, const double* P, int64_t n,
+                        const double* pixels, double* rectified) {
+  if (!ctx) return MCBA_ERR_ARG;
+  REQUIRE(R && P, MCBA_ERR_ARG, "null R or P");
+  return run_points(ctx, false, model, camera, n, pixels, rectified, R, P);
 }
 
 int mcba_project_points(mcba_ctx* ctx, int32_t model, const double* camera, int64_t n, const double* points, double* pixels) {

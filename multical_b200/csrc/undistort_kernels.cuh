@@ -112,13 +112,23 @@ struct UndistortCamera {
   int w, h;
 };
 
+template <int MODEL>
+__host__ __device__ inline void distorted_pixel(const UndistortCamera& c, double x, double y, float& mx, float& my);
+
 // initUndistortRectifyMap (R = I, newK = K) at pixel (u, v) -> float32 (mx, my)
 template <int MODEL>
 __host__ __device__ inline void undistort_map_pixel(const UndistortCamera& c, int u, int v, float& mx, float& my) {
   const double fx = c.k[0], fy = c.k[1], cx = c.k[2], cy = c.k[3], s = c.k[4];
-  const double* d = c.k + 5;
   const double y = dadd((double)v, -cy) / fy;
   const double x = dadd(dadd((double)u, -cx), -dmul(s, y)) / fx;
+  distorted_pixel<MODEL>(c, x, y, mx, my);
+}
+
+// the map entry of the normalised point (x, y): OpenCV's distortion and projection (fx, fy, cx, cy; K[0][1] unused), cast to float32
+template <int MODEL>
+__host__ __device__ inline void distorted_pixel(const UndistortCamera& c, double x, double y, float& mx, float& my) {
+  const double fx = c.k[0], fy = c.k[1], cx = c.k[2], cy = c.k[3];
+  const double* d = c.k + 5;
   double mu, mv;
   if constexpr (MODEL == MODEL_FISHEYE) {
     // cv2.fisheye.initUndistortRectifyMap: theta_d = theta (1 + k1 theta^2 + k2 theta^4 + k3 theta^6 + k4 theta^8), scale = theta_d / r
@@ -245,6 +255,91 @@ __global__ void __launch_bounds__(UND_THREADS) k_undistort_points(UndistortCamer
   double u, v;
   undistort_pixel<MODEL>(c.k, in[2 * i], in[2 * i + 1], u, v);
   out[2 * i] = u; out[2 * i + 1] = v;
+}
+
+// ---- rectification: initUndistortRectifyMap(K, dist, R, P) and undistortPoints(pts, K, dist, R, P) --------------------------------------
+// ir = (P[:, :3] R)^-1 and rr = P[:, :3] R, both row-major fp64 from the host (its 3x3 Gaussian elimination); cam.w, cam.h are the map size.
+//
+// Map (k_rectify_map): OpenCV walks each row i from (x, y, w) = i * ir[1, 4, 7] + ir[2, 5, 8] in steps of ir[0, 3, 6], and the
+// walk's rounding reaches the float32 map.  Pinhole (undistort.simd.hpp, 2 vectors of 4 doubles): blocks of RECT_BLOCK = 8 pixels
+// start at `cur`, pixel k of a block is cur + k * step, then cur += 8 * step while a whole block is left; the last W mod 8 pixels take
+// cur, then cur += step, one at a time.  x = _x * (1 / _w).  Fisheye (fisheye.cpp): one pixel at a time, cur += step, x = _x / _w, and
+// _w <= 0 gives an infinite map entry.  Three threads of the row's CTA write the walk's values (block starts, then the tail) into shared
+// memory, the CTA synchronises, and every thread finishes its pixels with distorted_pixel<MODEL>.
+constexpr int RECT_BLOCK = 8;
+constexpr int RECT_SMEM_MAX = 200 * 1024;          // the walk of one row: fisheye maps up to 8533 pixels wide
+
+struct RectifyCamera {
+  UndistortCamera cam;
+  double ir[9], rr[9];
+};
+
+// entries of the walk one row keeps in shared memory: block starts and tail pixels (pinhole), every pixel (fisheye)
+__host__ __device__ __forceinline__ int rectify_walk_len(int model, int w) {
+  return model == MODEL_FISHEYE ? w : w / RECT_BLOCK + w % RECT_BLOCK;
+}
+
+// one CTA of UND_THREADS per map row; dynamic shared memory 3 * rectify_walk_len doubles.  fmap (float2 [h][w]) may be null.
+template <int MODEL>
+__global__ void __launch_bounds__(UND_THREADS) k_rectify_map(RectifyCamera c, float2* fmap, uint32_t* org, uint16_t* idx) {
+  extern __shared__ double walk[];
+  const int w = c.cam.w, i = blockIdx.x, n = rectify_walk_len(MODEL, w);
+  constexpr int B = MODEL == MODEL_FISHEYE ? 1 : RECT_BLOCK;
+  const int nb = w / B;                                  // whole blocks
+  if (threadIdx.x < 3) {
+    const int r = threadIdx.x;                           // 0: x, 1: y, 2: w
+    const double step = c.ir[3 * r], bstep = dmul((double)B, step);
+    double cur = dadd(dmul((double)i, c.ir[3 * r + 1]), c.ir[3 * r + 2]);
+    double* out = walk + r * n;
+    for (int b = 0; b < nb; b++) { out[b] = cur; cur = dadd(cur, bstep); }
+    for (int t = nb; t < n; t++) { out[t] = cur; cur = dadd(cur, step); }
+  }
+  __syncthreads();
+  for (int j = threadIdx.x; j < w; j += blockDim.x) {
+    double v[3];
+    const int b = j / B, k = j - b * B;
+#pragma unroll
+    for (int r = 0; r < 3; r++) {
+      const double* in = walk + r * n;
+      if (MODEL == MODEL_FISHEYE) v[r] = in[j];
+      else v[r] = b < nb ? dadd(in[b], dmul((double)k, c.ir[3 * r])) : in[nb + (j - nb * B)];
+    }
+    float mx, my;
+    if constexpr (MODEL == MODEL_FISHEYE) {
+      if (v[2] <= 0.0) {
+        mx = v[0] > 0.0 ? -INFINITY : INFINITY;
+        my = v[1] > 0.0 ? -INFINITY : INFINITY;
+      } else {
+        distorted_pixel<MODEL>(c.cam, v[0] / v[2], v[1] / v[2], mx, my);
+      }
+    } else {
+      const double iw = 1.0 / v[2];
+      distorted_pixel<MODEL>(c.cam, dmul(v[0], iw), dmul(v[1], iw), mx, my);
+    }
+    const size_t p = (size_t)i * w + j;
+    if (fmap) { float2 f; f.x = mx; f.y = my; fmap[p] = f; }
+    fixed_point_entry(mx, my, org[p], idx[p]);
+  }
+}
+
+// cv2.undistortPoints(pts, K, dist, R = R, P = P) / cv2.fisheye.undistortPoints(pts, K, dist, R, P), one thread each: the normalised
+// undistorted point is undistort_pixel<MODEL> under K = I after the division by the focal lengths (both exact in IEEE arithmetic), then
+// OpenCV's (xx, yy, ww) = rr (x, y, 1), pixel (xx, yy) / ww.  A fisheye point whose Newton iteration fails keeps the -1e6 sentinel.
+template <int MODEL>
+__global__ void __launch_bounds__(UND_THREADS) k_rectify_points(RectifyCamera c, int64_t n, const double* in, double* out) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  double kn[5 + 14];
+  kn[0] = 1.0; kn[1] = 1.0; kn[2] = 0.0; kn[3] = 0.0; kn[4] = 0.0;
+  for (int d = 0; d < model_nd(MODEL); d++) kn[5 + d] = c.cam.k[5 + d];
+  const double* k = c.cam.k;
+  double x, y;
+  undistort_pixel<MODEL>(kn, (in[2 * i] - k[2]) / k[0], (in[2 * i + 1] - k[3]) / k[1], x, y);
+  if (MODEL == MODEL_FISHEYE && x == -1000000.0 && y == -1000000.0) { out[2 * i] = x; out[2 * i + 1] = y; return; }
+  const double* R = c.rr;
+  const double xx = R[0] * x + R[1] * y + R[2], yy = R[3] * x + R[4] * y + R[5], ww = R[6] * x + R[7] * y + R[8];
+  if (MODEL == MODEL_FISHEYE) { out[2 * i] = xx / ww; out[2 * i + 1] = yy / ww; }
+  else { const double iw = 1.0 / ww; out[2 * i] = xx * iw; out[2 * i + 1] = yy * iw; }
 }
 
 }  // namespace mcba

@@ -331,6 +331,50 @@ class Engine:
     self._ck(self.lib.mcba_undistort_points(self.h, mid, nat.dptr(cam), len(pts), nat.dptr(pts), nat.dptr(out)))
     return out[:len(pts)]
 
+  @staticmethod
+  def _rect(R, P):
+    R, P = nat.f64(R).reshape(3, 3), nat.f64(P).reshape(3, -1)
+    return nat.f64(R).reshape(-1), nat.f64(P[:, :3]).reshape(-1)
+
+  def rectify_map(self, model, camera, R, P, size, want_map=True):
+    """initUndistortRectifyMap(K, dist, R, P, size) of camera [fx fy cx cy skew dist...] (P 3x3 or 3x4): the map stays resident on the
+    device; returns it as float32 [h, w, 2] (None with want_map=False)."""
+    mid, cam = self._camera(model, camera)
+    R, P = self._rect(R, P)
+    w, h = (int(v) for v in size)
+    out = np.empty((h, w, 2), np.float32) if want_map else None
+    self._ck(self.lib.mcba_rectify_map(self.h, mid, nat.dptr(cam), nat.dptr(R), nat.dptr(P), w, h,
+                                       None if out is None else out.ctypes.data_as(C.POINTER(C.c_float))))
+    return out
+
+  def rectify_images(self, model, camera, R, P, size, images):
+    """undistort_images through the camera's resident rectification map of (R, P, size = (w, h))."""
+    mid, cam = self._camera(model, camera)
+    R, P = self._rect(R, P)
+    w, h = (int(v) for v in size)
+    if len(images) == 0: return []
+    src = [np.ascontiguousarray(im) for im in images]
+    shape, dtype = src[0].shape, src[0].dtype
+    assert all(im.shape == shape and im.dtype == dtype for im in src), "images of one camera must share one shape and dtype"
+    channels = 1 if len(shape) == 2 else shape[2]
+    dt = nat.IMAGE_UINT8 if dtype == np.uint8 else -1
+    out_shape = (h, w) if len(shape) == 2 or channels == 1 else (h, w, channels)
+    dst = [np.empty(out_shape, np.uint8) for _ in src]
+    U8 = C.POINTER(C.c_uint8)
+    sp, dp = (U8 * len(src))(*[im.ctypes.data_as(U8) for im in src]), (U8 * len(dst))(*[im.ctypes.data_as(U8) for im in dst])
+    self._ck(self.lib.mcba_rectify_images(self.h, mid, nat.dptr(cam), nat.dptr(R), nat.dptr(P), w, h, len(src), shape[1], shape[0],
+                                          channels, dt, sp, dp))
+    return dst
+
+  def rectify_points(self, model, camera, R, P, pixels):
+    """cv2.undistortPoints(pixels, K, dist, R=R, P=P) (fisheye: cv2.fisheye.undistortPoints): f64 [n, 2] -> f64 [n, 2]."""
+    mid, cam = self._camera(model, camera)
+    R, P = self._rect(R, P)
+    pts = nat.f64(pixels).reshape(-1, 2)
+    out = np.zeros((max(len(pts), 1), 2))
+    self._ck(self.lib.mcba_rectify_points(self.h, mid, nat.dptr(cam), nat.dptr(R), nat.dptr(P), len(pts), nat.dptr(pts), nat.dptr(out)))
+    return out[:len(pts)]
+
   def remap_cubic_table(self):
     """The fixed-point bicubic weights of the remap, int32 [1024, 16] (include/mcba.h mcba_remap_cubic_table)."""
     tab = np.zeros((1024, 16), np.int32)
