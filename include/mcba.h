@@ -356,6 +356,25 @@ int  mcba_rectify_images(mcba_ctx* ctx, int32_t model, const double* camera, con
 int  mcba_rectify_points(mcba_ctx* ctx, int32_t model, const double* camera, const double* R, const double* P, int64_t n,
                          const double* pixels, double* rectified);
 
+/* -- triangulating points of a calibrated rig (DESIGN.md §3j) -----------------------------------------------------------------------
+ * mcba_triangulate: N points seen by C cameras of one model (1 <= C <= MCBA_TRI_MAX_CAMERAS).  cameras f64[C][5 + nd] as above;
+ *   poses f64[C][16] rig -> camera (x_cam = T_c x_rig, row-major 4x4, last row ignored); pixels f64[C][N][2]; valid uint8[C][N]
+ *   (non-zero: camera c sees point n).  Out: points f64[N][3] in the rig frame, ok uint8[N], rms f64[N] (pixels, over the point's valid
+ *   views).  Each point: the linear (DLT) solution from the undistorted normalised views, refined by Levenberg-Marquardt on the
+ *   reprojection error through the full camera model.  A point is invalid (ok = 0, point and rms NaN) with fewer than 2 valid views,
+ *   a non-finite valid pixel, a DLT w that is non-finite or zero at working precision, a valid view with z_cam <= 0 at the end, or a
+ *   non-finite result.
+ * mcba_triangulate_linear: cv2.triangulatePoints(P1, P2, x1, x2): P1, P2 f64[12] (3x4 row-major), x1, x2 f64[2][N] (row 0 x, row 1 y),
+ *   out f64[4][N], the homogeneous points of unit norm (the sign is unspecified, as OpenCV's).  No distortion and no refinement.
+ * Both work on chunks of points, so the device memory of a call stays within MCBA_TRI_CHUNK_BYTES plus the cameras.  Identical calls
+ * agree bit for bit.  Bad arguments fail with MCBA_ERR_ARG; non-finite camera parameters, poses or P with MCBA_ERR_NONFINITE.  Neither
+ * touches the uploaded problem. */
+enum { MCBA_TRI_MAX_CAMERAS = 256, MCBA_TRI_CHUNK_BYTES = 64 << 20 };
+int  mcba_triangulate(mcba_ctx* ctx, int32_t model, int32_t C, const double* cameras, const double* poses, int64_t N,
+                      const double* pixels, const uint8_t* valid, double* points, uint8_t* ok, double* rms);
+int  mcba_triangulate_linear(mcba_ctx* ctx, const double* P1, const double* P2, int64_t N, const double* x1, const double* x2,
+                             double* out);
+
 /* -- measurement hooks (bench.py): launch one kernel family on the context stream -------------- */
 enum { MCBA_BENCH_LINEARIZE = 0, MCBA_BENCH_RESIDUAL = 1, MCBA_BENCH_COST = 2,
        MCBA_BENCH_NO_PREPARE = 256 /* or-ed in: reuse the pose tables of the previous call (times the kernel alone) */ };

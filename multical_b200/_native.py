@@ -32,7 +32,7 @@ EXPORTS = ["mcba_create", "mcba_destroy", "mcba_last_error", "mcba_set_stream", 
            "mcba_intrinsic_init", "mcba_view_errors", "mcba_pose_pairs", "mcba_pose_times", "mcba_pose_cluster",
            "mcba_hand_eye_quads", "mcba_hand_eye_vote", "mcba_undistort_map", "mcba_undistort_images", "mcba_project_points",
            "mcba_undistort_points", "mcba_remap_cubic_table", "mcba_stereo_init", "mcba_rectify_map", "mcba_rectify_images",
-           "mcba_rectify_points"]
+           "mcba_rectify_points", "mcba_triangulate", "mcba_triangulate_linear"]
 IMAGE_UINT8 = 0          # include/mcba.h MCBA_IMAGE_UINT8
 TABLE_VALID, TABLE_INLIERS = 0, 1
 
@@ -143,6 +143,8 @@ def load():
   lib.mcba_rectify_map.argtypes = [P, i32, D, D, D, i32, i32, C.POINTER(C.c_float)]
   lib.mcba_rectify_images.argtypes = [P, i32, D, D, D, i32, i32, i32, i32, i32, i32, i32, U8P, U8P]
   lib.mcba_rectify_points.argtypes = [P, i32, D, D, D, C.c_int64, D, D]
+  lib.mcba_triangulate.argtypes = [P, i32, i32, D, D, C.c_int64, D, U8, D, U8, D]
+  lib.mcba_triangulate_linear.argtypes = [P, D, D, C.c_int64, D, D, D]
   _lib = lib
   return lib
 

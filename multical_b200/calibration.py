@@ -251,6 +251,21 @@ class Calibration(Parameters):
   def reprojection_inliers(self):
     return self._valid_errors[self.inliers[self.valid]]
 
+  def triangulate(self):
+    """The calibration's inlier detections triangulated through its cameras and camera poses (multical_b200/triangulate.py): a Table of
+    points [F, B, P, 3] in each frame's rig coordinates (where the projection reads camera_pose @ rig point, the rig point being
+    frame_pose @ board_pose @ X), valid [F, B, P] (at least two inlier views) and rms [F, B, P] in pixels.  Independent of the solved
+    frame and board poses, so it checks a calibration against them.  RollingFrames raise NotImplementedError: each image row sees the
+    rig at another time, so a detection has no single rig point."""
+    if motion_kind(self.motion) == MOTION_ROLLING:
+      raise NotImplementedError("triangulation of RollingFrames: each image row sees the rig at a different time, so there is no single "
+                                "rig point to triangulate")
+    from .triangulate import triangulate
+    C, F, B, P = self.size.cameras, self.size.rig_poses, self.size.boards, self.size.points
+    pixels = np.asarray(self.point_table.points, np.float64).reshape(C, F * B * P, 2)
+    res = triangulate(list(self.cameras), np.asarray(self.camera_poses.poses), pixels, np.asarray(self.inliers).reshape(C, F * B * P))
+    return Table.create(points=res.points.reshape(F, B, P, 3), valid=res.valid.reshape(F, B, P), rms=res.rms.reshape(F, B, P))
+
   # ---- parameters (calibration.py:144-171) ------------------------------------------------------
   @cached_property
   def param_objects(self):

@@ -27,6 +27,7 @@
 #include "hand_eye_init_kernels.cuh"
 #include "undistort_kernels.cuh"
 #include "stereo_kernels.cuh"
+#include "triangulate_kernels.cuh"
 
 using namespace mcba;
 
@@ -95,6 +96,18 @@ void with_model(int model, bool roll, Fn&& f) {
     case MODEL_THIN_PRISM: pick(std::integral_constant<int, MODEL_THIN_PRISM>{}); break;
     case MODEL_TILTED: pick(std::integral_constant<int, MODEL_TILTED>{}); break;
     default: pick(std::integral_constant<int, MODEL_FISHEYE>{}); break;
+  }
+}
+
+// calls f(integral_constant<int, LANES>) for the lanes of a triangulation group
+template <typename Fn>
+void with_lanes(int lanes, Fn&& f) {
+  switch (lanes) {
+    case 2: f(std::integral_constant<int, 2>{}); break;
+    case 4: f(std::integral_constant<int, 4>{}); break;
+    case 8: f(std::integral_constant<int, 8>{}); break;
+    case 16: f(std::integral_constant<int, 16>{}); break;
+    default: f(std::integral_constant<int, 32>{}); break;
   }
 }
 
@@ -188,6 +201,10 @@ struct mcba_ctx {
     uint8_t* host_in[UND_STREAMS] = {}; uint8_t* host_out[UND_STREAMS] = {}; size_t host_in_cap = 0, host_out_cap = 0;
     DevBuf<uint8_t> dev_in[UND_STREAMS], dev_out[UND_STREAMS];
   } und;
+  // triangulation (mcba_triangulate / mcba_triangulate_linear): the cameras, one chunk's inputs and outputs
+  struct TriangulateBuffers {
+    DevBuf<double> cams, poses, points, rms, lin; DevBuf<double2> px; DevBuf<uint8_t> valid, ok;
+  } tri;
 };
 
 #define CK(call)                                                                                   \
@@ -713,6 +730,8 @@ int mcba_create(int device, mcba_ctx** out) {
   for (int model = MODEL_STANDARD; model <= MODEL_TILTED; model++)
     with_model(model, false, [](auto M, auto) {
       cudaFuncSetAttribute(k_rectify_map<decltype(M)::value>, cudaFuncAttributeMaxDynamicSharedMemorySize, RECT_SMEM_MAX);
+      cudaFuncSetAttribute(k_triangulate<decltype(M)::value, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           (int)tri_smem((MCBA_TRI_MAX_CAMERAS + 31) / 32));
     });
   *out = ctx;
   return MCBA_OK;
@@ -1797,6 +1816,95 @@ int mcba_remap_cubic_table(mcba_ctx* ctx, int32_t* table) {
   { int r = ensure_cubic_table(ctx); if (r) return r; }
   CK(cudaMemcpyAsync(table, U.tab.p, sizeof(int32_t) * 16 * UND_TAB_ENTRIES, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
+  return MCBA_OK;
+}
+
+namespace {
+
+// points of one chunk: the chunk's device memory, at `bytes` per point, within MCBA_TRI_CHUNK_BYTES
+int64_t tri_chunk(int64_t N, size_t bytes) { return std::max<int64_t>(1, std::min<int64_t>(N, (int64_t)(MCBA_TRI_CHUNK_BYTES / bytes))); }
+
+}  // namespace
+
+// N-view triangulation (k_triangulate), chunk by chunk: per chunk the pixels and masks of every camera go in (one copy per camera), one
+// launch, the points, flags and rms come out
+int mcba_triangulate(mcba_ctx* ctx, int32_t model, int32_t C, const double* cameras, const double* poses, int64_t N,
+                     const double* pixels, const uint8_t* valid, double* points, uint8_t* ok, double* rms) {
+  if (!ctx) return MCBA_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  REQUIRE(model >= MODEL_STANDARD && model <= MODEL_TILTED, MCBA_ERR_ARG, "unknown camera model");
+  REQUIRE(C >= 1 && C <= MCBA_TRI_MAX_CAMERAS, MCBA_ERR_ARG, "camera count out of range (1 .. " + std::to_string(MCBA_TRI_MAX_CAMERAS) + ")");
+  REQUIRE(N >= 0, MCBA_ERR_ARG, "negative point count");
+  REQUIRE(cameras && poses, MCBA_ERR_ARG, "null cameras or poses");
+  const int kd = 5 + model_nd(model);
+  for (int c = 0; c < C; c++) {
+    int r = check_camera(ctx, model, cameras + (size_t)kd * c);
+    if (r) { ctx->err = "camera " + std::to_string(c) + ": " + ctx->err; return r; }
+  }
+  REQUIRE(all_finite(poses, 16 * (size_t)C), MCBA_ERR_NONFINITE, "non-finite camera pose");
+  if (N == 0) return MCBA_OK;
+  REQUIRE(pixels && valid && points && ok && rms, MCBA_ERR_ARG, "null argument");
+  auto& T = ctx->tri;
+  cudaStream_t s = ctx->stream;
+  std::vector<double> cams((size_t)TRI_KD * C, 0.0);
+  for (int c = 0; c < C; c++) std::copy(cameras + (size_t)kd * c, cameras + (size_t)kd * (c + 1), cams.begin() + (size_t)TRI_KD * c);
+  const int lanes = tri_lanes(C), nk = (C + lanes - 1) / lanes;
+  const int64_t chunk = tri_chunk(N, (size_t)C * (sizeof(double2) + 1) + 4 * sizeof(double) + 1);
+  CK(T.cams.alloc(cams.size())); CK(T.poses.alloc(16 * (size_t)C));
+  CK(T.px.alloc((size_t)C * chunk)); CK(T.valid.alloc((size_t)C * chunk));
+  CK(T.points.alloc(3 * (size_t)chunk)); CK(T.rms.alloc(chunk)); CK(T.ok.alloc(chunk));
+  CK(cudaMemcpyAsync(T.cams.p, cams.data(), sizeof(double) * cams.size(), cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(T.poses.p, poses, sizeof(double) * 16 * C, cudaMemcpyHostToDevice, s));
+  for (int64_t p0 = 0; p0 < N; p0 += chunk) {
+    const int64_t n = std::min(chunk, N - p0);
+    for (int c = 0; c < C; c++) {
+      CK(cudaMemcpyAsync(T.px.p + (size_t)c * n, pixels + 2 * ((size_t)c * N + p0), sizeof(double2) * n, cudaMemcpyHostToDevice, s));
+      CK(cudaMemcpyAsync(T.valid.p + (size_t)c * n, valid + (size_t)c * N + p0, n, cudaMemcpyHostToDevice, s));
+    }
+    TriArgs a{C, nk, n, T.cams.p, T.poses.p, T.px.p, T.valid.p, T.points.p, T.ok.p, T.rms.p};
+    const unsigned blocks = (unsigned)((n * lanes + TRI_THREADS - 1) / TRI_THREADS);
+    with_model(model, false, [&](auto M, auto) {
+      with_lanes(lanes, [&](auto L) {
+        k_triangulate<decltype(M)::value, decltype(L)::value><<<blocks, TRI_THREADS, tri_smem(nk), s>>>(a);
+      });
+    });
+    CKL();
+    CK(cudaMemcpyAsync(points + 3 * p0, T.points.p, sizeof(double) * 3 * n, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(ok + p0, T.ok.p, n, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(rms + p0, T.rms.p, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
+  }
+  CK(cudaStreamSynchronize(s));
+  return MCBA_OK;
+}
+
+// cv2.triangulatePoints (k_triangulate_linear), chunk by chunk
+int mcba_triangulate_linear(mcba_ctx* ctx, const double* P1, const double* P2, int64_t N, const double* x1, const double* x2, double* out) {
+  if (!ctx) return MCBA_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  REQUIRE(P1 && P2, MCBA_ERR_ARG, "null projection matrix");
+  REQUIRE(all_finite(P1, 12) && all_finite(P2, 12), MCBA_ERR_NONFINITE, "non-finite projection matrix");
+  REQUIRE(N >= 0, MCBA_ERR_ARG, "negative point count");
+  if (N == 0) return MCBA_OK;
+  REQUIRE(x1 && x2 && out, MCBA_ERR_ARG, "null argument");
+  auto& T = ctx->tri;
+  cudaStream_t s = ctx->stream;
+  const int64_t chunk = tri_chunk(N, 8 * sizeof(double));
+  CK(T.lin.alloc(8 * (size_t)chunk));
+  TriLinearArgs a{};
+  for (int j = 0; j < 12; j++) { a.P[0][j] = P1[j]; a.P[1][j] = P2[j]; }
+  for (int64_t p0 = 0; p0 < N; p0 += chunk) {
+    const int64_t n = std::min(chunk, N - p0);
+    double* dx = T.lin.p;                            // [x1 x; x1 y; x2 x; x2 y] of the chunk, then [4][n] out
+    for (int r = 0; r < 2; r++) {
+      CK(cudaMemcpyAsync(dx + r * n, x1 + r * N + p0, sizeof(double) * n, cudaMemcpyHostToDevice, s));
+      CK(cudaMemcpyAsync(dx + (2 + r) * n, x2 + r * N + p0, sizeof(double) * n, cudaMemcpyHostToDevice, s));
+    }
+    a.n = n; a.x[0] = dx; a.x[1] = dx + 2 * n; a.out = dx + 4 * n;
+    k_triangulate_linear<<<(unsigned)((2 * n + TRI_THREADS - 1) / TRI_THREADS), TRI_THREADS, tri_smem(1), s>>>(a);
+    CKL();
+    for (int j = 0; j < 4; j++) CK(cudaMemcpyAsync(out + j * N + p0, a.out + j * n, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
+  }
+  CK(cudaStreamSynchronize(s));
   return MCBA_OK;
 }
 

@@ -375,6 +375,31 @@ class Engine:
     self._ck(self.lib.mcba_rectify_points(self.h, mid, nat.dptr(cam), nat.dptr(R), nat.dptr(P), len(pts), nat.dptr(pts), nat.dptr(out)))
     return out[:len(pts)]
 
+  def triangulate(self, model, cameras, poses, pixels, valid):
+    """mcba_triangulate: cameras [C, 5 + nd] of one model, poses [C, 4, 4] rig -> camera, pixels [C, N, 2], valid [C, N] ->
+    (points f64 [N, 3] in the rig frame, valid bool [N], rms f64 [N]); invalid points hold NaN."""
+    mid = nat.MODEL_IDS[model]
+    cams = nat.f64(cameras).reshape(len(cameras), -1)
+    assert cams.shape[1] == 5 + nat.DIST_SIZES[model], f"camera model {model} takes {5 + nat.DIST_SIZES[model]} parameters"
+    T = nat.f64(poses).reshape(len(cams), 16)
+    px = nat.f64(pixels).reshape(len(cams), -1, 2)
+    ok_in = np.ascontiguousarray(valid, dtype=np.uint8).reshape(len(cams), -1)
+    N = px.shape[1]
+    points, ok, rms = np.empty((max(N, 1), 3)), np.zeros(max(N, 1), np.uint8), np.empty(max(N, 1))
+    U8 = C.POINTER(C.c_uint8)
+    self._ck(self.lib.mcba_triangulate(self.h, mid, len(cams), nat.dptr(cams), nat.dptr(T), N, nat.dptr(px), ok_in.ctypes.data_as(U8),
+                                       nat.dptr(points), ok.ctypes.data_as(U8), nat.dptr(rms)))
+    return points[:N], ok[:N].astype(bool), rms[:N]
+
+  def triangulate_linear(self, P1, P2, x1, x2):
+    """mcba_triangulate_linear (cv2.triangulatePoints): P1, P2 [3, 4], x1, x2 [2, N] -> f64 [4, N] of unit-norm columns."""
+    P1, P2 = nat.f64(P1).reshape(12), nat.f64(P2).reshape(12)
+    x1, x2 = nat.f64(x1).reshape(2, -1), nat.f64(x2).reshape(2, -1)
+    N = x1.shape[1]
+    out = np.empty((4, max(N, 1)))
+    self._ck(self.lib.mcba_triangulate_linear(self.h, nat.dptr(P1), nat.dptr(P2), N, nat.dptr(x1), nat.dptr(x2), nat.dptr(out)))
+    return out[:, :N]
+
   def remap_cubic_table(self):
     """The fixed-point bicubic weights of the remap, int32 [1024, 16] (include/mcba.h mcba_remap_cubic_table)."""
     tab = np.zeros((1024, 16), np.int32)
