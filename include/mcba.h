@@ -105,30 +105,22 @@ int  mcba_peer_export(mcba_ctx* ctx, int64_t cap_doubles, char out_handle[64]);
 int  mcba_peer_import(mcba_ctx* ctx, const char* handles /* world x 64 bytes in rank order */);
 
 /* -- problem upload: replaces what `evaluate` closes over (calibration.py:204-206) --------------
- * cam/frame/board/point: int32[N] rows of np.argwhere(inliers) (frame ids local to this rank);
- * obs: f64[N][2] = point_table.points[inliers] (calibration.py:206);
- * board_points: f64[B][P][3] = tables.stack_boards(boards).points (tables.py:385-394).            */
-int  mcba_upload(mcba_ctx* ctx, const mcba_problem_desc* desc,
-                 const int32_t* cam, const int32_t* frame, const int32_t* board, const int32_t* point,
-                 const double* obs, const double* board_points);
-
-/* Dense variant (the reference's own wire format): mask uint8[C][F][B][P] = calib.inliers (calibration.py:78-81),
- * points f64[C][F][B][P][2] = point_table.points (tables.make_point_table, tables.py:68-81).  Packing into the
- * frame-major corner arrays happens on the device; *n_corners receives the number of selected corners.  The packed
- * order seen through mcba_residuals is still np.argwhere(mask) order.                                              */
-int  mcba_upload_dense(mcba_ctx* ctx, const mcba_problem_desc* desc, const uint8_t* mask, const double* points,
-                       const double* board_points, int64_t* n_corners);
-/* The same with the mask in the two parts the reference builds it from (calibration.py:73-81: `valid` = point_table.valid &
- * pose validity broadcast over the points): valid uint8[C][F][B][P] = point_table.valid as detected, view_valid uint8[C][F][B] =
- * camera_poses.valid x motion.valid x board_poses.valid (may be NULL: all views valid).  The conjunction is taken on the device, so
- * the caller hands over the detection table untouched (no 1-byte-per-point host pass before the copy).                          */
-int  mcba_upload_dense_views(mcba_ctx* ctx, const mcba_problem_desc* desc, const uint8_t* valid, const uint8_t* view_valid,
-                             const double* points, const double* board_points, int64_t* n_corners);
-/* The same for a float32 table, points f32[C][F][B][P][2]: make_point_table keeps the dtype of the detector's corners (tables.py:15-17
- * fill_sparse: `dtype=values.dtype`; cv2's aruco / charuco detectors return float32), so this IS the reference's table for real
- * detections -- half the bytes over the link and no float64 copy of the table on the host.  The packed observations are f64 (exact). */
-int  mcba_upload_dense_views_f32(mcba_ctx* ctx, const mcba_problem_desc* desc, const uint8_t* valid, const uint8_t* view_valid,
-                                 const float* points, const double* board_points, int64_t* n_corners);
+ * The reference's own wire format: valid uint8[C][F][B][P] selects the corners (calib.inliers, calibration.py:78-81, or
+ * point_table.valid as detected), points [C][F][B][P][2] are their pixels (point_table.points, tables.make_point_table,
+ * tables.py:68-81), board_points f64[B][P][3] = tables.stack_boards(boards).points (tables.py:385-394).  view_valid uint8[C][F][B]
+ * (may be NULL: all views valid) is the other part the reference builds the mask from (calibration.py:73-81: camera_poses.valid x
+ * motion.valid x board_poses.valid); the conjunction valid & view_valid is taken on the device, so the caller hands the detection
+ * table over untouched.  point_type MCBA_POINTS_F64 or MCBA_POINTS_F32: make_point_table keeps the dtype of the detector's corners
+ * (tables.py:15-17 fill_sparse: `dtype=values.dtype`; cv2's aruco / charuco detectors return float32), so a float32 table IS the
+ * reference's table for real detections -- half the bytes over the link; the packed observations are f64 (exact).
+ * Packing into the frame-major corner arrays happens on the device; *n_corners receives the number of selected corners.  The packed
+ * order seen through mcba_residuals is np.argwhere(valid & view_valid) order (frame ids local to this rank).
+ * Every upload (also mcba_table_upload / mcba_table_from_detections) replaces the context's problem: a refused one, for its inputs or
+ * later (too many boards for the linearisation kernel: MCBA_ERR_UNSUPPORTED), leaves none, and the entry points that need one fail
+ * with MCBA_ERR_STATE until an upload succeeds. */
+enum { MCBA_POINTS_F64 = 0, MCBA_POINTS_F32 = 1 };
+int  mcba_upload_dense(mcba_ctx* ctx, const mcba_problem_desc* desc, const uint8_t* valid, const uint8_t* view_valid,
+                       const void* points, int32_t point_type, const double* board_points, int64_t* n_corners);
 
 /* full parameter state (also the values of disabled/fixed blocks):
  * cam_rt f64[C][6], board_rt f64[B][6], frame_rt f64[F][6] (PoseSet.params, pose_set.py:51-53),
@@ -185,8 +177,8 @@ int  mcba_solve(mcba_ctx* ctx, const mcba_solve_opts* opts, mcba_solve_result* r
  * mcba_table_from_detections: the same table built on the device from the per-image detection lists the
  *   reference keeps before tables.make_point_table (tables.py:68-81; fill_sparse 15-21): list w = (c*F+f)*B+b
  *   holds det_ids[det_start[w]..det_start[w+1]) (point ids on board b) and det_xy (pixel corners).  Ids outside
- *   [0,P) fail with MCBA_ERR_ARG; a repeated id within one list keeps an unspecified one of its corners.
- * Both reset the parameter state to zero like mcba_upload; set it afterwards.                                    */
+ *   [0,P), and an id repeated within one list, fail with MCBA_ERR_ARG.
+ * Both reset the parameter state to zero like mcba_upload_dense; set it afterwards.                              */
 typedef struct mcba_table_stats {
   int64_t n_valid, n_inliers;          /* corners in `valid` / in the current inlier mask                        */
   double  sumsq_valid, sumsq_inliers;  /* sum of squared pixel errors over each set (mse = sumsq / n)            */

@@ -23,7 +23,7 @@ STATUS_MESSAGES = {
   4: "Both `ftol` and `xtol` termination conditions are satisfied.",
 }
 EXPORTS = ["mcba_create", "mcba_destroy", "mcba_last_error", "mcba_set_stream", "mcba_version",
-           "mcba_comm_unique_id", "mcba_comm_init", "mcba_peer_export", "mcba_peer_import", "mcba_upload", "mcba_upload_dense", "mcba_upload_dense_views", "mcba_upload_dense_views_f32", "mcba_set_params", "mcba_get_params", "mcba_set_state_matrices", "mcba_get_state_matrices",
+           "mcba_comm_unique_id", "mcba_comm_init", "mcba_peer_export", "mcba_peer_import", "mcba_upload_dense", "mcba_set_params", "mcba_get_params", "mcba_set_state_matrices", "mcba_get_state_matrices",
            "mcba_set_rolling", "mcba_get_rolling", "mcba_set_hand_eye", "mcba_get_hand_eye", "mcba_set_fixed_intrinsics",
            "mcba_num_params", "mcba_get_param_vec", "mcba_set_param_vec", "mcba_residuals",
            "mcba_linearize", "mcba_reprojection_error", "mcba_solve", "mcba_bench_launch", "mcba_bench_info",
@@ -34,6 +34,7 @@ EXPORTS = ["mcba_create", "mcba_destroy", "mcba_last_error", "mcba_set_stream", 
            "mcba_undistort_points", "mcba_remap_cubic_table", "mcba_stereo_init", "mcba_rectify_map", "mcba_rectify_images",
            "mcba_rectify_points", "mcba_triangulate", "mcba_triangulate_linear"]
 IMAGE_UINT8 = 0          # include/mcba.h MCBA_IMAGE_UINT8
+POINTS_F64, POINTS_F32 = 0, 1          # include/mcba.h MCBA_POINTS_*
 TABLE_VALID, TABLE_INLIERS = 0, 1
 
 
@@ -91,10 +92,8 @@ def load():
   lib.mcba_comm_init.argtypes = [P, C.c_char_p, C.c_int, C.c_int]
   lib.mcba_peer_export.argtypes = [P, C.c_int64, C.c_char_p]
   lib.mcba_peer_import.argtypes = [P, C.c_char_p]
-  lib.mcba_upload.argtypes = [P, C.POINTER(ProblemDesc), I32, I32, I32, I32, D, D]
-  lib.mcba_upload_dense.argtypes = [P, C.POINTER(ProblemDesc), C.POINTER(C.c_uint8), D, D, C.POINTER(C.c_int64)]
-  lib.mcba_upload_dense_views.argtypes = [P, C.POINTER(ProblemDesc), C.POINTER(C.c_uint8), C.POINTER(C.c_uint8), D, D, C.POINTER(C.c_int64)]
-  lib.mcba_upload_dense_views_f32.argtypes = [P, C.POINTER(ProblemDesc), C.POINTER(C.c_uint8), C.POINTER(C.c_uint8), C.POINTER(C.c_float), D, C.POINTER(C.c_int64)]
+  lib.mcba_upload_dense.argtypes = [P, C.POINTER(ProblemDesc), C.POINTER(C.c_uint8), C.POINTER(C.c_uint8), P, C.c_int32, D,
+                                    C.POINTER(C.c_int64)]
   lib.mcba_set_params.argtypes = [P, D, D, D, D]
   lib.mcba_get_params.argtypes = [P, D, D, D, D]
   lib.mcba_set_state_matrices.argtypes = [P, D, D]

@@ -17,7 +17,7 @@ from . import rtvec
 from ._native import OPT_BITS, OPT_FIX_ASPECT
 from .board import stack_boards
 from .camera import engine_model_of
-from .engine import Engine, format_log, pack_corners
+from .engine import Engine, format_log
 from .log import info
 from .motion import MOTION_HAND_EYE, MOTION_ROLLING, motion_kind
 from .outliers import QuantileThreshold, select_threshold      # noqa: F401  (select_threshold: calibration.py:37-40)

@@ -1,6 +1,6 @@
 // kernels.cuh — sm_90a kernels of the bundle-adjustment hot path.
 //
-// Data layout in HBM (built once per upload: on the host by mcba_upload, on the device by pack_kernels.cuh): corners are stored FRAME-MAJOR, sorted by
+// Data layout in HBM (built once per upload from the dense table, on the device by pack_kernels.cuh): corners are stored FRAME-MAJOR, sorted by
 // (frame, camera, board, point), so that every "view" (frame,camera,board) is one contiguous run and all
 // views of one frame are contiguous (frames are also the multi-GPU sharding unit, SURVEY.md §8e):
 //   obs   double2[N]   observed (u,v)                       16 B / corner   (point_table.points, calibration.py:206)

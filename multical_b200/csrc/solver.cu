@@ -127,8 +127,9 @@ struct mcba_ctx {
   // problem arrays
   DevBuf<double2> obs; DevBuf<uint16_t> pid; DevBuf<uint32_t> orig;
   DevBuf<int> view_start, view_cam, view_frame, view_board, frame_view_start;
-  DevBuf<uint8_t> dense_mask, view_valid; DevBuf<double2> dense_pts; DevBuf<float2> dense_pts32; DevBuf<int> scan;
-  cudaStream_t copy_stream = nullptr; cudaEvent_t copy_done = nullptr, copy_go = nullptr;      // observations of mcba_upload_dense* in flight beside the view count
+  // the staged dense [C,F,B,P] table every upload packs from (the resident table's `valid` and observations): selection mask, pixels
+  DevBuf<uint8_t> valid_mask, view_valid; DevBuf<double2> dense_pts; DevBuf<float2> dense_pts32; DevBuf<int> scan;
+  cudaStream_t copy_stream = nullptr; cudaEvent_t copy_done = nullptr, copy_go = nullptr;      // observations in flight beside the view count
   DevBuf<PoseT> cam_T, frame_T, board_T;
   // parameter state (state_layout): current and trial
   StateLayout layout{};
@@ -158,11 +159,11 @@ struct mcba_ctx {
   double* peer_base[PEER_MAX_WORLD] = {nullptr};
   std::vector<void*> peer_opened;
   std::vector<int> perm;   // internal index -> canonical param_vec index
-  // resident point table (mcba_table_*): `valid` and inlier masks, sorted per-corner errors
+  // resident point table (mcba_table_*): inlier mask, sorted per-corner errors
   bool table = false; int table_selected = -1; bool errors_current = false;
   mcba_problem_desc table_desc{};
   int64_t n_valid = 0, n_inliers = 0;
-  DevBuf<uint8_t> valid_mask, inlier_mask;
+  DevBuf<uint8_t> inlier_mask;
   DevBuf<double> err_valid, err_sorted, err_inl, err_inl_sorted, table_part, table_out;
   DevBuf<int64_t> table_ranks;
   DevBuf<unsigned char> sort_tmp;
@@ -655,6 +656,7 @@ int pack_dense(mcba_ctx* ctx, const mcba_problem_desc* desc, const uint8_t* d_ma
   int* cnt_can = ctx->scan.p; int* cnt_fm = cnt_can + (nv + 1); int* flag_fm = cnt_fm + (nv + 1);
   int totals[2] = {0, 0};
   UploadClock clk(ctx->profiling);
+  ctx->uploaded = false;      // the problem's buffers change from here on: set again only when setup_problem succeeds
   if (nv > 0) {
     k_pack_count<<<(unsigned)(((size_t)nv * 32 + 255) / 256), 256, 0, s>>>(d_mask, d_view_valid, C, F, B, Pn, cnt_can, cnt_fm, flag_fm); CKL();
     k_scan_exclusive<<<3, 1024, 0, s>>>(cnt_can, nv, nv + 1); CKL();      // cnt_can | cnt_fm | flag_fm
@@ -822,154 +824,137 @@ int mcba_peer_import(mcba_ctx* ctx, const char* handles /* world x 64 bytes, ran
   return MCBA_OK;
 }
 
-int mcba_upload(mcba_ctx* ctx, const mcba_problem_desc* desc, const int32_t* cam, const int32_t* frame,
-                const int32_t* board, const int32_t* point, const double* obs, const double* board_points) {
-  if (!ctx || !desc) return MCBA_ERR_ARG;
-  CK(cudaSetDevice(ctx->device));
-  const int C = desc->C, F = desc->F, B = desc->B, Pn = desc->P;
-  const int64_t N = desc->N;
-  { int r = check_desc(ctx, desc); if (r) return r; }
-  REQUIRE(N >= 0 && N < ((int64_t)1 << 31), MCBA_ERR_UNSUPPORTED, "corner count out of range");
-  REQUIRE(N == 0 || (cam && frame && board && point && obs), MCBA_ERR_ARG, "null corner arrays");
-  REQUIRE(board_points != nullptr, MCBA_ERR_ARG, "null board points");
-  ctx->table = false; ctx->table_selected = -1; ctx->errors_current = false;
+// ---------------------------------------------------------------------------------------------------------------
+// Problem intake.  Every problem reaches the kernels the same way: a dense [C,F,B,P] table is staged on the device (ctx->valid_mask
+// selects the corners, ctx->dense_pts or dense_pts32 holds their pixels) and pack_dense packs the selection frame-major
+// (pack_kernels.cuh).  A caller's inputs are checked before any buffer of the context changes.
 
-  // ---- pack: stable counting sort of the canonical (c,f,b,p)-ordered corners by frame => (f,c,b,p) order
-  std::vector<int64_t> fcount((size_t)F + 1, 0);
-  for (int64_t k = 0; k < N; k++) {
-    const int c = cam[k], f = frame[k], b = board[k], p = point[k];
-    if (c < 0 || c >= C || f < 0 || f >= F || b < 0 || b >= B || p < 0 || p >= Pn) { ctx->err = "corner index out of range"; return MCBA_ERR_ARG; }
-    fcount[(size_t)f + 1]++;
-  }
-  for (int f = 0; f < F; f++) fcount[(size_t)f + 1] += fcount[f];
-  std::vector<uint32_t> order((size_t)N);
-  {
-    std::vector<int64_t> cursor(fcount.begin(), fcount.end() - 1);
-    for (int64_t k = 0; k < N; k++) order[(size_t)cursor[frame[k]]++] = (uint32_t)k;
-  }
-  std::vector<double2> h_obs((size_t)N);
-  std::vector<uint16_t> h_pid((size_t)N);
-  std::vector<int> vstart, vcam, vframe, vboard, fvs((size_t)F + 1, 0);
-  int prev_c = -1, prev_f = -1, prev_b = -1;
-  for (int64_t i = 0; i < N; i++) {
-    const uint32_t k = order[(size_t)i];
-    h_obs[(size_t)i] = make_double2(obs[2 * (size_t)k], obs[2 * (size_t)k + 1]);
-    h_pid[(size_t)i] = (uint16_t)point[k];
-    const int c = cam[k], f = frame[k], b = board[k];
-    if (c != prev_c || f != prev_f || b != prev_b) {
-      vstart.push_back((int)i); vcam.push_back(c); vframe.push_back(f); vboard.push_back(b);
-      prev_c = c; prev_f = f; prev_b = b;
-    }
-  }
-  const int V = (int)vcam.size();
-  vstart.push_back((int)N);
-  {
-    std::vector<int> cnt((size_t)F + 1, 0);
-    for (int v = 0; v < V; v++) cnt[(size_t)vframe[v] + 1]++;
-    for (int f = 0; f < F; f++) cnt[(size_t)f + 1] += cnt[f];
-    fvs = cnt;
-  }
+namespace {
 
-#define UP(buf, vec) do { CK(ctx->buf.alloc((vec).size())); if (!(vec).empty()) CK(cudaMemcpyAsync(ctx->buf.p, (vec).data(), (vec).size() * sizeof((vec)[0]), cudaMemcpyHostToDevice, ctx->stream)); } while (0)
-  UP(obs, h_obs); UP(pid, h_pid); UP(orig, order);
-  UP(view_start, vstart); UP(view_cam, vcam); UP(view_frame, vframe); UP(view_board, vboard);
-  UP(frame_view_start, fvs);
-#undef UP
-  double* bpts = nullptr;
-  { int r = alloc_state(ctx, desc, &bpts); if (r) return r; }
-  CK(cudaMemcpyAsync(bpts, board_points, sizeof(double) * (size_t)B * Pn * 3, cudaMemcpyHostToDevice, ctx->stream));
-  { int r = setup_problem(ctx, desc, N, V); if (r) return r; }
-  CK(cudaStreamSynchronize(ctx->stream));    // host staging vectors go out of scope
-  ctx->uploaded = true;
+bool all_finite(const double* p, size_t n) {
+  for (size_t i = 0; i < n; i++) if (!std::isfinite(p[i])) return false;
+  return true;
+}
+
+// The caller's detection lists: list w = (c*F+f)*B+b of the C*F*B views holds point ids det_ids[det_start[w]:det_start[w+1]] in [0, P) and
+// their pixel corners det_xy (a CSR layout); the boards' id grids, when given, are at most 64 x 64.
+int check_detections(mcba_ctx* ctx, const mcba_problem_desc* desc, const int64_t* det_start, const int32_t* det_ids, const double* det_xy,
+                     const int32_t* board_grid) {
+  const int nv = desc->C * desc->F * desc->B;
+  const int64_t total = det_start[nv];
+  REQUIRE(det_start[0] == 0 && total >= 0 && total < ((int64_t)1 << 31), MCBA_ERR_ARG, "bad detection offsets");
+  REQUIRE(total == 0 || (det_ids && det_xy), MCBA_ERR_ARG, "null detection arrays");
+  for (int w = 0; w < nv; w++) REQUIRE(det_start[w + 1] >= det_start[w], MCBA_ERR_ARG, "detection offsets are not a monotone CSR over C*F*B lists");
+  for (int64_t i = 0; i < total; i++) REQUIRE(det_ids[i] >= 0 && det_ids[i] < desc->P, MCBA_ERR_ARG, "detection id outside [0, P)");
+  for (int b = 0; board_grid && b < desc->B; b++)
+    REQUIRE(board_grid[5 * b] > 0 && board_grid[5 * b + 1] > 0 && board_grid[5 * b + 2] > 0 && board_grid[5 * b] <= 64 && board_grid[5 * b + 1] <= 64,
+            MCBA_ERR_UNSUPPORTED, "id grids are limited to 64 x 64 (bit masks of the occupied rows / columns)");
   return MCBA_OK;
 }
 
-// Dense variant: the [C,F,B,P] inlier mask and [C,F,B,P,2] observations go to the device as they are and the
-// packing (frame-major order, view records, canonical index map) happens there (pack_kernels.cuh).
-namespace {
-int upload_dense_any(mcba_ctx* ctx, const mcba_problem_desc* desc, const uint8_t* valid, const uint8_t* view_valid, const void* points, bool points_f32,
-                     const double* board_points, int64_t* n_corners) {
+// detection lists in that layout -> ctx->pnp, with the id grids and the board points when given (the point table needs the lists only)
+int stage_detections(mcba_ctx* ctx, const mcba_problem_desc* desc, const int64_t* det_start, const int32_t* det_ids, const double* det_xy,
+                     const int32_t* board_grid, const double* board_points) {
+  const int nv = desc->C * desc->F * desc->B, B = desc->B, Pn = desc->P;
+  const int64_t total = det_start[nv];
+  cudaStream_t s = ctx->stream;
+  auto& pb = ctx->pnp;
+  const size_t tot = (size_t)std::max<int64_t>(total, 1);
+  CK(pb.start.alloc((size_t)nv + 1)); CK(pb.ids.alloc(tot)); CK(pb.xy.alloc(tot));
+  CK(cudaMemcpyAsync(pb.start.p, det_start, sizeof(int64_t) * ((size_t)nv + 1), cudaMemcpyHostToDevice, s));
+  if (total) {
+    CK(cudaMemcpyAsync(pb.ids.p, det_ids, sizeof(int32_t) * (size_t)total, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(pb.xy.p, det_xy, sizeof(double2) * (size_t)total, cudaMemcpyHostToDevice, s));
+  }
+  if (board_grid) {
+    CK(pb.grid.alloc((size_t)B * 5));
+    CK(cudaMemcpyAsync(pb.grid.p, board_grid, sizeof(int32_t) * (size_t)B * 5, cudaMemcpyHostToDevice, s));
+  }
+  if (board_points) {
+    CK(pb.bp.alloc((size_t)B * Pn * 3));
+    CK(cudaMemcpyAsync(pb.bp.p, board_points, sizeof(double) * (size_t)B * Pn * 3, cudaMemcpyHostToDevice, s));
+  }
+  return MCBA_OK;
+}
+
+// k_pnp_views over the staged lists: one warp per list, poses under the intrinsics intr [C][kint] (device) of camera model `model`
+int launch_pnp(mcba_ctx* ctx, const mcba_problem_desc* desc, int model, int kint, const double* intr) {
+  auto& pb = ctx->pnp;
+  PnpArgs a{};
+  a.C = desc->C; a.F = desc->F; a.B = desc->B; a.P = desc->P; a.model = model; a.kint = kint; a.nv = desc->C * desc->F * desc->B;
+  CK(pb.und.alloc(pb.ids.n)); CK(pb.pose.alloc((size_t)a.nv * 16)); CK(pb.err.alloc(a.nv)); CK(pb.n.alloc(a.nv)); CK(pb.ok.alloc(a.nv));
+  a.det_start = pb.start.p; a.det_ids = pb.ids.p; a.det_xy = pb.xy.p; a.board_pts = pb.bp.p; a.intr = intr; a.grid = pb.grid.p;
+  a.und = pb.und.p; a.poses = pb.pose.p; a.err = pb.err.p; a.npts = pb.n.p; a.valid = pb.ok.p; a.max_iters = 50;
+  const int blocks = (a.nv + PNP_WARPS - 1) / PNP_WARPS;
+  with_model(model, false, [&](auto M, auto) {
+    constexpr int MODEL = decltype(M)::value;
+    k_pnp_views<MODEL><<<blocks, PNP_WARPS * 32, 0, ctx->stream>>>(a);
+  });
+  CKL();
+  return MCBA_OK;
+}
+
+// Every upload starts here: whatever it refuses, and however late, it leaves no problem rather than a stale one (the entry points that
+// need one fail with MCBA_ERR_STATE until an upload succeeds).
+void drop_problem(mcba_ctx* ctx) {
+  ctx->uploaded = false; ctx->table = false; ctx->table_selected = -1; ctx->errors_current = false;
+}
+
+// the dense table and the parameter state of `desc`; *board_pts receives where the board points go
+int begin_intake(mcba_ctx* ctx, const mcba_problem_desc* desc, bool points_f32, double** board_pts) {
+  const size_t dense = std::max<size_t>((size_t)desc->C * desc->F * desc->B * desc->P, 1);
+  CK(ctx->valid_mask.alloc(dense));
+  if (points_f32) CK(ctx->dense_pts32.alloc(dense)); else CK(ctx->dense_pts.alloc(dense));
+  return alloc_state(ctx, desc, board_pts);
+}
+
+// A dense host table -> ctx->valid_mask (and ctx->view_valid), its points -> dense_pts or dense_pts32, the board points -> the state.
+// *points_ready: the event after which the points are on the device, or null.
+int stage_dense(mcba_ctx* ctx, const mcba_problem_desc* desc, const uint8_t* valid, const uint8_t* view_valid, const void* points,
+                int32_t point_type, const double* board_points, cudaEvent_t* points_ready) {
   if (!ctx || !desc) return MCBA_ERR_ARG;
+  drop_problem(ctx);
   CK(cudaSetDevice(ctx->device));
   { int r = check_desc(ctx, desc); if (r) return r; }
   REQUIRE(valid && points && board_points, MCBA_ERR_ARG, "null dense table");
-  const int C = desc->C, F = desc->F, B = desc->B, Pn = desc->P;
-  const int nv = C * F * B;
-  const size_t dense = (size_t)nv * Pn;
-  cudaStream_t s = ctx->stream;
-  CK(ctx->dense_mask.alloc(std::max<size_t>(dense, 1)));
-  if (points_f32) CK(ctx->dense_pts32.alloc(std::max<size_t>(dense, 1))); else CK(ctx->dense_pts.alloc(std::max<size_t>(dense, 1)));
-  CK(ctx->view_valid.alloc(std::max<size_t>((size_t)nv, 1)));
-  CK(ctx->scan.alloc((size_t)3 * (nv + 1)));
+  REQUIRE(point_type == MCBA_POINTS_F64 || point_type == MCBA_POINTS_F32, MCBA_ERR_ARG, "unknown point type");
+  const bool points_f32 = point_type == MCBA_POINTS_F32;
+  const int nv = desc->C * desc->F * desc->B;
+  const size_t dense = (size_t)nv * desc->P;
   double* bpts = nullptr;
-  { int r = alloc_state(ctx, desc, &bpts); if (r) return r; }
-  cudaEvent_t ready = nullptr;
+  { int r = begin_intake(ctx, desc, points_f32, &bpts); if (r) return r; }
+  if (view_valid) CK(ctx->view_valid.alloc((size_t)std::max(nv, 1)));
+  cudaStream_t s = ctx->stream;
   UploadClock clk(ctx->profiling);
+  *points_ready = nullptr;
+  // the mask (1 B/point) goes first on the solver's stream; the observations (16 B/point) follow on the copy stream while the views
+  // are counted and scanned, and the scatter waits for them
+  if (dense) CK(cudaMemcpyAsync(ctx->valid_mask.p, valid, dense, cudaMemcpyHostToDevice, s));
+  if (dense && view_valid) CK(cudaMemcpyAsync(ctx->view_valid.p, view_valid, (size_t)nv, cudaMemcpyHostToDevice, s));
+  // the small copies from pageable memory go BEFORE the table: such a copy returns when it is done, and behind 100 MB on the copy engine
+  // it would hold the host back until the table has crossed the link -- with it the count / scan kernels that should run beside it
+  CK(cudaMemcpyAsync(bpts, board_points, sizeof(double) * (size_t)desc->B * desc->P * 3, cudaMemcpyHostToDevice, s));
   if (dense) {
-    // the mask (1 B/point) goes first on the solver's stream; the observations (16 B/point) follow on the copy stream while the views
-    // are counted and scanned, and the scatter waits for them
-    CK(cudaMemcpyAsync(ctx->dense_mask.p, valid, dense, cudaMemcpyHostToDevice, s));
-    if (view_valid) CK(cudaMemcpyAsync(ctx->view_valid.p, view_valid, (size_t)nv, cudaMemcpyHostToDevice, s));
-    // the small copies from pageable memory go BEFORE the table: such a copy returns when it is done, and behind 100 MB on the copy engine
-    // it would hold the host back until the table has crossed the link -- with it the count / scan kernels that should run beside it
-    CK(cudaMemcpyAsync(bpts, board_points, sizeof(double) * (size_t)B * Pn * 3, cudaMemcpyHostToDevice, s));
     if (!ctx->copy_stream) { CK(cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking)); CK(cudaEventCreateWithFlags(&ctx->copy_done, cudaEventDisableTiming)); CK(cudaEventCreateWithFlags(&ctx->copy_go, cudaEventDisableTiming)); }
     CK(cudaEventRecord(ctx->copy_go, s));                          // work queued on `s` before this call may still read dense_pts
     CK(cudaStreamWaitEvent(ctx->copy_stream, ctx->copy_go, 0));
     if (points_f32) CK(cudaMemcpyAsync(ctx->dense_pts32.p, points, dense * sizeof(float2), cudaMemcpyHostToDevice, ctx->copy_stream));
     else CK(cudaMemcpyAsync(ctx->dense_pts.p, points, dense * sizeof(double2), cudaMemcpyHostToDevice, ctx->copy_stream));
     CK(cudaEventRecord(ctx->copy_done, ctx->copy_stream));
-    ready = ctx->copy_done;
+    *points_ready = ctx->copy_done;
     clk.mark("upload: copies issued");
-  } else {
-    CK(cudaMemcpyAsync(bpts, board_points, sizeof(double) * (size_t)B * Pn * 3, cudaMemcpyHostToDevice, s));
   }
-  ctx->table = false; ctx->table_selected = -1; ctx->errors_current = false;
-  return pack_dense(ctx, desc, ctx->dense_mask.p, false, n_corners, view_valid ? ctx->view_valid.p : nullptr, ready, points_f32);
-}
-}  // namespace
-
-int mcba_upload_dense_views(mcba_ctx* ctx, const mcba_problem_desc* desc, const uint8_t* valid, const uint8_t* view_valid, const double* points,
-                            const double* board_points, int64_t* n_corners) {
-  return upload_dense_any(ctx, desc, valid, view_valid, points, false, board_points, n_corners);
-}
-
-int mcba_upload_dense_views_f32(mcba_ctx* ctx, const mcba_problem_desc* desc, const uint8_t* valid, const uint8_t* view_valid, const float* points,
-                                const double* board_points, int64_t* n_corners) {
-  return upload_dense_any(ctx, desc, valid, view_valid, points, true, board_points, n_corners);
-}
-
-int mcba_upload_dense(mcba_ctx* ctx, const mcba_problem_desc* desc, const uint8_t* mask, const double* points,
-                      const double* board_points, int64_t* n_corners) {
-  return mcba_upload_dense_views(ctx, desc, mask, nullptr, points, board_points, n_corners);
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// Resident point table (include/mcba.h "resident point table"): Calibration.adjust_outliers without host round trips.
-
-namespace {
-
-int table_begin(mcba_ctx* ctx, const mcba_problem_desc* desc, const double* board_points, size_t* dense_out) {
-  CK(cudaSetDevice(ctx->device));
-  { int r = check_desc(ctx, desc); if (r) return r; }
-  REQUIRE(board_points != nullptr, MCBA_ERR_ARG, "null board points");
-  const size_t dense = (size_t)desc->C * desc->F * desc->B * desc->P;
-  CK(ctx->valid_mask.alloc(std::max<size_t>(dense, 1))); CK(ctx->inlier_mask.alloc(std::max<size_t>(dense, 1)));
-  CK(ctx->dense_pts.alloc(std::max<size_t>(dense, 1)));
-  double* bpts = nullptr;
-  { int r = alloc_state(ctx, desc, &bpts); if (r) return r; }
-  CK(cudaMemcpyAsync(bpts, board_points, sizeof(double) * (size_t)desc->B * desc->P * 3, cudaMemcpyHostToDevice, ctx->stream));
-  ctx->table = false; ctx->table_selected = -1; ctx->errors_current = false;
-  *dense_out = dense;
   return MCBA_OK;
 }
 
-// inliers = valid, pack `valid`, remember the description
-int table_finish(mcba_ctx* ctx, const mcba_problem_desc* desc, size_t dense, int64_t* n_valid) {
+// the staged table becomes the resident one: inliers = valid, pack `valid`, remember the description
+int table_finish(mcba_ctx* ctx, const mcba_problem_desc* desc, cudaEvent_t points_ready, int64_t* n_valid) {
+  const size_t dense = (size_t)desc->C * desc->F * desc->B * desc->P;
+  CK(ctx->inlier_mask.alloc(std::max<size_t>(dense, 1)));
   if (dense) CK(cudaMemcpyAsync(ctx->inlier_mask.p, ctx->valid_mask.p, dense, cudaMemcpyDeviceToDevice, ctx->stream));
   ctx->table_desc = *desc;
   int64_t n = 0;
-  { int r = pack_dense(ctx, desc, ctx->valid_mask.p, false, &n); if (r) return r; }
+  { int r = pack_dense(ctx, desc, ctx->valid_mask.p, false, &n, nullptr, points_ready); if (r) return r; }
   ctx->table = true; ctx->table_selected = MCBA_TABLE_VALID;
   ctx->n_valid = n; ctx->n_inliers = n;
   if (n_valid) *n_valid = n;
@@ -993,116 +978,57 @@ int sort_errors(mcba_ctx* ctx, const double* in, double* out, int64_t n) {
 
 }  // namespace
 
+int mcba_upload_dense(mcba_ctx* ctx, const mcba_problem_desc* desc, const uint8_t* valid, const uint8_t* view_valid, const void* points,
+                      int32_t point_type, const double* board_points, int64_t* n_corners) {
+  cudaEvent_t ready = nullptr;
+  { int r = stage_dense(ctx, desc, valid, view_valid, points, point_type, board_points, &ready); if (r) return r; }
+  return pack_dense(ctx, desc, ctx->valid_mask.p, false, n_corners, view_valid ? ctx->view_valid.p : nullptr, ready,
+                    point_type == MCBA_POINTS_F32);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Resident point table (include/mcba.h "resident point table"): Calibration.adjust_outliers without host round trips.
+
 int mcba_table_upload(mcba_ctx* ctx, const mcba_problem_desc* desc, const uint8_t* valid, const double* points,
                       const double* board_points, int64_t* n_valid) {
-  if (!ctx || !desc) return MCBA_ERR_ARG;
-  REQUIRE(valid && points, MCBA_ERR_ARG, "null dense table");
-  size_t dense = 0;
-  { int r = table_begin(ctx, desc, board_points, &dense); if (r) return r; }
-  if (dense) {
-    CK(cudaMemcpyAsync(ctx->valid_mask.p, valid, dense, cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpyAsync(ctx->dense_pts.p, points, dense * sizeof(double2), cudaMemcpyHostToDevice, ctx->stream));
-  }
-  return table_finish(ctx, desc, dense, n_valid);
+  cudaEvent_t ready = nullptr;
+  { int r = stage_dense(ctx, desc, valid, nullptr, points, MCBA_POINTS_F64, board_points, &ready); if (r) return r; }
+  return table_finish(ctx, desc, ready, n_valid);
 }
 
 int mcba_table_from_detections(mcba_ctx* ctx, const mcba_problem_desc* desc, const int64_t* det_start, const int32_t* det_ids,
                                const double* det_xy, const double* board_points, int64_t* n_valid) {
   if (!ctx || !desc) return MCBA_ERR_ARG;
-  REQUIRE(det_start != nullptr, MCBA_ERR_ARG, "null detection offsets");
-  size_t dense = 0;
-  { int r = table_begin(ctx, desc, board_points, &dense); if (r) return r; }
+  drop_problem(ctx);
+  CK(cudaSetDevice(ctx->device));
+  { int r = check_desc(ctx, desc); if (r) return r; }
+  REQUIRE(det_start && board_points, MCBA_ERR_ARG, "null argument");
+  { int r = check_detections(ctx, desc, det_start, det_ids, det_xy, nullptr); if (r) return r; }
   const int nv = desc->C * desc->F * desc->B;
-  const int64_t total = det_start[nv];
-  REQUIRE(det_start[0] == 0 && total >= 0 && total < ((int64_t)1 << 31), MCBA_ERR_ARG, "bad detection offsets");
-  REQUIRE(total == 0 || (det_ids && det_xy), MCBA_ERR_ARG, "null detection arrays");
-  cudaStream_t s = ctx->stream;
-  DevBuf<int64_t> d_start; DevBuf<int32_t> d_ids; DevBuf<double2> d_xy; DevBuf<int> d_bad;
-  CK(d_start.alloc((size_t)nv + 1)); CK(d_ids.alloc((size_t)std::max<int64_t>(total, 1))); CK(d_xy.alloc((size_t)std::max<int64_t>(total, 1))); CK(d_bad.alloc(1));
-  CK(cudaMemcpyAsync(d_start.p, det_start, sizeof(int64_t) * ((size_t)nv + 1), cudaMemcpyHostToDevice, s));
-  if (total) {
-    CK(cudaMemcpyAsync(d_ids.p, det_ids, sizeof(int32_t) * (size_t)total, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(d_xy.p, det_xy, sizeof(double2) * (size_t)total, cudaMemcpyHostToDevice, s));
+  {   // a table entry holds one corner
+    std::vector<int> list_of((size_t)desc->P, -1);
+    for (int w = 0; w < nv; w++)
+      for (int64_t i = det_start[w]; i < det_start[w + 1]; i++) {
+        REQUIRE(list_of[det_ids[i]] != w, MCBA_ERR_ARG, "detection list " + std::to_string(w) + " repeats point id " + std::to_string(det_ids[i]));
+        list_of[det_ids[i]] = w;
+      }
   }
-  CK(cudaMemsetAsync(d_bad.p, 0, sizeof(int), s));
+  const size_t dense = (size_t)nv * desc->P;
+  cudaStream_t s = ctx->stream;
+  double* bpts = nullptr;
+  { int r = begin_intake(ctx, desc, false, &bpts); if (r) return r; }
+  CK(cudaMemcpyAsync(bpts, board_points, sizeof(double) * (size_t)desc->B * desc->P * 3, cudaMemcpyHostToDevice, s));
+  { int r = stage_detections(ctx, desc, det_start, det_ids, det_xy, nullptr, nullptr); if (r) return r; }
   if (dense) {
     CK(cudaMemsetAsync(ctx->valid_mask.p, 0, dense, s));
     CK(cudaMemsetAsync(ctx->dense_pts.p, 0, dense * sizeof(double2), s));    // fill_sparse leaves zeros where nothing was detected
   }
-  int bad = 0;
-  k_table_check_offsets<<<(nv + 1 + 255) / 256, 256, 0, s>>>(d_start.p, nv, total, d_bad.p); CKL();
-  CK(cudaMemcpyAsync(&bad, d_bad.p, sizeof(int), cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  REQUIRE(!bad, MCBA_ERR_ARG, "detection offsets are not a monotone CSR over C*F*B lists");
-  if (nv > 0 && total > 0) {
-    k_table_fill<<<(unsigned)(((size_t)nv * 32 + 255) / 256), 256, 0, s>>>(d_start.p, d_ids.p, d_xy.p, nv, desc->P, ctx->valid_mask.p, ctx->dense_pts.p, d_bad.p); CKL();
-    CK(cudaMemcpyAsync(&bad, d_bad.p, sizeof(int), cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    REQUIRE(!bad, MCBA_ERR_ARG, "detection id outside [0, P)");
+  if (det_start[nv] > 0) {      // the ids were checked above: k_table_fill's range guard never writes its flag
+    auto& pb = ctx->pnp;
+    k_table_fill<<<(unsigned)(((size_t)nv * 32 + 255) / 256), 256, 0, s>>>(pb.start.p, pb.ids.p, pb.xy.p, nv, desc->P, ctx->valid_mask.p, ctx->dense_pts.p, nullptr); CKL();
   }
-  return table_finish(ctx, desc, dense, n_valid);
+  return table_finish(ctx, desc, nullptr, n_valid);
 }
-
-namespace {
-
-bool all_finite(const double* p, size_t n) {
-  for (size_t i = 0; i < n; i++) if (!std::isfinite(p[i])) return false;
-  return true;
-}
-
-// The caller's detection lists: list w = (c*F+f)*B+b of the C*F*B views holds point ids det_ids[det_start[w]:det_start[w+1]] in [0, P) and
-// their pixel corners det_xy (a CSR layout); the boards' id grids are at most 64 x 64.
-int check_detections(mcba_ctx* ctx, const mcba_problem_desc* desc, const int64_t* det_start, const int32_t* det_ids, const double* det_xy,
-                     const int32_t* board_grid) {
-  const int nv = desc->C * desc->F * desc->B;
-  const int64_t total = det_start[nv];
-  REQUIRE(det_start[0] == 0 && total >= 0 && total < ((int64_t)1 << 31), MCBA_ERR_ARG, "bad detection offsets");
-  REQUIRE(total == 0 || (det_ids && det_xy), MCBA_ERR_ARG, "null detection arrays");
-  for (int w = 0; w < nv; w++) REQUIRE(det_start[w + 1] >= det_start[w], MCBA_ERR_ARG, "detection offsets are not a monotone CSR over C*F*B lists");
-  for (int64_t i = 0; i < total; i++) REQUIRE(det_ids[i] >= 0 && det_ids[i] < desc->P, MCBA_ERR_ARG, "detection id outside [0, P)");
-  for (int b = 0; b < desc->B; b++)
-    REQUIRE(board_grid[5 * b] > 0 && board_grid[5 * b + 1] > 0 && board_grid[5 * b + 2] > 0 && board_grid[5 * b] <= 64 && board_grid[5 * b + 1] <= 64,
-            MCBA_ERR_UNSUPPORTED, "id grids are limited to 64 x 64 (bit masks of the occupied rows / columns)");
-  return MCBA_OK;
-}
-
-// detection lists in that layout, the id grids and the board points -> ctx->pnp, with room for the outputs of k_pnp_views
-int stage_detections(mcba_ctx* ctx, const mcba_problem_desc* desc, const int64_t* det_start, const int32_t* det_ids, const double* det_xy,
-                     const int32_t* board_grid, const double* board_points) {
-  const int nv = desc->C * desc->F * desc->B, B = desc->B, Pn = desc->P;
-  const int64_t total = det_start[nv];
-  cudaStream_t s = ctx->stream;
-  auto& pb = ctx->pnp;
-  const size_t tot = (size_t)std::max<int64_t>(total, 1);
-  CK(pb.start.alloc((size_t)nv + 1)); CK(pb.ids.alloc(tot)); CK(pb.xy.alloc(tot)); CK(pb.und.alloc(tot)); CK(pb.grid.alloc((size_t)B * 5));
-  CK(pb.bp.alloc((size_t)B * Pn * 3)); CK(pb.pose.alloc((size_t)nv * 16)); CK(pb.err.alloc(nv)); CK(pb.n.alloc(nv)); CK(pb.ok.alloc(nv));
-  CK(cudaMemcpyAsync(pb.start.p, det_start, sizeof(int64_t) * ((size_t)nv + 1), cudaMemcpyHostToDevice, s));
-  if (total) {
-    CK(cudaMemcpyAsync(pb.ids.p, det_ids, sizeof(int32_t) * (size_t)total, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(pb.xy.p, det_xy, sizeof(double2) * (size_t)total, cudaMemcpyHostToDevice, s));
-  }
-  CK(cudaMemcpyAsync(pb.grid.p, board_grid, sizeof(int32_t) * (size_t)B * 5, cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(pb.bp.p, board_points, sizeof(double) * (size_t)B * Pn * 3, cudaMemcpyHostToDevice, s));
-  return MCBA_OK;
-}
-
-// k_pnp_views over the staged lists: one warp per list, poses under the intrinsics intr [C][kint] (device) of camera model `model`
-int launch_pnp(mcba_ctx* ctx, const mcba_problem_desc* desc, int model, int kint, const double* intr) {
-  auto& pb = ctx->pnp;
-  PnpArgs a{};
-  a.C = desc->C; a.F = desc->F; a.B = desc->B; a.P = desc->P; a.model = model; a.kint = kint; a.nv = desc->C * desc->F * desc->B;
-  a.det_start = pb.start.p; a.det_ids = pb.ids.p; a.det_xy = pb.xy.p; a.board_pts = pb.bp.p; a.intr = intr; a.grid = pb.grid.p;
-  a.und = pb.und.p; a.poses = pb.pose.p; a.err = pb.err.p; a.npts = pb.n.p; a.valid = pb.ok.p; a.max_iters = 50;
-  const int blocks = (a.nv + PNP_WARPS - 1) / PNP_WARPS;
-  with_model(model, false, [&](auto M, auto) {
-    constexpr int MODEL = decltype(M)::value;
-    k_pnp_views<MODEL><<<blocks, PNP_WARPS * 32, 0, ctx->stream>>>(a);
-  });
-  CKL();
-  return MCBA_OK;
-}
-
-}  // namespace
 
 // Batched board-pose initialisation (pnp_kernels.cuh): one warp per detection list.  Independent of the uploaded problem.
 int mcba_pnp_views(mcba_ctx* ctx, const mcba_problem_desc* desc, const int64_t* det_start, const int32_t* det_ids, const double* det_xy,
@@ -1239,7 +1165,7 @@ int mcba_stereo_init(mcba_ctx* ctx, const mcba_problem_desc* desc, const int64_t
 // Per-view sums of squared pixel errors and corner counts of the packed problem at the current parameters (intrinsics_kernels.cuh)
 int mcba_view_errors(mcba_ctx* ctx, double* sumsq, int64_t* count) {
   if (!ctx || !sumsq || !count) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "mcba_upload has not been called");
+  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
   CK(cudaSetDevice(ctx->device));
   DeviceProblem P = with_state(ctx, false);
   const size_t nv = (size_t)P.C * P.F * P.B;
@@ -1957,6 +1883,7 @@ int mcba_table_select(mcba_ctx* ctx, int which, int64_t* n_corners) {
   if (ctx->table_selected != which) {
     ctx->errors_current = false;
     const uint8_t* m = which == MCBA_TABLE_VALID ? ctx->valid_mask.p : ctx->inlier_mask.p;
+    ctx->table_selected = -1;      // until the packing succeeds
     int r = pack_dense(ctx, &ctx->table_desc, m, true, &n); if (r) return r;
     ctx->table_selected = which;
     if (which == MCBA_TABLE_INLIERS) ctx->n_inliers = n;
@@ -2055,7 +1982,7 @@ int mcba_table_reject(mcba_ctx* ctx, double threshold, int64_t* n_valid, int64_t
 
 int mcba_set_params(mcba_ctx* ctx, const double* cam_rt, const double* board_rt, const double* frame_rt, const double* intrinsics) {
   if (!ctx) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "mcba_upload has not been called");
+  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
   REQUIRE(cam_rt && board_rt && intrinsics && (frame_rt || ctx->P.F == 0 || ctx->P.fb == 0), MCBA_ERR_ARG, "null parameter array");
   const DeviceProblem& P = ctx->P;
   CK(cudaSetDevice(ctx->device));
@@ -2072,7 +1999,7 @@ int mcba_set_params(mcba_ctx* ctx, const double* cam_rt, const double* board_rt,
 // mats: f64[C+B+F][4][4] in the order cameras, boards, frames.
 int mcba_set_state_matrices(mcba_ctx* ctx, const double* mats, const double* intrinsics) {
   if (!ctx) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "mcba_upload has not been called");
+  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
   REQUIRE(mats && intrinsics, MCBA_ERR_ARG, "null parameter array");
   const DeviceProblem& P = ctx->P;
   CK(cudaSetDevice(ctx->device));
@@ -2088,7 +2015,7 @@ int mcba_set_state_matrices(mcba_ctx* ctx, const double* mats, const double* int
 
 int mcba_get_state_matrices(mcba_ctx* ctx, double* mats, double* intrinsics) {
   if (!ctx) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "mcba_upload has not been called");
+  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
   const DeviceProblem& P = ctx->P;
   CK(cudaSetDevice(ctx->device));
   const int np = P.C + P.B + P.F;
@@ -2108,7 +2035,7 @@ int mcba_get_state_matrices(mcba_ctx* ctx, double* mats, double* intrinsics) {
 // f64[F][4][4] and the image heights f64[C] that turn an observed row into the blend weight (rolling_times, 15-19) come here.
 int mcba_set_rolling(mcba_ctx* ctx, const double* end_pose_matrices, const double* image_heights) {
   if (!ctx) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "mcba_upload has not been called");
+  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
   const DeviceProblem& P = ctx->P;
   REQUIRE(P.motion == MOTION_ROLLING, MCBA_ERR_STATE, "the problem was not uploaded with MCBA_MOTION_ROLLING");
   REQUIRE((end_pose_matrices || P.F == 0) && image_heights, MCBA_ERR_ARG, "null parameter array");
@@ -2128,7 +2055,7 @@ int mcba_set_rolling(mcba_ctx* ctx, const double* end_pose_matrices, const doubl
 
 int mcba_get_rolling(mcba_ctx* ctx, double* end_pose_matrices) {
   if (!ctx || !end_pose_matrices) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "mcba_upload has not been called");
+  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
   const DeviceProblem& P = ctx->P;
   REQUIRE(P.motion == MOTION_ROLLING, MCBA_ERR_STATE, "the problem was not uploaded with MCBA_MOTION_ROLLING");
   CK(cudaSetDevice(ctx->device));
@@ -2145,7 +2072,7 @@ int mcba_get_rolling(mcba_ctx* ctx, double* end_pose_matrices) {
 // constants, the two outer transforms are the 12 motion parameters.  The frames of mcba_set_state_matrices are ignored.
 int mcba_set_hand_eye(mcba_ctx* ctx, const double* base_wrt_gripper, const double* world_wrt_base, const double* gripper_wrt_camera) {
   if (!ctx) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "mcba_upload has not been called");
+  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
   const DeviceProblem& P = ctx->P;
   REQUIRE(P.motion == MOTION_HAND_EYE, MCBA_ERR_STATE, "the problem was not uploaded with MCBA_MOTION_HAND_EYE");
   REQUIRE((base_wrt_gripper || P.F == 0) && world_wrt_base && gripper_wrt_camera, MCBA_ERR_ARG, "null parameter array");
@@ -2169,7 +2096,7 @@ int mcba_set_hand_eye(mcba_ctx* ctx, const double* base_wrt_gripper, const doubl
 
 int mcba_get_hand_eye(mcba_ctx* ctx, double* world_wrt_base, double* gripper_wrt_camera) {
   if (!ctx) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "mcba_upload has not been called");
+  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
   const DeviceProblem& P = ctx->P;
   REQUIRE(P.motion == MOTION_HAND_EYE, MCBA_ERR_STATE, "the problem was not uploaded with MCBA_MOTION_HAND_EYE");
   CK(cudaSetDevice(ctx->device));
@@ -2185,7 +2112,7 @@ int mcba_get_hand_eye(mcba_ctx* ctx, double* world_wrt_base, double* gripper_wrt
 // launch takes by value (and so in the key of the solve's cached graph); setup_problem clears it on every upload.
 int mcba_set_fixed_intrinsics(mcba_ctx* ctx, const uint8_t* fixed) {
   if (!ctx) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "mcba_upload has not been called");
+  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
   DeviceProblem& P = ctx->P;
   uint32_t m = 0;
   for (int i = 0; fixed && i < P.kint; i++) {
@@ -2200,7 +2127,7 @@ int mcba_set_fixed_intrinsics(mcba_ctx* ctx, const uint8_t* fixed) {
 
 int mcba_get_params(mcba_ctx* ctx, double* cam_rt, double* board_rt, double* frame_rt, double* intrinsics) {
   if (!ctx) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "mcba_upload has not been called");
+  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
   const DeviceProblem& P = ctx->P;
   CK(cudaSetDevice(ctx->device));
   if (cam_rt) CK(cudaMemcpyAsync(cam_rt, P.cam_rt, sizeof(double) * P.C * 6, cudaMemcpyDeviceToHost, ctx->stream));
@@ -2213,7 +2140,7 @@ int mcba_get_params(mcba_ctx* ctx, double* cam_rt, double* board_rt, double* fra
 
 int mcba_num_params(mcba_ctx* ctx, int64_t* n) {
   if (!ctx || !n) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "mcba_upload has not been called");
+  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
   *n = ctx->P.n;
   return MCBA_OK;
 }
@@ -2240,14 +2167,14 @@ static int write_x_canonical(mcba_ctx* ctx, const double* x, double* dev_x) {
 
 int mcba_get_param_vec(mcba_ctx* ctx, double* x) {
   if (!ctx || !x) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "mcba_upload has not been called");
+  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
   CK(cudaSetDevice(ctx->device));
   return read_x_canonical(ctx, x);
 }
 
 int mcba_set_param_vec(mcba_ctx* ctx, const double* x) {
   if (!ctx || !x) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "mcba_upload has not been called");
+  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
   CK(cudaSetDevice(ctx->device));
   ctx->errors_current = false;
   int r = write_x_canonical(ctx, x, ctx->x.p); if (r) return r;
@@ -2258,7 +2185,7 @@ int mcba_set_param_vec(mcba_ctx* ctx, const double* x) {
 
 int mcba_residuals(mcba_ctx* ctx, const double* x, double* r_out, double* cost) {
   if (!ctx) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "mcba_upload has not been called");
+  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
   CK(cudaSetDevice(ctx->device));
   bool trial = false;
   if (x) {
@@ -2287,7 +2214,7 @@ int mcba_residuals(mcba_ctx* ctx, const double* x, double* r_out, double* cost) 
 
 int mcba_reprojection_error(mcba_ctx* ctx, double* err) {
   if (!ctx || !err) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "mcba_upload has not been called");
+  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
   CK(cudaSetDevice(ctx->device));
   DeviceProblem P = with_state(ctx, false);
   if (P.N == 0) return MCBA_OK;
@@ -2302,7 +2229,7 @@ int mcba_reprojection_error(mcba_ctx* ctx, double* err) {
 
 int mcba_linearize(mcba_ctx* ctx, const double* x, double* JtJ, double* Jtr, double* cost) {
   if (!ctx) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "mcba_upload has not been called");
+  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
   CK(cudaSetDevice(ctx->device));
   const DeviceProblem& P = ctx->P;
   if (x) { int r = mcba_set_param_vec(ctx, x); if (r) return r; }
@@ -2338,7 +2265,7 @@ int mcba_linearize(mcba_ctx* ctx, const double* x, double* JtJ, double* Jtr, dou
 
 int mcba_solve(mcba_ctx* ctx, const mcba_solve_opts* opts, mcba_solve_result* result, mcba_log_row* log, int32_t log_capacity) {
   if (!ctx || !opts || !result) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "mcba_upload has not been called");
+  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
   REQUIRE(opts->loss >= 0 && opts->loss <= 4, MCBA_ERR_ARG, "unknown loss");
   REQUIRE(opts->max_nfev > 0, MCBA_ERR_ARG, "max_nfev must be positive");
   REQUIRE(opts->f_scale > 0, MCBA_ERR_ARG, "f_scale must be positive");
@@ -2412,7 +2339,7 @@ int mcba_solve(mcba_ctx* ctx, const mcba_solve_opts* opts, mcba_solve_result* re
 
 int mcba_bench_info(mcba_ctx* ctx, int which, int64_t* corners, int64_t* bytes, int32_t* launches) {
   if (!ctx) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "mcba_upload has not been called");
+  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
   const DeviceProblem& P = ctx->P;
   int64_t per_corner = 18, per_view = 16, l = 1;
   if (which == MCBA_BENCH_RESIDUAL) per_corner = 18 + 4 + 16;
@@ -2424,7 +2351,7 @@ int mcba_bench_info(mcba_ctx* ctx, int which, int64_t* corners, int64_t* bytes, 
 
 int mcba_bench_launch(mcba_ctx* ctx, int which, int repeats) {
   if (!ctx) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "mcba_upload has not been called");
+  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
   CK(cudaSetDevice(ctx->device));
   DeviceProblem P = with_state(ctx, false);
   int r;

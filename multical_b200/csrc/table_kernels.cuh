@@ -30,17 +30,6 @@ __global__ void k_table_fill(const int64_t* det_start, const int32_t* det_ids, c
   }
 }
 
-// monotone check of the list offsets (a bad CSR would send k_table_fill out of bounds)
-__global__ void k_table_check_offsets(const int64_t* det_start, int nv, int64_t total, int* bad) {
-  const int w = blockIdx.x * blockDim.x + threadIdx.x;
-  if (w > nv) return;
-  const int64_t a = det_start[w];
-  if (a < 0 || a > total) atomicExch(bad, 1);
-  if (w < nv && det_start[w + 1] < a) atomicExch(bad, 1);
-  if (w == 0 && a != 0) atomicExch(bad, 1);
-  if (w == nv && a != total) atomicExch(bad, 1);
-}
-
 __global__ void k_mask_and(const uint8_t* a, const uint8_t* b, size_t n, uint8_t* out) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) out[i] = (a[i] && b[i]) ? 1 : 0;

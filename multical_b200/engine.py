@@ -78,59 +78,32 @@ class Engine:
     self._ck(self.lib.mcba_peer_import(self.h, blob))
 
   # ---- problem ----------------------------------------------------------------------------------
-  def upload(self, model, optimize_bits, dims, idx, obs, board_points):
-    Cn, F, B, P = (int(v) for v in dims)
-    idx = np.ascontiguousarray(idx, dtype=np.int32).reshape(-1, 4)
-    cols = [np.ascontiguousarray(idx[:, j]) for j in range(4)]
-    obs = nat.f64(obs).reshape(-1, 2)
-    bp = nat.f64(board_points).reshape(B, P, 3)
-    d = nat.ProblemDesc(Cn, F, B, P, nat.MODEL_IDS[model], int(optimize_bits), idx.shape[0])
-    self._ck(self.lib.mcba_upload(self.h, C.byref(d), nat.iptr(cols[0]), nat.iptr(cols[1]), nat.iptr(cols[2]),
-                                  nat.iptr(cols[3]), nat.dptr(obs), nat.dptr(bp)))
-    self.desc = d
-    self.model = model
-    self.kint = 5 + nat.DIST_SIZES[model]
-    self.N = idx.shape[0]
-
   def upload_dense(self, model, optimize_bits, mask, points, board_points, view_valid=None):
     """Dense [C,F,B,P] mask + [C,F,B,P,2] observations as the reference holds them (point_table, inliers);
     the packing into frame-major corner arrays happens on the device (csrc/pack_kernels.cuh).  With `view_valid` ([C,F,B]) the
     selection is mask & view_valid[..., None], the conjunction taken on the device (calibration.py:73-81 without the host pass)."""
-    mask = np.ascontiguousarray(mask)
-    Cn, F, B, P = mask.shape
     u8 = lambda a: a.view(np.uint8) if a.dtype == np.bool_ else np.ascontiguousarray(a, dtype=np.uint8)
-    m8 = u8(mask)
+    u8p = lambda a: None if a is None else a.ctypes.data_as(C.POINTER(C.c_uint8))
+    m8 = u8(np.ascontiguousarray(mask))
+    Cn, F, B, P = m8.shape
     # a float32 table (what make_point_table yields for cv2's float32 corners, tables.py:15-17) goes over as it is; anything else as f64
     f32 = np.asarray(points).dtype == np.float32
     pts = np.ascontiguousarray(points) if f32 else nat.f64(points)
-    assert pts.shape == (Cn, F, B, P, 2), f"points {pts.shape} do not match mask {mask.shape}"
+    assert pts.shape == (Cn, F, B, P, 2), f"points {pts.shape} do not match mask {m8.shape}"
+    v8 = None if view_valid is None else u8(np.ascontiguousarray(view_valid))
+    assert v8 is None or v8.shape == (Cn, F, B), f"view_valid {v8.shape} does not match mask {m8.shape}"
     bp = nat.f64(board_points).reshape(B, P, 3)
     d = nat.ProblemDesc(Cn, F, B, P, nat.MODEL_IDS[model], int(optimize_bits), 0)
     n = C.c_int64()
-    if f32:
-      v8 = None if view_valid is None else u8(np.ascontiguousarray(view_valid))
-      self._ck(self.lib.mcba_upload_dense_views_f32(self.h, C.byref(d), m8.ctypes.data_as(C.POINTER(C.c_uint8)),
-                                                    None if v8 is None else v8.ctypes.data_as(C.POINTER(C.c_uint8)),
-                                                    pts.ctypes.data_as(C.POINTER(C.c_float)), nat.dptr(bp), C.byref(n)))
-    elif view_valid is None:
-      self._ck(self.lib.mcba_upload_dense(self.h, C.byref(d), m8.ctypes.data_as(C.POINTER(C.c_uint8)), nat.dptr(pts),
-                                          nat.dptr(bp), C.byref(n)))
-    else:
-      v8 = u8(np.ascontiguousarray(view_valid))
-      assert v8.shape == (Cn, F, B), f"view_valid {v8.shape} does not match mask {mask.shape}"
-      self._ck(self.lib.mcba_upload_dense_views(self.h, C.byref(d), m8.ctypes.data_as(C.POINTER(C.c_uint8)),
-                                                v8.ctypes.data_as(C.POINTER(C.c_uint8)), nat.dptr(pts), nat.dptr(bp), C.byref(n)))
-    d.N = n.value
-    self.desc = d
-    self.model = model
-    self.kint = 5 + nat.DIST_SIZES[model]
-    self.N = n.value
+    self._ck(self.lib.mcba_upload_dense(self.h, C.byref(d), u8p(m8), u8p(v8), pts.ctypes.data_as(C.c_void_p),
+                                        nat.POINTS_F32 if f32 else nat.POINTS_F64, nat.dptr(bp), C.byref(n)))
+    self._uploaded(d, model, n.value)
 
-  # ---- resident point table (include/mcba.h "resident point table") ------------------------------
-  def _table_ready(self, d, model, n):
+  def _uploaded(self, d, model, n):
     d.N = n
     self.desc, self.model, self.kint, self.N = d, model, 5 + nat.DIST_SIZES[model], n
 
+  # ---- resident point table (include/mcba.h "resident point table") ------------------------------
   def table_upload(self, model, optimize_bits, valid, points, board_points):
     """Keep the whole [C,F,B,P] table on the device: `valid` mask + observations.  Inliers start equal to `valid`,
     which is also the packed selection; returns the number of valid corners."""
@@ -144,7 +117,7 @@ class Engine:
     n = C.c_int64()
     self._ck(self.lib.mcba_table_upload(self.h, C.byref(d), v8.ctypes.data_as(C.POINTER(C.c_uint8)), nat.dptr(pts),
                                         nat.dptr(bp), C.byref(n)))
-    self._table_ready(d, model, n.value)
+    self._uploaded(d, model, n.value)
     return n.value
 
   @staticmethod
@@ -167,7 +140,7 @@ class Engine:
     n = C.c_int64()
     self._ck(self.lib.mcba_table_from_detections(self.h, C.byref(d), det_start.ctypes.data_as(C.POINTER(C.c_int64)),
                                                  nat.iptr(det_ids), nat.dptr(det_xy), nat.dptr(bp), C.byref(n)))
-    self._table_ready(d, model, n.value)
+    self._uploaded(d, model, n.value)
     return n.value
 
   def pnp_views(self, model, dims, det_start, det_ids, det_xy, board_points, intrinsics, board_grid):

@@ -157,11 +157,13 @@ def _solve_camera(eng, model, fix_aspect, views, k0, poses, board_points, solve_
   """One calibrateCameraExtended: the views as frames of a one-camera problem, started from K0 and the PnP poses."""
   nv = len(views)
   B, P = board_points.shape[:2]
-  rows = np.concatenate([np.stack([np.zeros(v.ids.size, np.int32), np.full(v.ids.size, i, np.int32), np.full(v.ids.size, v.board, np.int32),
-                                   v.ids.astype(np.int32)], axis=1) for i, v in enumerate(views)])
-  obs = np.concatenate([v.corners.astype(np.float64) for v in views])
+  counts = np.zeros(nv * B, np.int64)                 # list i*B + v.board holds view i, every other list is empty
+  for i, v in enumerate(views): counts[i * B + v.board] = v.ids.size
+  det_start = np.concatenate([[0], np.cumsum(counts)])
+  det_ids = np.concatenate([v.ids for v in views])
+  det_xy = np.concatenate([v.corners.astype(np.float64) for v in views])
   bits = nat.OPT_BITS["motion"] | nat.OPT_BITS["cameras"] | (nat.OPT_FIX_ASPECT if fix_aspect else 0)
-  eng.upload(model, bits, (1, nv, B, P), rows, obs, board_points)
+  eng.table_from_detections(model, bits, (1, nv, B, P), det_start, det_ids, det_xy, board_points)
   mats = np.concatenate([np.eye(4)[None], np.tile(np.eye(4), (B, 1, 1)), poses])
   eng.set_state_matrices(mats, k0[None])          # K0: zero distortion, and the principal point OpenCV holds fixed
   if fixed is not None: eng.set_fixed_intrinsics(fixed)

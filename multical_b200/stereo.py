@@ -76,14 +76,10 @@ def solve_pair(model, intrinsics, problem, fix_intrinsic=True, fix_aspect=False,
   rt0, left, ok = stereo_init(model, intrinsics, problem, eng)
   if not ok.all():
     raise ValueError(f"view {int(np.flatnonzero(~ok)[0])}: the initial pose of the left or the right camera failed")
-  lens = np.diff(det_start)
-  cam = np.repeat(np.repeat([0, 1], F), lens).astype(np.int32)
-  frame = np.repeat(np.tile(np.arange(F), 2), lens).astype(np.int32)
-  rows = np.stack([cam, frame, np.zeros_like(cam), det_ids], axis=1)
   bits = nat.OPT_BITS["camera_poses"] | nat.OPT_BITS["motion"]
   if not fix_intrinsic:
     bits |= nat.OPT_BITS["cameras"] | (nat.OPT_FIX_ASPECT if fix_aspect else 0)
-  eng.upload(model, bits, (2, F, 1, len(board)), rows, det_xy, board[None])
+  eng.table_from_detections(model, bits, (2, F, 1, len(board)), det_start, det_ids, det_xy, board[None])
   mats = np.concatenate([np.eye(4)[None], to_matrix(rt0)[None], np.eye(4)[None], left])
   eng.set_state_matrices(mats, intrinsics)
   info = eng.solve(**opts)

@@ -35,7 +35,7 @@ class FakeEngine(Engine):
     self.calls.append("upload_dense")
     self.table = None
     mask = np.asarray(mask)
-    if view_valid is not None: mask = mask & np.asarray(view_valid)[..., None]      # the conjunction the device takes (mcba_upload_dense_views)
+    if view_valid is not None: mask = mask & np.asarray(view_valid)[..., None]      # the conjunction the device takes (mcba_upload_dense with view_valid)
     self._set_problem(model, optimize_bits, mask, points, board_points)
 
   def set_state_matrices(self, pose_matrices, intrinsics):

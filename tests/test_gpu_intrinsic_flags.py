@@ -243,8 +243,8 @@ def run_mask_arguments():
   with pytest.raises(AssertionError, match="expected 10 entries"):
     eng.set_fixed_intrinsics(np.zeros(9, bool))
   from multical_b200 import _native as nat
-  eng.upload("standard", nat.OPT_BITS["cameras"] | nat.OPT_FIX_ASPECT, (1, 1, 1, 1), np.zeros((1, 4), np.int32), np.zeros((1, 2)),
-             np.zeros((1, 1, 3)))
+  eng.upload_dense("standard", nat.OPT_BITS["cameras"] | nat.OPT_FIX_ASPECT, np.ones((1, 1, 1, 1), bool), np.zeros((1, 1, 1, 1, 2)),
+                   np.zeros((1, 1, 3)))
   with pytest.raises(AssertionError, match="fy follows fx"):
     eng.set_fixed_intrinsics(np.array([0, 1] + [0] * 8, bool))
   eng.set_fixed_intrinsics(np.array([1, 1] + [0] * 8, bool))

@@ -106,15 +106,16 @@ def run_acceptance_scan(model, motion, C):
   limit = board_limit(model, roll, C)
   eng = get_engine()
   bits = OPT_BITS["cameras"] | (MOTION_ROLLING if roll else 0)
-  obs = np.tile([[960.0, 540.0]], (C, 1))
   for B in range(1, limit + 2):
-    idx = np.array([[c, 0, B - 1, 0] for c in range(C)])
+    mask = np.zeros((C, 1, B, 1), bool); mask[:, 0, B - 1, 0] = True
+    pts = np.tile([960.0, 540.0], (C, 1, B, 1, 1))
     bp = np.zeros((B, 1, 3))
     if B <= limit:
-      eng.upload(model, bits, (C, 1, B, 1), idx, obs, bp)
+      eng.upload_dense(model, bits, mask, pts, bp)
+      assert eng.N == C
     else:
       with pytest.raises(NotImplementedError, match="too many boards"):
-        eng.upload(model, bits, (C, 1, B, 1), idx, obs, bp)
+        eng.upload_dense(model, bits, mask, pts, bp)
   return limit
 
 

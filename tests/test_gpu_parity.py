@@ -296,37 +296,29 @@ def test_large_scene_properties(workload):
 
 
 @pytest.mark.parametrize("name", ["standard_2x6", "cube3_3x6", "invalid_poses_3x6"])
-def test_device_packing_equals_host_packing(name):
-  """mcba_upload_dense (mask + dense table, packed on the GPU) and mcba_upload (np.argwhere rows packed on the host)
-  must give the same corner order, residuals and normal equations."""
-  from multical_b200.calibration import get_engine
-  from multical_b200.engine import pack_corners
+def test_dense_uploads_pack_the_same_corners(name):
+  """Every dense upload packs the same corners in the same order: the inlier mask, the two-part mask (detections + view validity)
+  and a float32 table give the residuals of the float64 upload (the order itself is pinned to np.argwhere by
+  test_residuals_match_reference_golden_and_oracle)."""
   scene, z, calib, prob = make(name)
-  eng = calib._upload(calib.inliers)                 # dense path
+  eng = calib._upload(calib.inliers)
+  n = int(calib.inliers.sum())
+  assert eng.N == n
   r_dense = eng.residuals(z["x1"]).copy()
-  H_dense, g_dense, _ = eng.linearize(z["x1"])
-  idx, obs = pack_corners(calib.inliers, np.asarray(calib.point_table.points))
-  s = calib.size
-  eng.upload(calib.engine_model, calib._optimize_bits(), (s.cameras, s.rig_poses, s.boards, s.points), idx, obs, calib.board_points.points)
-  eng.set_params(*calib._state_arrays())
-  assert eng.N == idx.shape[0]
-  assert np.array_equal(eng.residuals(z["x1"]), r_dense)
-  H, g, _ = eng.linearize(z["x1"])
-  assert np.allclose(H, H_dense, rtol=1e-12, atol=0) and np.allclose(g, g_dense, rtol=1e-10, atol=1e-9)
   # the two-part mask (detections as they are + pose validity per view, conjunction on the device: what bundle_adjust uploads)
   fresh = from_scene(scene).enable(cameras=True)
   assert "valid" not in fresh.__dict__
   eng = fresh._upload_inliers()
-  assert "valid" not in fresh.__dict__ and eng.N == idx.shape[0]
+  assert "valid" not in fresh.__dict__ and eng.N == n
   assert np.array_equal(eng.residuals(z["x1"]), r_dense)
   # a float32 table (the dtype make_point_table keeps for cv2's corners) goes over as float32 and must be the float64 table of the same values
   pts32 = np.asarray(calib.point_table.points).astype(np.float32)
   eng = calib._upload(calib.inliers, points=pts32.astype(np.float64))
   r_64 = eng.residuals(z["x1"]).copy()
   eng = calib._upload(calib.inliers, points=pts32)
-  assert eng.N == idx.shape[0] and np.array_equal(eng.residuals(z["x1"]), r_64)
+  assert eng.N == n and np.array_equal(eng.residuals(z["x1"]), r_64)
   eng = calib._upload(np.asarray(calib.point_table.valid), points=pts32, view_valid=calib.pose_valid)
-  assert eng.N == idx.shape[0] and np.array_equal(eng.residuals(z["x1"]), r_64)
+  assert eng.N == n and np.array_equal(eng.residuals(z["x1"]), r_64)
 
 
 def test_empty_and_ragged_inputs():

@@ -120,6 +120,40 @@ def test_table_from_detections_is_make_point_table():
       eng.table_from_detections(calib.engine_model, calib._optimize_bits(), valid_pts.shape, bad_start, ids, xy, calib.board_points.points)
 
 
+@pytest.mark.parametrize("refusal", ["too many boards", "detection id outside"])
+def test_a_refused_upload_leaves_no_problem(refusal):
+  """An upload replaces the problem even when it is refused: one refused inside setup_problem (too many boards for k_linearize's
+  shared memory) or for its detection lists leaves none, so the next residuals refuse instead of running on the previous problem."""
+  scene, calib = scene_and_calib(seed=65)
+  eng = calib._upload(calib.valid)
+  eng.residuals()
+  if refusal == "too many boards":      # 2 cameras: 63 boards at most (tests/test_gpu_linearize_shapes.py BOARD_LIMITS)
+    mask = np.zeros((2, 1, 64, 1), bool); mask[:, 0, -1, 0] = True
+    with pytest.raises(NotImplementedError, match=refusal):
+      eng.upload_dense("standard", calib._optimize_bits(), mask, np.zeros((2, 1, 64, 1, 2)), np.zeros((64, 1, 3)))
+  else:
+    valid_pts = np.asarray(calib.point_table.valid)
+    start, ids, xy = detection_lists(valid_pts, np.asarray(calib.point_table.points))
+    ids[0] = valid_pts.shape[3]
+    with pytest.raises(AssertionError, match=refusal):
+      eng.table_from_detections(calib.engine_model, calib._optimize_bits(), valid_pts.shape, start, ids, xy, calib.board_points.points)
+  with pytest.raises(_native.NativeError, match="no problem uploaded"):
+    eng.residuals()
+  calib._upload(calib.valid).residuals()
+
+
+def test_a_repeated_detection_id_is_refused():
+  """A dense table holds one corner per (view, point id): a detection list that repeats an id is refused."""
+  scene, calib = scene_and_calib(seed=66)
+  valid_pts = np.asarray(calib.point_table.valid)
+  start, ids, xy = detection_lists(valid_pts, np.asarray(calib.point_table.points))
+  w = int(np.flatnonzero(np.diff(start) >= 2)[0])
+  ids[start[w] + 1] = ids[start[w]]
+  with pytest.raises(AssertionError, match="repeats point id"):
+    get_engine().table_from_detections(calib.engine_model, calib._optimize_bits(), valid_pts.shape, start, ids, xy,
+                                       calib.board_points.points)
+
+
 def test_table_state_machine_refuses_stale_errors():
   scene, calib = scene_and_calib(seed=64)
   eng = calib._upload(calib.valid)                                       # packed upload: no resident table

@@ -54,7 +54,7 @@ def test_robust_losses_follow_scipy(loss):
 test_outlier_loop_matches_reference_semantics = gp.test_outlier_loop_matches_reference_semantics
 test_fixed_blocks_and_fix_aspect = gp.test_fixed_blocks_and_fix_aspect
 test_bad_inputs_raise_like_the_reference = gp.test_bad_inputs_raise_like_the_reference
-test_device_packing_equals_host_packing = gp.test_device_packing_equals_host_packing
+test_dense_uploads_pack_the_same_corners = gp.test_dense_uploads_pack_the_same_corners
 test_empty_and_ragged_inputs = gp.test_empty_and_ragged_inputs
 test_board_points_as_parameters = gp.test_board_points_as_parameters
 test_iteration_table_matches_the_trf_model = gp.test_iteration_table_matches_the_trf_model
@@ -134,6 +134,8 @@ test_table_errors_ranks_and_reject_are_numpy_on_the_same_errors = gt.test_table_
 test_resident_adjust_outliers_equals_host_loop = gt.test_resident_adjust_outliers_equals_host_loop
 test_table_from_detections_is_make_point_table = gt.test_table_from_detections_is_make_point_table
 test_table_state_machine_refuses_stale_errors = gt.test_table_state_machine_refuses_stale_errors
+test_a_refused_upload_leaves_no_problem = gt.test_a_refused_upload_leaves_no_problem
+test_a_repeated_detection_id_is_refused = gt.test_a_repeated_detection_id_is_refused
 test_outlier_steps_match_reference_golden = gt.test_outlier_steps_match_reference_golden
 test_workspace_calibrate_is_enable_plus_the_outlier_loop = gt.test_workspace_calibrate_is_enable_plus_the_outlier_loop
 
