@@ -363,11 +363,12 @@ __device__ __forceinline__ void syrk_tile(const LmArgs& a, int ti, int tj, int c
 }
 
 // ---- blocked right-looking Cholesky for n_s > CHOL_SMALL_MAX, NB = 32 panels, the grid cooperating between barriers.
-// The diagonal block by ONE warp: lane i keeps row i in registers, a column is one shuffle of the pivot, one rsqrt and a
-// shuffle per trailing column -- no block barrier on the column path (scripts/chol_bench.cu times it against the
-// 256-thread version, whose column costs two __syncthreads).  The inverse of the factor follows in the same warp, lane j solving
-// for column j with four independent partial sums per row.
+// The diagonal block by ONE warp: lane i keeps row i in registers, a column is one shuffle of the pivot, one rsqrt and one broadcast
+// of the column through shared memory -- no block barrier on the column path (scripts/chol_bench.cu times it against the 256-thread
+// version, whose column costs two __syncthreads).  The inverse of the factor is formed in the same pass, lane j holding column j.
+// sh: 2 x 32 x 33 + 32 x 64 doubles.
 __device__ __noinline__ void chol_diag_warp_body(int n, int kb, double* S, double* Linv_all, int* chol_fail, double* sh) {
+  static_assert(2 * CHOL_NB * (CHOL_NB + 1) + 64 * CHOL_NB <= 5 * CHOL_NB * (CHOL_NB + 1), "within the shared memory of chol_fused_tile");
   double (*Lm)[CHOL_NB + 1] = reinterpret_cast<double (*)[CHOL_NB + 1]>(sh);
   double (*Liv)[CHOL_NB + 1] = reinterpret_cast<double (*)[CHOL_NB + 1]>(sh + CHOL_NB * (CHOL_NB + 1));
   const int nb = min(CHOL_NB, n - kb);
@@ -387,40 +388,45 @@ __device__ __noinline__ void chol_diag_warp_body(int n, int kb, double* S, doubl
   }
   __syncthreads();
   if (tid < 32) {
+    // Column k is one trip of a loop that is NOT unrolled: the body stays in the instruction cache (the fully unrolled factor and
+    // inverse were 5.5 k straight-line instructions, fetched afresh for every panel and from HBM for the first one of an iteration).
+    // The register rows are kept ROTATED so that every index in the body is static: at column k, lane i holds a[m] = A[i][k + m]
+    // and b[m] = B[k + m][i] of L B = I (B = L^-1, lane i = column i), right-looking.  Column k of L goes to shared memory once,
+    // shifted so that col[32 + m] = L[k + m][k] (zero past the last row), and both updates read it there as 16 broadcast pairs.
+    // The next pivot does not wait for that update: lane k + 1 updates its own diagonal entry first (the same operation as in the
+    // update), so the pivot's shuffle and reciprocal square root of column k + 1 are issued ahead of column k's 62 updates.
     const int lane = tid;
-    double a[CHOL_NB], rsd[CHOL_NB];
+    double* colk = sh + 2 * CHOL_NB * (CHOL_NB + 1);    // [CHOL_NB][64], 16-byte aligned rows
+    double a[CHOL_NB], b[CHOL_NB];
 #pragma unroll
-    for (int j = 0; j < CHOL_NB; j++) a[j] = j <= lane ? Lm[lane][j] : 0.0;
-#pragma unroll
+    for (int m = 0; m < CHOL_NB; m++) { a[m] = m <= lane ? Lm[lane][m] : 0.0; b[m] = m == lane ? 1.0 : 0.0; }
+    __syncwarp();
+    const double a00 = __shfl_sync(0xffffffffu, a[0], 0);
+    if (lane == 0 && !(a00 > 0.0)) *chol_fail += 1;
+    double rs = fast_rsqrt(fmin(fmax(a00, 1e-30), 1e30));
+#pragma unroll 1
     for (int k = 0; k < CHOL_NB; k++) {
-      const double akk = __shfl_sync(0xffffffffu, a[k], k);
-      if (lane == 0 && k < nb && !(akk > 0.0)) *chol_fail += 1;
-      const double rs = fast_rsqrt(fmin(fmax(akk, 1e-30), 1e30));
-      rsd[k] = rs;
-      const double l = lane >= k ? a[k] * rs : 0.0;
-      a[k] = l;
+      const double l = lane >= k ? a[0] * rs : 0.0;
+      const double akn = __shfl_sync(0xffffffffu, a[1] - l * l, (k + 1) & (CHOL_NB - 1));
+      if (lane == 0 && k + 1 < nb && !(akn > 0.0)) *chol_fail += 1;
+      const double rsn = fast_rsqrt(fmin(fmax(akn, 1e-30), 1e30));
+      double* col = colk + 64 * k;
+      col[32 + lane - k] = l;
+      if (lane < k) col[64 + lane - k] = 0.0;
+      Lm[lane][k] = l;
+      const double x = b[0] * rs;                       // X[k][lane]
+      Liv[k][lane] = x;
+      __syncwarp();
+      const double2* c2 = reinterpret_cast<const double2*>(col + 32);
 #pragma unroll
-      for (int j = k + 1; j < CHOL_NB; j++) { const double ljk = __shfl_sync(0xffffffffu, l, j); a[j] -= l * ljk; }
-    }
-    __syncwarp();
-#pragma unroll
-    for (int j = 0; j < CHOL_NB; j++) Lm[lane][j] = j <= lane ? a[j] : 0.0;
-    __syncwarp();
-    double z[CHOL_NB];
-#pragma unroll
-    for (int i = 0; i < CHOL_NB; i++) {
-      double t0 = (i == lane) ? 1.0 : 0.0, t1 = 0.0, t2 = 0.0, t3 = 0.0;
-#pragma unroll
-      for (int m = 0; m < CHOL_NB; m += 4) {
-        if (m < i) t0 -= Lm[i][m] * z[m];
-        if (m + 1 < i) t1 -= Lm[i][m + 1] * z[m + 1];
-        if (m + 2 < i) t2 -= Lm[i][m + 2] * z[m + 2];
-        if (m + 3 < i) t3 -= Lm[i][m + 3] * z[m + 3];
+      for (int m2 = 0; m2 < CHOL_NB / 2; m2++) {
+        const double2 c = c2[m2];
+        if (m2 > 0) { a[2 * m2 - 1] = a[2 * m2] - l * c.x; b[2 * m2 - 1] = b[2 * m2] - c.x * x; }
+        a[2 * m2] = a[2 * m2 + 1] - l * c.y; b[2 * m2] = b[2 * m2 + 1] - c.y * x;
       }
-      z[i] = (i >= lane) ? ((t0 + t1) + (t2 + t3)) * rsd[i] : 0.0;
+      a[CHOL_NB - 1] = 0.0; b[CHOL_NB - 1] = 0.0;
+      rs = rsn;
     }
-#pragma unroll
-    for (int i = 0; i < CHOL_NB; i++) Liv[i][lane] = z[i];
   }
   __syncthreads();
   double* Li = Linv_all + (size_t)(kb / CHOL_NB) * CHOL_NB * CHOL_NB;
