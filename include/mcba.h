@@ -149,6 +149,19 @@ int  mcba_get_hand_eye(mcba_ctx* ctx, double* world_wrt_base, double* gripper_wr
  * Entries other than 0 / 1, or fx and fy fixed apart under MCBA_OPT_FIX_ASPECT (fy follows fx), fail with MCBA_ERR_ARG.  Every upload
  * clears the mask. */
 int  mcba_set_fixed_intrinsics(mcba_ctx* ctx, const uint8_t* fixed);
+/* the trust-region step of mcba_solve (scipy least_squares' tr_solver):
+ *   MCBA_TR_SUBSPACE  the exact Gauss-Newton direction, then the step in the 2-D subspace span{g, gn} (the default);
+ *   MCBA_TR_EXACT     the full trust-region subproblem, tr_solver='exact': the Gauss-Newton step if A = D J^T J D is nonsingular and it
+ *                     lies inside the radius, else Newton iterations on the Levenberg-Marquardt parameter alpha (at most 10, each a
+ *                     factorisation of A + alpha I) until ||p(alpha)|| is within 1% of the radius.  Slower per iteration; reaches the
+ *                     minimum of long curved valleys where the subspace step stops on xtol above it (the rational intrinsics).
+ * Other values fail with MCBA_ERR_ARG.  A solve on several ranks in MCBA_TR_EXACT fails with MCBA_ERR_UNSUPPORTED.  Every upload resets
+ * the mode to MCBA_TR_SUBSPACE. */
+enum { MCBA_TR_SUBSPACE = 0, MCBA_TR_EXACT = 1 };
+int  mcba_set_trust_region(mcba_ctx* ctx, int32_t mode);
+/* alpha iterations of the last mcba_solve summed over its trial steps (scipy's n_iter of solve_lsq_trust_region: 0 for a Gauss-Newton
+ * step); 0 after a MCBA_TR_SUBSPACE solve */
+int  mcba_last_alpha_iterations(mcba_ctx* ctx, int32_t* total);
 int  mcba_num_params(mcba_ctx* ctx, int64_t* n);      /* length of param_vec for the enabled blocks    */
 int  mcba_get_param_vec(mcba_ctx* ctx, double* x);    /* Parameters.param_vec (parameters.py:44-46)    */
 int  mcba_set_param_vec(mcba_ctx* ctx, const double* x);   /* with_param_vec (parameters.py:48-50)     */

@@ -25,6 +25,7 @@ STATUS_MESSAGES = {
 EXPORTS = ["mcba_create", "mcba_destroy", "mcba_last_error", "mcba_set_stream", "mcba_version",
            "mcba_comm_unique_id", "mcba_comm_init", "mcba_peer_export", "mcba_peer_import", "mcba_upload_dense", "mcba_set_params", "mcba_get_params", "mcba_set_state_matrices", "mcba_get_state_matrices",
            "mcba_set_rolling", "mcba_get_rolling", "mcba_set_hand_eye", "mcba_get_hand_eye", "mcba_set_fixed_intrinsics",
+           "mcba_set_trust_region", "mcba_last_alpha_iterations",
            "mcba_num_params", "mcba_get_param_vec", "mcba_set_param_vec", "mcba_residuals",
            "mcba_linearize", "mcba_reprojection_error", "mcba_solve", "mcba_bench_launch", "mcba_bench_info",
            "mcba_table_upload", "mcba_table_from_detections", "mcba_table_download", "mcba_table_set_inliers",
@@ -36,6 +37,7 @@ EXPORTS = ["mcba_create", "mcba_destroy", "mcba_last_error", "mcba_set_stream", 
 IMAGE_UINT8 = 0          # include/mcba.h MCBA_IMAGE_UINT8
 POINTS_F64, POINTS_F32 = 0, 1          # include/mcba.h MCBA_POINTS_*
 TABLE_VALID, TABLE_INLIERS = 0, 1
+TR_SOLVERS = {"lsmr": 0, "exact": 1}    # include/mcba.h MCBA_TR_SUBSPACE / MCBA_TR_EXACT, named after scipy's tr_solver
 
 
 class ProblemDesc(C.Structure):
@@ -103,6 +105,8 @@ def load():
   lib.mcba_set_hand_eye.argtypes = [P, D, D, D]
   lib.mcba_get_hand_eye.argtypes = [P, D, D]
   lib.mcba_set_fixed_intrinsics.argtypes = [P, C.POINTER(C.c_uint8)]
+  lib.mcba_set_trust_region.argtypes = [P, C.c_int32]
+  lib.mcba_last_alpha_iterations.argtypes = [P, I32]
   lib.mcba_num_params.argtypes = [P, C.POINTER(C.c_int64)]
   lib.mcba_get_param_vec.argtypes = [P, D]
   lib.mcba_set_param_vec.argtypes = [P, D]

@@ -333,18 +333,21 @@ class Calibration(Parameters):
     return S
 
   # ---- the hot path -----------------------------------------------------------------------------
-  def bundle_adjust(self, tolerance=1e-4, f_scale=1.0, max_iterations=100, loss="linear", xtol=1e-8, gtol=1e-8):
+  def bundle_adjust(self, tolerance=1e-4, f_scale=1.0, max_iterations=100, loss="linear", xtol=1e-8, gtol=1e-8, tr_solver="lsmr"):
     """Non-linear least squares on point reprojection error (calibration.py:199-212), solved on the GPU
-    with scipy-TRF semantics: ftol=tolerance, max_nfev=max_iterations, x_scale='jac', robust `loss`."""
+    with scipy-TRF semantics: ftol=tolerance, max_nfev=max_iterations, x_scale='jac', robust `loss`.  tr_solver="exact" solves the
+    full trust-region subproblem (scipy's tr_solver='exact') instead of the 2-D subspace step of the default "lsmr" (Engine.solve)."""
     eng = self._upload_inliers()
-    res = self._solve_logged(eng, tolerance, f_scale, max_iterations, loss, xtol, gtol)
+    res = self._solve_logged(eng, tolerance, f_scale, max_iterations, loss, xtol, gtol, tr_solver)
     out = self._with_engine_state(eng)
     out.__dict__["last_solve"] = res
     return out
 
   @staticmethod
-  def _solve_logged(eng, tolerance=1e-4, f_scale=1.0, max_iterations=100, loss="linear", xtol=1e-8, gtol=1e-8):
-    res = eng.solve(ftol=tolerance, xtol=xtol, gtol=gtol, f_scale=f_scale, max_nfev=max_iterations, loss=loss)
+  def _solve_logged(eng, tolerance=1e-4, f_scale=1.0, max_iterations=100, loss="linear", xtol=1e-8, gtol=1e-8, tr_solver="lsmr"):
+    # the default step is the call it always was, so an engine stand-in without the keyword still takes it
+    extra = {} if tr_solver == "lsmr" else dict(tr_solver=tr_solver)
+    res = eng.solve(ftol=tolerance, xtol=xtol, gtol=gtol, f_scale=f_scale, max_nfev=max_iterations, loss=loss, **extra)
     for line in format_log(res.log): info(line)
     info(res.message)
     info(f"Function evaluations {res.nfev}, initial cost {res.initial_cost:.4e}, final cost {res.cost:.4e}, "
@@ -469,9 +472,9 @@ class Calibration(Parameters):
                  None if self.inlier_mask is None else error_stats(self.reprojection_inliers))
 
 
-def _solve_args(tolerance=1e-4, max_iterations=100, loss="linear", xtol=1e-8, gtol=1e-8):
+def _solve_args(tolerance=1e-4, max_iterations=100, loss="linear", xtol=1e-8, gtol=1e-8, tr_solver="lsmr"):
   """bundle_adjust's keyword arguments (f_scale is chosen by the outlier loop), checked the way a call would check them."""
-  return dict(tolerance=tolerance, max_iterations=max_iterations, loss=loss, xtol=xtol, gtol=gtol)
+  return dict(tolerance=tolerance, max_iterations=max_iterations, loss=loss, xtol=xtol, gtol=gtol, tr_solver=tr_solver)
 
 
 def _report_line(stage, everything, kept):

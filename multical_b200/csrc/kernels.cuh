@@ -53,6 +53,8 @@ struct DeviceProblem {
   int motion_on, fix_aspect;            // motion_on: per-frame blocks are free (static / rolling frames)
   uint32_t fixed_intr;                  // bit i: entry i of every camera's [fx fy cx cy skew dist...] is held at its current value
                                         // (mcba_set_fixed_intrinsics): a dead column, like skew's
+  int tr_exact;                         // mcba_solve launches k_lm<FB, true>: scipy's tr_solver='exact' step instead of the 2-D subspace
+                                        // one (mcba_set_trust_region; a field here so that it is part of the solve graph's key)
   int frame_blocks;                     // the linearisation emits H_ff, g_f (at g + n_s) and W_f: motion_on, or hand-eye with free
                                         // hand-eye parameters (k_fold_hand_eye folds the frame blocks into them)
   // motion model (the `motion` argument of Calibration, calibration.py:44-46)

@@ -86,6 +86,7 @@ struct LmArgs {
   int syrk_chunks, syrk_cf;
   // partial sums (indexed by frame / virtual block: independent of the grid size where it matters for reproducibility)
   double *part_scale, *part_quad, *part_step;
+  double *gq, *piv;                  // tr_solver='exact': (A + alpha I)^-1 gn, and the reduced factor's diagonal of the probe at alpha = 0
   SolverState* st;
   mcba_log_row* log; int log_cap;
   unsigned long long* bar;
@@ -441,61 +442,65 @@ __device__ __noinline__ void chol_diag_warp_body(int n, int kb, double* S, doubl
 // A[ty + 16 p][tx + 16 q].  After every 16 columns the register tile is ROTATED (a[p][q] <- a[p+1][q+1]) so that the active pivot
 // block is always a[0][0] / column block q = 0: every register index on the pivot path is static, the path is ~45 instructions
 // (round 1's switch over the column block: ~150).  The factor goes to shared memory column by column as it is produced.
+// factor == false: only the substitutions, with the factor a previous call left in shm (tr_solver='exact': a second right-hand side).
 template <int R>
-__device__ __forceinline__ void chol_rot_body(int n, const double* Sg, const double* rhs, const double* gh, double reg, int* chol_fail, double* out, double* shm) {
+__device__ __forceinline__ void chol_rot_body(int n, const double* Sg, const double* rhs, const double* gh, double reg, int* chol_fail, double* out, double* shm,
+                                              bool factor = true) {
   const int ld = n | 1;
   double* Lm = shm;                       // n x ld factor
   double* colbuf = Lm + (size_t)n * ld;   // n (+16 pad)
   double* invd = colbuf + n + 16;         // n
   double* piv = invd + n;                 // 2
   const int tid = threadIdx.x, ty = tid & 15, tx = tid >> 4;
-  double a[R][R];
-#pragma unroll
-  for (int p = 0; p < R; p++)
-#pragma unroll
-    for (int q = 0; q < R; q++) {
-      const int i = ty + 16 * p, j = tx + 16 * q;
-      a[p][q] = (i < n && j < n) ? __ldcg(&Sg[(size_t)j * n + i]) + (i == j ? reg : 0.0) : 0.0;     // S is symmetric: coalesced read
-    }
-  __syncthreads();
-  if (tid == 0) piv[0] = a[0][0];
-  __syncthreads();
-  const int nblk = (n + 15) >> 4;
-  for (int kb = 0; kb < nblk; kb++) {
-    const int k0 = 16 * kb;
-    const int kend = min(16, n - k0);
-    for (int kt = 0; kt < kend; kt++) {
-      const int k = k0 + kt;
-      if (tx == kt) {                      // the 16 threads that hold column k (block column 0 of the rotated tile)
-        const double akk = piv[0];
-        const double rs = fast_rsqrt(fmin(fmax(akk, 1e-30), 1e30));
-        if (ty == kt) { invd[k] = rs; if (!(akk > 0.0)) *chol_fail += 1; }
-#pragma unroll
-        for (int p = 0; p < R; p++) {
-          const int i = k0 + ty + 16 * p;
-          if (i >= k && i < n) { const double lv = a[p][0] * rs; colbuf[i] = lv; Lm[i * ld + k] = lv; }
-        }
-      }
-      __syncthreads();
-      double ci[R], cj[R];
-#pragma unroll
-      for (int p = 0; p < R; p++) { const int i = k0 + ty + 16 * p; ci[p] = (i > k && i < n) ? colbuf[i] : 0.0; }
-#pragma unroll
-      for (int q = 0; q < R; q++) { const int j = k0 + tx + 16 * q; cj[q] = (j > k && j < n) ? colbuf[j] : 0.0; }
-#pragma unroll
-      for (int p = 0; p < R; p++)
-#pragma unroll
-        for (int q = 0; q < R; q++) a[p][q] -= ci[p] * cj[q];       // (also touches the unused upper triangle: harmless)
-      // publish the next pivot: thread (kt+1, kt+1) of this block, or (0,0) of the next block (its a[1][1] before the rotation)
-      if (kt + 1 < 16) { if (ty == kt + 1 && tx == kt + 1) piv[0] = a[0][0]; }
-      else if (R > 1) { if (ty == 0 && tx == 0) piv[0] = a[R > 1 ? 1 : 0][R > 1 ? 1 : 0]; }
-      __syncthreads();
-    }
-    // rotate: the next 16 x 16 pivot block moves to a[0][0]
+  if (factor) {
+    double a[R][R];
 #pragma unroll
     for (int p = 0; p < R; p++)
 #pragma unroll
-      for (int q = 0; q < R; q++) a[p][q] = (p + 1 < R && q + 1 < R) ? a[p + 1 < R ? p + 1 : p][q + 1 < R ? q + 1 : q] : 0.0;
+      for (int q = 0; q < R; q++) {
+        const int i = ty + 16 * p, j = tx + 16 * q;
+        a[p][q] = (i < n && j < n) ? __ldcg(&Sg[(size_t)j * n + i]) + (i == j ? reg : 0.0) : 0.0;     // S is symmetric: coalesced read
+      }
+    __syncthreads();
+    if (tid == 0) piv[0] = a[0][0];
+    __syncthreads();
+    const int nblk = (n + 15) >> 4;
+    for (int kb = 0; kb < nblk; kb++) {
+      const int k0 = 16 * kb;
+      const int kend = min(16, n - k0);
+      for (int kt = 0; kt < kend; kt++) {
+        const int k = k0 + kt;
+        if (tx == kt) {                      // the 16 threads that hold column k (block column 0 of the rotated tile)
+          const double akk = piv[0];
+          const double rs = fast_rsqrt(fmin(fmax(akk, 1e-30), 1e30));
+          if (ty == kt) { invd[k] = rs; if (!(akk > 0.0)) *chol_fail += 1; }
+#pragma unroll
+          for (int p = 0; p < R; p++) {
+            const int i = k0 + ty + 16 * p;
+            if (i >= k && i < n) { const double lv = a[p][0] * rs; colbuf[i] = lv; Lm[i * ld + k] = lv; }
+          }
+        }
+        __syncthreads();
+        double ci[R], cj[R];
+#pragma unroll
+        for (int p = 0; p < R; p++) { const int i = k0 + ty + 16 * p; ci[p] = (i > k && i < n) ? colbuf[i] : 0.0; }
+#pragma unroll
+        for (int q = 0; q < R; q++) { const int j = k0 + tx + 16 * q; cj[q] = (j > k && j < n) ? colbuf[j] : 0.0; }
+#pragma unroll
+        for (int p = 0; p < R; p++)
+#pragma unroll
+          for (int q = 0; q < R; q++) a[p][q] -= ci[p] * cj[q];       // (also touches the unused upper triangle: harmless)
+        // publish the next pivot: thread (kt+1, kt+1) of this block, or (0,0) of the next block (its a[1][1] before the rotation)
+        if (kt + 1 < 16) { if (ty == kt + 1 && tx == kt + 1) piv[0] = a[0][0]; }
+        else if (R > 1) { if (ty == 0 && tx == 0) piv[0] = a[R > 1 ? 1 : 0][R > 1 ? 1 : 0]; }
+        __syncthreads();
+      }
+      // rotate: the next 16 x 16 pivot block moves to a[0][0]
+#pragma unroll
+      for (int p = 0; p < R; p++)
+#pragma unroll
+        for (int q = 0; q < R; q++) a[p][q] = (p + 1 < R && q + 1 < R) ? a[p + 1 < R ? p + 1 : p][q + 1 < R ? q + 1 : q] : 0.0;
+    }
   }
   __syncthreads();
   if (tid < 32) {
@@ -744,13 +749,17 @@ __host__ __device__ inline size_t lm_smem_doubles(int n_s, int fb) {
 }
 
 // ---------------------------------------------------------------- the kernel
-template <int FB>
+// EXACT: tr_solver='exact' (the alpha search below).  A template argument, not a run-time flag, so that the default kernel is compiled
+// as if the search did not exist (it would otherwise share the register allocation of the loop around phases D-G, and spill).
+template <int FB, bool EXACT>
 __global__ void __launch_bounds__(LM_THREADS, 1)
 k_lm(LmArgs a) {
   extern __shared__ double ksm[];
   __shared__ SolverState S;
   __shared__ double sm[32];
   __shared__ int xerr, chol_fail_s;
+  __shared__ int ex_stage, ex_iters, ex_gn, ex_cf0;                   // tr_solver='exact': the alpha search (shared: nothing of it
+                                                                      // stays live in registers across the phases)
   __shared__ __align__(8) unsigned long long sbar[SYRK_STAGES];      // mbarriers of the SYRK operand pipeline
   unsigned sphases = 0;                                               // their phase parities (same in every thread)
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -760,6 +769,7 @@ k_lm(LmArgs a) {
   const int gthread = blockIdx.x * LM_THREADS + tid, gstride = nblk * LM_THREADS;
   const int gwarp = blockIdx.x * LM_WARPS + warp, gwarps = nblk * LM_WARPS;
   const bool multi = a.peer.world > 1;
+  constexpr bool exact = EXACT;                        // (one rank: mcba_solve refuses several)
   const bool writer = blockIdx.x == 0 && tid == 0;
   double* work = ksm + 64;
 
@@ -816,6 +826,15 @@ k_lm(LmArgs a) {
         S.cost = S.cost_new; S.njev += 1; S.last_reduction = S.actual_reduction; S.last_step_norm = S.step_norm;
         S.iteration += 1; S.accepted = 0; S.pending = 0;
       }
+    } else if (may_retry && exact) {
+      // the exact step factors A + alpha I again at the smaller radius, but the normal equations in the buffers are the rejected trial's:
+      // the next pass linearises the current point (trial state := current state) and solves from there without a log row
+      for (int i = gthread; i < a.n_items; i += gstride) make_trial_item(a.P, a.x, a.trial, i);
+      __syncthreads();
+      if (tid == 0) { S.relin = 1; S.relins += 1; S.pending = 0; }
+      __syncthreads();
+      if (writer) { *a.st = S; if (a.use_cond) cudaGraphSetConditional((cudaGraphConditionalHandle)a.cond_handle, 1); }
+      return;
     } else if (may_retry) {
       need_solve = false;                                 // shrink the radius and try again from the same model (trf.py inner loop)
     } else {
@@ -882,8 +901,9 @@ k_lm(LmArgs a) {
         if (!isfinite(S.cost)) { S.done = 1; S.status = -2; }          // non-finite residuals at the initial point (scipy raises ValueError)
       }
       __syncthreads();
-      log_row(S.iteration, S.nfev, S.cost, S.iteration == 0 ? NAN : S.last_reduction, S.iteration == 0 ? NAN : S.last_step_norm, S.g_norm);
+      if (!S.relin) log_row(S.iteration, S.nfev, S.cost, S.iteration == 0 ? NAN : S.last_reduction, S.iteration == 0 ? NAN : S.last_step_norm, S.g_norm);
       __syncthreads();
+      if (tid == 0) S.relin = 0;
       if (S.done) {
         if (writer) { *a.st = S; if (multi) *a.peer.seq = xseq; if (a.use_cond) cudaGraphSetConditional((cudaGraphConditionalHandle)a.cond_handle, 0); }
         return;
@@ -948,148 +968,271 @@ k_lm(LmArgs a) {
         }
       }
     };
-    LMPH(3)
-    quad_pass(a.gh, a.gh, 0, a.part_quad + 8);
-    grid_barrier(a.bar, nblk);
-    {
-      double agg = sum_records(a.part_quad + 8, F + nsh, 5, 0, sm);
-      if (multi) {
-        // H_ss is this rank's local part: its quadratic form sums over the ranks like the frame parts
-        if (writer) a.part_quad[0] = agg;
-        grid_barrier(a.bar, nblk);
-        XSeg seg[1] = {{a.part_quad, 1, 0}};
-        exchange(a, seg, 1, ++xseq, &xerr);
-        agg = __ldcg(&a.part_quad[0]);
+    // ---------------------------------------------------------------------------------------- phases D-G as functions of the damping
+    // backsub(v): the frame parts of v from its shared part v_s, v_f = L_f^-T (z_f - Y_f^T v_s)
+    auto backsub = [&](double* vec) {
+      for (int f = gwarp; f < F; f += gwarps) {
+        const double* Yf = a.Y + (size_t)f * SYRK_TILE * FB;
+        const size_t ytile = (size_t)a.F * SYRK_TILE * FB;
+        double t[FB];
+#pragma unroll
+        for (int k = 0; k < FB; k++) t[k] = 0.0;
+#pragma unroll 4
+        for (int s = lane; s < n_s; s += 32) {
+          const double ps = __ldcg(&vec[s]);
+          const double2* y2 = reinterpret_cast<const double2*>(Yf + (size_t)(s >> 5) * ytile + (size_t)(s & 31) * FB);
+#pragma unroll
+          for (int k = 0; k < FB / 2; k++) { const double2 y = y2[k]; t[2 * k] += y.x * ps; t[2 * k + 1] += y.y * ps; }
+        }
+#pragma unroll
+        for (int k = 0; k < FB; k++) {
+#pragma unroll
+          for (int o = 16; o > 0; o >>= 1) t[k] += __shfl_xor_sync(0xffffffffu, t[k], o);
+        }
+        if (lane == 0) {
+          const double* L = a.Lf + (size_t)f * FB * FB;
+          double y[FB];
+#pragma unroll
+          for (int i = 0; i < FB; i++) y[i] = a.zf[(size_t)f * FB + i] - t[i];
+#pragma unroll
+          for (int i = FB - 1; i >= 0; i--) {
+            double v = y[i];
+#pragma unroll
+            for (int k = 0; k < FB; k++) if (k > i) v -= L[k * FB + i] * y[k];
+            y[i] = v * L[i * FB + i];                            // the stored diagonal is 1 / L_ii
+          }
+#pragma unroll
+          for (int i = 0; i < FB; i++) vec[n_s + FB * f + i] = y[i];
+        }
+        __syncwarp();
       }
-      if (tid == 0) { reg_compute(&S, agg); S.agg = agg; }
-      __syncthreads();
-    }
-    LMPH(4)
-    const double reg = S.reg;
-    // ---------------------------------------------------------------------------------------- phase D: frames out, S in
-    for (size_t idx = gthread; idx < (size_t)n_s * n_s; idx += gstride) {
-      const int i = idx / n_s, j = idx % n_s;
-      a.S[idx] = a.d[i] * a.d[j] * a.Hss[idx];
-    }
-    if (F > 0) {
-      double* Lw = work + (size_t)warp * (FB * FB + FB);
-      for (int f = gwarp; f < F; f += gwarps) schur_frame<FB>(a, f, reg, lane, Lw);
-    }
-    grid_barrier(a.bar, nblk);
-    // ---------------------------------------------------------------------------------------- phase E: S -= sum_f Y_f Y_f^T
-    LMPH(5)
-    if (F > 0 && n_s > 0) {
-      const int tiles = (n_s + SYRK_TILE - 1) / SYRK_TILE;
-      const int npair = tiles * (tiles + 1) / 2;
-      for (int vb = blockIdx.x; vb < npair * a.syrk_chunks; vb += nblk) {
-        const int chunk = vb / npair; int pr = vb % npair;
-        int ti = 0; while (pr >= tiles - ti) { pr -= tiles - ti; ti++; }
-        const int tj = ti + pr;
-        syrk_tile<FB>(a, ti, tj, chunk, work, sbar, sphases);
-      }
-      grid_barrier(a.bar, nblk);
-      // fixed-order sum over the frame chunks; tiles hold the upper triangle (ti <= tj), S is kept full
+      __syncthreads();      // a warp's stores of v_f are read by the same warp next (same frame -> same warp: gwarp stride is identical)
+    };
+    // solve_reg(reg): (A + reg I) gn = g_h -- the factors of A + reg I stay behind (L_f, Y_f, the reduced factor)
+    auto solve_reg = [&](double reg) {
+      // ---------------------------------------------------------------------------------------- phase D: frames out, S in
       for (size_t idx = gthread; idx < (size_t)n_s * n_s; idx += gstride) {
         const int i = idx / n_s, j = idx % n_s;
-        const int ii = min(i, j), jj = max(i, j);
-        // inside a diagonal tile both triangles were computed; everywhere else take the (ii, jj) entry
-        double s = 0.0;
-        for (int c = 0; c < a.syrk_chunks; c++) s += __ldcg(&a.Spart[(size_t)c * n_s * n_s + (size_t)ii * n_s + jj]);
-        a.S[idx] -= s;
+        a.S[idx] = a.d[i] * a.d[j] * a.Hss[idx];
       }
-      for (int i = gthread; i < n_s; i += gstride) {
-        double s = 0.0;
-        for (int c = 0; c < a.syrk_chunks; c++) s += __ldcg(&a.rpart[(size_t)c * n_s + i]);
-        a.rhs[i] = -s;
+      if (F > 0) {
+        double* Lw = work + (size_t)warp * (FB * FB + FB);
+        for (int f = gwarp; f < F; f += gwarps) schur_frame<FB>(a, f, reg, lane, Lw);
       }
-    } else {
-      for (int i = gthread; i < n_s; i += gstride) a.rhs[i] = 0.0;
-    }
-    grid_barrier(a.bar, nblk);
-    if (multi && n_s > 0) {
-      XSeg seg[2] = {{a.S, n_s * n_s, 0}, {a.rhs, n_s, 0}};
-      exchange(a, seg, 2, ++xseq, &xerr);
-    }
-    // ---------------------------------------------------------------------------------------- phase F: reduced solve
-    LMPH(6)
-    if (n_s > 0) {
-      if (n_s <= CHOL_SMALL_MAX) {
-        if (blockIdx.x == 0) {
-          const int R = (n_s + 15) / 16;
-#define CS(RR) case RR: chol_rot_body<RR>(n_s, a.S, a.rhs, a.gh, reg, &chol_fail_s, a.gn, work); break;
-          switch (R) { CS(1) CS(2) CS(3) CS(4) CS(5) CS(6) CS(7) CS(8) }
-#undef CS
+      grid_barrier(a.bar, nblk);
+      // ---------------------------------------------------------------------------------------- phase E: S -= sum_f Y_f Y_f^T
+      LMPH(5)
+      if (F > 0 && n_s > 0) {
+        const int tiles = (n_s + SYRK_TILE - 1) / SYRK_TILE;
+        const int npair = tiles * (tiles + 1) / 2;
+        for (int vb = blockIdx.x; vb < npair * a.syrk_chunks; vb += nblk) {
+          const int chunk = vb / npair; int pr = vb % npair;
+          int ti = 0; while (pr >= tiles - ti) { pr -= tiles - ti; ti++; }
+          const int tj = ti + pr;
+          syrk_tile<FB>(a, ti, tj, chunk, work, sbar, sphases);
+        }
+        grid_barrier(a.bar, nblk);
+        // fixed-order sum over the frame chunks; tiles hold the upper triangle (ti <= tj), S is kept full
+        for (size_t idx = gthread; idx < (size_t)n_s * n_s; idx += gstride) {
+          const int i = idx / n_s, j = idx % n_s;
+          const int ii = min(i, j), jj = max(i, j);
+          // inside a diagonal tile both triangles were computed; everywhere else take the (ii, jj) entry
+          double s = 0.0;
+          for (int c = 0; c < a.syrk_chunks; c++) s += __ldcg(&a.Spart[(size_t)c * n_s * n_s + (size_t)ii * n_s + jj]);
+          a.S[idx] -= s;
+        }
+        for (int i = gthread; i < n_s; i += gstride) {
+          double s = 0.0;
+          for (int c = 0; c < a.syrk_chunks; c++) s += __ldcg(&a.rpart[(size_t)c * n_s + i]);
+          a.rhs[i] = -s;
         }
       } else {
-        for (int i = gthread; i < n_s; i += gstride) a.S[(size_t)i * n_s + i] += reg;
-        grid_barrier(a.bar, nblk);
-        // one barrier per panel: CTA 0 finishes the next diagonal block's tile of the previous trailing update first and factors it
-        // (look-ahead) while the other CTAs work off the rest of that update
-        const int npan = (n_s + CHOL_NB - 1) / CHOL_NB;
-        for (int b = 0; b < npan; b++) {
-          const int kb = CHOL_NB * b;
-          const int rem = b > 0 ? n_s - kb : 0;                       // rows of the trailing matrix of panel b-1
-          const int t = (rem + CHOL_NB - 1) / CHOL_NB, ntile = t * (t + 1) / 2;
+        for (int i = gthread; i < n_s; i += gstride) a.rhs[i] = 0.0;
+      }
+      grid_barrier(a.bar, nblk);
+      if (multi && n_s > 0) {
+        XSeg seg[2] = {{a.S, n_s * n_s, 0}, {a.rhs, n_s, 0}};
+        exchange(a, seg, 2, ++xseq, &xerr);
+      }
+      // ---------------------------------------------------------------------------------------- phase F: reduced solve
+      LMPH(6)
+      if (n_s > 0) {
+        if (n_s <= CHOL_SMALL_MAX) {
           if (blockIdx.x == 0) {
-            if (b > 0) chol_fused_tile(n_s, b - 1, 0, 0, a.S, a.Linv, work);
-            chol_diag_warp_body(n_s, kb, a.S, a.Linv, &chol_fail_s, work);
+            const int R = (n_s + 15) / 16;
+#define CS(RR) case RR: chol_rot_body<RR>(n_s, a.S, a.rhs, a.gh, reg, &chol_fail_s, a.gn, work); break;
+            switch (R) { CS(1) CS(2) CS(3) CS(4) CS(5) CS(6) CS(7) CS(8) }
+#undef CS
           }
-          if (b > 0) {
-            const int first = nblk > 1 ? (int)blockIdx.x - 1 : 0, step = nblk > 1 ? nblk - 1 : 1;
-            if (nblk == 1 || blockIdx.x > 0)
-              for (int vb = 1 + first; vb < ntile; vb += step) {
-                int ti = 0, pr = vb; while (pr > ti) { pr -= ti + 1; ti++; }        // lower triangle: ti >= tj = pr
-                chol_fused_tile(n_s, b - 1, ti, pr, a.S, a.Linv, work);
-              }
-          }
+        } else {
+          for (int i = gthread; i < n_s; i += gstride) a.S[(size_t)i * n_s + i] += reg;
           grid_barrier(a.bar, nblk);
+          // one barrier per panel: CTA 0 finishes the next diagonal block's tile of the previous trailing update first and factors it
+          // (look-ahead) while the other CTAs work off the rest of that update
+          const int npan = (n_s + CHOL_NB - 1) / CHOL_NB;
+          for (int b = 0; b < npan; b++) {
+            const int kb = CHOL_NB * b;
+            const int rem = b > 0 ? n_s - kb : 0;                       // rows of the trailing matrix of panel b-1
+            const int t = (rem + CHOL_NB - 1) / CHOL_NB, ntile = t * (t + 1) / 2;
+            if (blockIdx.x == 0) {
+              if (b > 0) chol_fused_tile(n_s, b - 1, 0, 0, a.S, a.Linv, work);
+              chol_diag_warp_body(n_s, kb, a.S, a.Linv, &chol_fail_s, work);
+            }
+            if (b > 0) {
+              const int first = nblk > 1 ? (int)blockIdx.x - 1 : 0, step = nblk > 1 ? nblk - 1 : 1;
+              if (nblk == 1 || blockIdx.x > 0)
+                for (int vb = 1 + first; vb < ntile; vb += step) {
+                  int ti = 0, pr = vb; while (pr > ti) { pr -= ti + 1; ti++; }        // lower triangle: ti >= tj = pr
+                  chol_fused_tile(n_s, b - 1, ti, pr, a.S, a.Linv, work);
+                }
+            }
+            grid_barrier(a.bar, nblk);
+          }
+          LMPH(11)
+          if (blockIdx.x == 0) {
+            chol_substitute_body(n_s, a.S, a.Linv, a.rhs, a.gh, a.gn, work);
+          }
+          LMPH(12)
         }
-        LMPH(11)
-        if (blockIdx.x == 0) {
-          chol_substitute_body(n_s, a.S, a.Linv, a.rhs, a.gh, a.gn, work);
-        }
-        LMPH(12)
       }
+      grid_barrier(a.bar, nblk);
+      // ---------------------------------------------------------------------------------------- phase G: back-substitution + subspace forms
+      LMPH(7)
+      backsub(a.gn);
+    };
+    // ---------------------------------------------------------------------------------------- tr_solver='exact'
+    // solve_again(b, out): out = (A + reg I)^-1 b with the factors solve_reg left (z_f = L_f^-1 b_f, rhs = b_s - sum_f Y_f z_f, the
+    // reduced substitutions, backsub), then ||gn||^2 and gn . out summed in CTA order -> pq[0], pq[1] in every CTA
+    auto solve_again = [&](const double* b, double* out, double* pq) {
+      for (int f = gwarp; f < F; f += gwarps)
+        if (lane == 0) {                                // b_f was stored by this lane (backsub of the same frame)
+          const double* L = a.Lf + (size_t)f * FB * FB;
+          double z[FB];
+#pragma unroll
+          for (int i = 0; i < FB; i++) {
+            double t = b[n_s + FB * f + i];
+#pragma unroll
+            for (int k = 0; k < FB; k++) if (k < i) t -= L[i * FB + k] * z[k];
+            z[i] = t * L[i * FB + i];
+            a.zf[(size_t)f * FB + i] = z[i];
+          }
+        }
+      grid_barrier(a.bar, nblk);
+      if (F > 0 && n_s > 0) {
+        // row s of sum_f Y_f z_f per frame chunk (the chunks of the SYRK), then the chunks in order
+        const size_t ytile = (size_t)a.F * SYRK_TILE * FB;
+        for (int idx = gthread; idx < a.syrk_chunks * n_s; idx += gstride) {
+          const int c = idx / n_s, r = idx % n_s;
+          const int f0 = c * a.syrk_cf, f1 = min(F, f0 + a.syrk_cf);
+          const double* Yr = a.Y + (size_t)(r >> 5) * ytile + (size_t)(r & 31) * FB;
+          double acc = 0.0;
+          for (int f = f0; f < f1; f++) {
+#pragma unroll
+            for (int k = 0; k < FB; k++) acc += __ldcg(&Yr[(size_t)f * SYRK_TILE * FB + k]) * __ldcg(&a.zf[(size_t)f * FB + k]);
+          }
+          a.rpart[(size_t)c * n_s + r] = acc;
+        }
+        grid_barrier(a.bar, nblk);
+        for (int i = gthread; i < n_s; i += gstride) {
+          double t = 0.0;
+          for (int c = 0; c < a.syrk_chunks; c++) t += __ldcg(&a.rpart[(size_t)c * n_s + i]);
+          a.rhs[i] = -t;
+        }
+      } else {
+        for (int i = gthread; i < n_s; i += gstride) a.rhs[i] = 0.0;
+      }
+      grid_barrier(a.bar, nblk);
+      if (n_s > 0 && blockIdx.x == 0) {
+        if (n_s <= CHOL_SMALL_MAX) {
+          const int R = (n_s + 15) / 16;
+#define CS(RR) case RR: chol_rot_body<RR>(n_s, a.S, a.rhs, b, 0.0, &chol_fail_s, out, work, false); break;
+          switch (R) { CS(1) CS(2) CS(3) CS(4) CS(5) CS(6) CS(7) CS(8) }
+#undef CS
+        } else {
+          chol_substitute_body(n_s, a.S, a.Linv, a.rhs, b, out, work);
+        }
+      }
+      grid_barrier(a.bar, nblk);
+      backsub(out);
+      grid_barrier(a.bar, nblk);
+      double s1 = 0.0, s2 = 0.0;
+      for (int i = gthread; i < n; i += gstride) { const double g = __ldcg(&a.gn[i]); s1 += g * g; s2 += g * __ldcg(&out[i]); }
+      const double r1 = block_sum_all(s1, sm), r2 = block_sum_all(s2, sm);
+      if (tid == 0) { a.part_scale[(size_t)blockIdx.x * 6] = r1; a.part_scale[(size_t)blockIdx.x * 6 + 1] = r2; }
+      grid_barrier(a.bar, nblk);
+      pq[0] = sum_records(a.part_scale, nblk, 6, 0, sm);
+      pq[1] = sum_records(a.part_scale, nblk, 6, 1, sm);
+    };
+    double reg = 0.0;
+    if (!exact) {
+      LMPH(3)
+      quad_pass(a.gh, a.gh, 0, a.part_quad + 8);
+      grid_barrier(a.bar, nblk);
+      {
+        double agg = sum_records(a.part_quad + 8, F + nsh, 5, 0, sm);
+        if (multi) {
+          // H_ss is this rank's local part: its quadratic form sums over the ranks like the frame parts
+          if (writer) a.part_quad[0] = agg;
+          grid_barrier(a.bar, nblk);
+          XSeg seg[1] = {{a.part_quad, 1, 0}};
+          exchange(a, seg, 1, ++xseq, &xerr);
+          agg = __ldcg(&a.part_quad[0]);
+        }
+        if (tid == 0) { reg_compute(&S, agg); S.agg = agg; }
+        __syncthreads();
+      }
+      LMPH(4)
+      reg = S.reg;
     }
-    grid_barrier(a.bar, nblk);
-    // ---------------------------------------------------------------------------------------- phase G: back-substitution + subspace forms
-    LMPH(7)
-    for (int f = gwarp; f < F; f += gwarps) {
-      const double* Yf = a.Y + (size_t)f * SYRK_TILE * FB;
-      const size_t ytile = (size_t)a.F * SYRK_TILE * FB;
-      double t[FB];
-#pragma unroll
-      for (int k = 0; k < FB; k++) t[k] = 0.0;
-#pragma unroll 4
-      for (int s = lane; s < n_s; s += 32) {
-        const double ps = __ldcg(&a.gn[s]);
-        const double2* y2 = reinterpret_cast<const double2*>(Yf + (size_t)(s >> 5) * ytile + (size_t)(s & 31) * FB);
-#pragma unroll
-        for (int k = 0; k < FB / 2; k++) { const double2 y = y2[k]; t[2 * k] += y.x * ps; t[2 * k + 1] += y.y * ps; }
-      }
-#pragma unroll
-      for (int k = 0; k < FB; k++) {
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) t[k] += __shfl_xor_sync(0xffffffffu, t[k], o);
-      }
-      if (lane == 0) {
-        const double* L = a.Lf + (size_t)f * FB * FB;
-        double y[FB];
-#pragma unroll
-        for (int i = 0; i < FB; i++) y[i] = a.zf[(size_t)f * FB + i] - t[i];
-#pragma unroll
-        for (int i = FB - 1; i >= 0; i--) {
-          double v = y[i];
-#pragma unroll
-          for (int k = 0; k < FB; k++) if (k > i) v -= L[k * FB + i] * y[k];
-          y[i] = v * L[i * FB + i];                            // the stored diagonal is 1 / L_ii
-        }
-#pragma unroll
-        for (int i = 0; i < FB; i++) a.gn[n_s + FB * f + i] = y[i];
-      }
-      __syncwarp();
+    // tr_solver='exact': common.py solve_lsq_trust_region on factorisations of A + alpha I, one pass of the loop below per alpha --
+    // stage 0 the probe at alpha = 0 (the Gauss-Newton step if A is nonsingular and it lies inside Delta), stage 1 the Newton iterations
+    // on phi(alpha) = ||p(alpha)|| - Delta, stage 2 p at the last alpha, scaled onto the boundary.  A counts as nonsingular when the
+    // probe has every reduced pivot above n_s eps max_j A_jj, dead columns (zero row and column of A: their entries of every solve are
+    // zero) left out; otherwise every alpha factored is at least reg_floor.  The search state lives in S (tid 0 updates it, every thread
+    // reads it after a __syncthreads).  The default step makes one pass.
+    if (exact) {
+      if (tid == 0) { ex_stage = 0; ex_iters = 0; ex_gn = 0; ex_cf0 = chol_fail_s; }    // (the probe may fail on a singular A: not a retry)
+      __syncthreads();
     }
-    __syncthreads();      // a warp's gn_f stores are read by the same warp below (same frame -> same warp: gwarp stride is identical)
+    for (;;) {
+      solve_reg(reg);
+      if (!exact || ex_stage == 2) break;
+      if (ex_stage == 0) {
+        if (n_s > 0 && n_s <= CHOL_SMALL_MAX && blockIdx.x == 0)
+          for (int k = tid; k < n_s; k += LM_THREADS) a.piv[k] = work[(size_t)k * (n_s | 1) + k];      // L_kk of chol_rot_body's factor
+        grid_barrier(a.bar, nblk);
+        double amax = 0.0;
+        for (int k = tid; k < n_s; k += LM_THREADS) amax = fmax(amax, a.d[k] * a.d[k] * a.Hss[(size_t)k * n_s + k]);
+        amax = block_max_all(amax, sm);
+        const double tol = n_s * 2.220446049250313e-16 * amax;
+        double bad = 0.0;
+        for (int k = tid; k < n_s; k += LM_THREADS) {
+          if (a.d[k] * a.d[k] * a.Hss[(size_t)k * n_s + k] == 0.0) continue;
+          const double l = n_s <= CHOL_SMALL_MAX ? __ldcg(&a.piv[k]) : __ldcg(&a.S[(size_t)k * n_s + k]);
+          if (!(l > 0.0 && l * l > tol)) bad += 1.0;
+        }
+        bad = block_sum_all(bad, sm);
+        if (tid == 0) { S.full_rank = bad == 0.0; chol_fail_s = ex_cf0; }
+        __syncthreads();
+      }
+      double pq[2] = {0.0, 0.0};
+      if (ex_stage == 1 || S.full_rank) solve_again(a.gn, a.gq, pq);
+      __syncthreads();
+      if (tid == 0) {
+        if (ex_stage == 0) {
+          ex_gn = S.full_rank && sqrt(pq[0]) <= S.Delta;
+          if (ex_gn) S.tr_alpha = 0.0;
+          else { exact_begin(&S, pq[0], pq[1]); ex_stage = 1; }
+        } else {
+          ex_iters += 1;
+          if (exact_newton(&S, pq[0], pq[1]) || ex_iters == EXACT_MAX_ITER) ex_stage = 2;
+        }
+        if (ex_stage == 1) exact_reset(&S);
+      }
+      __syncthreads();
+      if (ex_gn) break;
+      reg = fmax(S.tr_alpha, S.full_rank ? 0.0 : S.reg_floor);
+    }
     LMPH(8)
     quad_pass(a.gh, a.gn, 1, a.part_quad + 8);
     grid_barrier(a.bar, nblk);
@@ -1104,14 +1247,21 @@ k_lm(LmArgs a) {
         exchange(a, seg, 1, ++xseq, &xerr);
         agn = __ldcg(&a.part_quad[0]); ann = __ldcg(&a.part_quad[1]); dtf = __ldcg(&a.part_quad[2]); g2f = __ldcg(&a.part_quad[3]);
       }
-      if (tid == 0) subspace_compute(&S, S.agg, agn, ann, dts, dtf, g2s, g2f);
+      if (tid == 0) {
+        if (!exact) subspace_compute(&S, S.agg, agn, ann, dts, dtf, g2s, g2f);
+        else {
+          const double gnn = sqrt(g2s + g2f);
+          exact_step(&S, ex_gn ? -1.0 : -S.Delta / gnn, gnn, ann, dts + dtf);
+          S.alpha_iters += ex_iters;
+        }
+      }
       __syncthreads();
     }
   }
 
   // ------------------------------------------------------------------------------------------ phase I: step and trial state
   LMPH(9)
-  if (tid == 0) tr_step_compute(&S);
+  if (tid == 0 && !exact) tr_step_compute(&S);
   __syncthreads();
   {
     const double al = S.alpha, be = S.beta;

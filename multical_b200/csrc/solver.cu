@@ -120,6 +120,7 @@ struct mcba_ctx {
   std::string err;
   int rank = 0, world = 1;
   int launches = 0;
+  int last_alpha_iters = 0;           // mcba_last_alpha_iterations
   int num_sms = 132;
 
   bool uploaded = false;
@@ -151,7 +152,7 @@ struct mcba_ctx {
   struct SolveGraph { cudaGraphExec_t exec = nullptr; cudaGraph_t graph = nullptr; std::vector<char> key; cudaStream_t stream = nullptr; int body_launches = 0; } sg;
   bool graph_launched = false;
   int lin_grid = 1, lin_split = 1, lin_warps = LIN_WARPS;
-  DevBuf<double> x, x_new, sinv, d, gh, gn, Y, Lf, zf, S, rhs, Linv;
+  DevBuf<double> x, x_new, sinv, d, gh, gn, gq, piv, Y, Lf, zf, S, rhs, Linv;
   DevBuf<double> lin_cost, eval_cost;     // cost at the last linearisation (k_reduce_shared), cost of mcba_residuals
   DevBuf<SolverState> state;
   // NVLink peer-memory exchange of the solver kernel (lm_kernel.cuh LmPeer)
@@ -378,7 +379,7 @@ LmArgs make_lm_args(mcba_ctx* ctx, int log_cap) {
   a.n_items = trial_items(P);
   a.Hss = ctx->Hss.p; a.Hff = ctx->Hff.p; a.W = ctx->W.p; a.g = ctx->g.p;
   a.frame_cost = ctx->frame_cost.p; a.lin_cost = ctx->lin_cost.p;
-  a.x = ctx->x.p; a.x_new = ctx->x_new.p; a.sinv = ctx->sinv.p; a.d = ctx->d.p; a.gh = ctx->gh.p; a.gn = ctx->gn.p;
+  a.x = ctx->x.p; a.x_new = ctx->x_new.p; a.sinv = ctx->sinv.p; a.d = ctx->d.p; a.gh = ctx->gh.p; a.gn = ctx->gn.p; a.gq = ctx->gq.p; a.piv = ctx->piv.p;
   a.Y = ctx->Y.p; a.Lf = ctx->Lf.p; a.zf = ctx->zf.p; a.S = ctx->S.p; a.rhs = ctx->rhs.p; a.Spart = ctx->Spart.p; a.rpart = ctx->rpart.p; a.Linv = ctx->Linv.p;
   a.syrk_chunks = ctx->syrk_chunks; a.syrk_cf = ctx->syrk_cf;
   a.part_scale = ctx->part_scale.p; a.part_quad = ctx->part_quad.p; a.part_step = ctx->part_step.p;
@@ -394,12 +395,17 @@ int launch_lm(mcba_ctx* ctx, const LmArgs& a) {
   const size_t sm = sizeof(double) * lm_smem_doubles(ctx->P.n_s, ctx->P.fb);
   LmArgs args = a;
 #ifdef MCBA_SIMT_BUILD
-  if (ctx->P.fb == 12) k_lm<12><<<ctx->lm_grid, LM_THREADS, sm, ctx->stream>>>(args); else k_lm<6><<<ctx->lm_grid, LM_THREADS, sm, ctx->stream>>>(args);
+  if (ctx->P.tr_exact) {
+    if (ctx->P.fb == 12) k_lm<12, true><<<ctx->lm_grid, LM_THREADS, sm, ctx->stream>>>(args); else k_lm<6, true><<<ctx->lm_grid, LM_THREADS, sm, ctx->stream>>>(args);
+  } else {
+    if (ctx->P.fb == 12) k_lm<12, false><<<ctx->lm_grid, LM_THREADS, sm, ctx->stream>>>(args); else k_lm<6, false><<<ctx->lm_grid, LM_THREADS, sm, ctx->stream>>>(args);
+  }
   CKL();
 #else
   // cooperative launch: every CTA of the grid is resident for the whole kernel (the grid barriers spin)
   void* params[] = {&args};
-  const void* fn = ctx->P.fb == 12 ? (const void*)k_lm<12> : (const void*)k_lm<6>;
+  const void* fn = ctx->P.tr_exact ? (ctx->P.fb == 12 ? (const void*)k_lm<12, true> : (const void*)k_lm<6, true>)
+                                   : (ctx->P.fb == 12 ? (const void*)k_lm<12, false> : (const void*)k_lm<6, false>);
   CK(cudaLaunchCooperativeKernel(fn, dim3(ctx->lm_grid), dim3(LM_THREADS), params, sm, ctx->stream));
   ctx->launches++;
 #endif
@@ -458,7 +464,7 @@ int run_lm_loop(mcba_ctx* ctx, int loss, double f_scale, int log_cap) {
   // host-driven loop (the SIMT interpreter build; MCBA_GRAPH=0): same kernels, one state read per body
   ctx->graph_launched = false;
   SolverState h{};
-  for (int it = 0; it < log_cap + 8; it++) {
+  for (int it = 0; it < 2 * (log_cap + 8); it++) {      // (tr_solver='exact': a rejected trial costs a second pass, a relinearisation)
     int r = lm_body(ctx, loss, f_scale, a); if (r) return r;
     CK(cudaMemcpyAsync(&h, ctx->state.p, sizeof(h), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
@@ -580,8 +586,8 @@ int setup_problem(mcba_ctx* ctx, const mcba_problem_desc* desc, int64_t N, int V
   CK(ctx->Lf.alloc((size_t)std::max(F, 1) * fbs * fbs)); CK(ctx->zf.alloc((size_t)std::max(F, 1) * fbs));
   CK(ctx->view_cost.alloc((size_t)std::max(V, 1)));
   const size_t nn = (size_t)std::max(P.n, 1);
-  CK(ctx->x.alloc(nn)); CK(ctx->x_new.alloc(nn)); CK(ctx->sinv.alloc(nn)); CK(ctx->d.alloc(nn)); CK(ctx->gh.alloc(nn)); CK(ctx->gn.alloc(nn));
-  CK(ctx->S.alloc((size_t)std::max(P.n_s, 1) * std::max(P.n_s, 1))); CK(ctx->rhs.alloc((size_t)std::max(P.n_s, 1)));
+  CK(ctx->x.alloc(nn)); CK(ctx->x_new.alloc(nn)); CK(ctx->sinv.alloc(nn)); CK(ctx->d.alloc(nn)); CK(ctx->gh.alloc(nn)); CK(ctx->gn.alloc(nn)); CK(ctx->gq.alloc(nn));
+  CK(ctx->S.alloc((size_t)std::max(P.n_s, 1) * std::max(P.n_s, 1))); CK(ctx->rhs.alloc((size_t)std::max(P.n_s, 1))); CK(ctx->piv.alloc((size_t)std::max(P.n_s, 1)));
   CK(ctx->Linv.alloc((size_t)((std::max(P.n_s, 1) + CHOL_NB - 1) / CHOL_NB) * CHOL_NB * CHOL_NB));
   CK(ctx->lin_cost.alloc(1)); CK(cudaMemsetAsync(ctx->lin_cost.p, 0, sizeof(double), ctx->stream));
   CK(ctx->eval_cost.alloc(1)); CK(cudaMemsetAsync(ctx->eval_cost.p, 0, sizeof(double), ctx->stream));
@@ -726,8 +732,10 @@ int mcba_create(int device, mcba_ctx** out) {
       });
   cudaFuncSetAttribute(k_reduce_shared<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
   cudaFuncSetAttribute(k_reduce_shared<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-  cudaFuncSetAttribute(k_lm<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-  cudaFuncSetAttribute(k_lm<12>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+  cudaFuncSetAttribute(k_lm<6, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+  cudaFuncSetAttribute(k_lm<12, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+  cudaFuncSetAttribute(k_lm<6, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+  cudaFuncSetAttribute(k_lm<12, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
   cudaFuncSetAttribute(k_pose_align<PI_SMALL_THREADS, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, PI_SMALL_MAX * PI_ROW_BYTES);
   for (int model = MODEL_STANDARD; model <= MODEL_TILTED; model++)
     with_model(model, false, [](auto M, auto) {
@@ -2125,6 +2133,21 @@ int mcba_set_fixed_intrinsics(mcba_ctx* ctx, const uint8_t* fixed) {
   return MCBA_OK;
 }
 
+// scipy's tr_solver: like the fixed-intrinsics mask a field of the problem descriptor (graph key; cleared by every upload)
+int mcba_set_trust_region(mcba_ctx* ctx, int32_t mode) {
+  if (!ctx) return MCBA_ERR_ARG;
+  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
+  REQUIRE(mode == MCBA_TR_SUBSPACE || mode == MCBA_TR_EXACT, MCBA_ERR_ARG, "trust region: MCBA_TR_SUBSPACE or MCBA_TR_EXACT");
+  ctx->P.tr_exact = mode == MCBA_TR_EXACT ? 1 : 0;
+  return MCBA_OK;
+}
+
+int mcba_last_alpha_iterations(mcba_ctx* ctx, int32_t* total) {
+  if (!ctx || !total) return MCBA_ERR_ARG;
+  *total = ctx->last_alpha_iters;
+  return MCBA_OK;
+}
+
 int mcba_get_params(mcba_ctx* ctx, double* cam_rt, double* board_rt, double* frame_rt, double* intrinsics) {
   if (!ctx) return MCBA_ERR_ARG;
   REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
@@ -2269,6 +2292,8 @@ int mcba_solve(mcba_ctx* ctx, const mcba_solve_opts* opts, mcba_solve_result* re
   REQUIRE(opts->loss >= 0 && opts->loss <= 4, MCBA_ERR_ARG, "unknown loss");
   REQUIRE(opts->max_nfev > 0, MCBA_ERR_ARG, "max_nfev must be positive");
   REQUIRE(opts->f_scale > 0, MCBA_ERR_ARG, "f_scale must be positive");
+  REQUIRE(ctx->world == 1 || !ctx->P.tr_exact, MCBA_ERR_UNSUPPORTED,
+          "tr_solver='exact' on several ranks: the alpha search would exchange the reduced system once per alpha");
   REQUIRE(ctx->world == 1 || ctx->peer_ready, MCBA_ERR_STATE, "several ranks: the exchanges run over NVLink peer memory (mcba_peer_export / mcba_peer_import first)");
   CK(cudaSetDevice(ctx->device));
   const DeviceProblem& P = ctx->P;
@@ -2278,6 +2303,7 @@ int mcba_solve(mcba_ctx* ctx, const mcba_solve_opts* opts, mcba_solve_result* re
   const int n = P.n;
   memset(result, 0, sizeof(*result));
   ctx->launches = 0;
+  ctx->last_alpha_iters = 0;
   ctx->errors_current = false;
   struct EventPair {       // destroyed on every return path
     cudaEvent_t a = nullptr, b = nullptr;
@@ -2332,7 +2358,8 @@ int mcba_solve(mcba_ctx* ctx, const mcba_solve_opts* opts, mcba_solve_result* re
   if (log) for (int i = 0; i < nlog && i < log_capacity; i++) log[i] = rows[(size_t)i];
   result->cost = h.cost; result->optimality = h.g_norm; result->nfev = h.nfev; result->njev = h.njev;
   result->status = h.status == -99 ? 0 : h.status; result->n_log = std::min(nlog, (int)log_capacity); result->device_ms = ms;
-  if (ctx->graph_launched) ctx->launches += ctx->sg.body_launches * h.nfev;      // the WHILE node ran the body once per evaluation
+  if (ctx->graph_launched) ctx->launches += ctx->sg.body_launches * (h.nfev + h.relins);      // the WHILE node ran the body once per evaluation and relinearisation
+  ctx->last_alpha_iters = h.alpha_iters;
   result->kernel_launches = ctx->launches; result->chol_retries = h.chol_fail;
   return MCBA_OK;
 }

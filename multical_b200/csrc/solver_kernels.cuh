@@ -24,6 +24,11 @@ struct SolverState {
   // device-resident loop (lm_kernel.cuh)
   int pending, step_parts, nlog, pad_;       // a trial state waits for its acceptance test | per-CTA step records | rows logged
   double step2_s, xn2_s, agg;                // shared (replicated) parts of ||step||^2 and ||x||^2 of the pending trial; g_h^T A g_h
+  // tr_solver='exact' (solve_lsq_trust_region): the Levenberg-Marquardt parameter carried from trial to trial, the bracket of the
+  // current trial's search, whether the probe factorisation at alpha = 0 found A nonsingular; a rejected trial relinearises the
+  // current point first (relin); totals of the alpha iterations and of those relinearisations
+  double tr_alpha, alpha_lo, alpha_hi;
+  int full_rank, relin, alpha_iters, relins;
 };
 
 // ---- NVLink peer-memory exchange of k_lm (lm_kernel.cuh LmPeer): layout of the per-rank buffers
@@ -231,8 +236,45 @@ __device__ inline void accept_compute(SolverState* st, double cost_new, double s
   int status = -99;
   if (ft && xt) status = 4; else if (ft) status = 2; else if (xt) status = 3;
   st->status = status;
-  if (status == -99) st->Delta = Dn;
+  if (status == -99) { st->tr_alpha *= st->Delta / Dn; st->Delta = Dn; }      // (tr_alpha: exact mode only, trf.py `alpha *= Delta / Delta_new`)
   st->accepted = actual > 0.0;
+}
+
+// ---- tr_solver='exact': the scalar part of common.py solve_lsq_trust_region.  With p(alpha) = -(A + alpha I)^-1 g_h the kernel supplies
+// ||p||^2 and p^T (A + alpha I)^-1 p, which give phi = ||p|| - Delta and phi' = -p^T (A + alpha I)^-1 p / ||p|| (phi_and_derivative).
+constexpr int EXACT_MAX_ITER = 10;
+constexpr double EXACT_RTOL = 1e-2;
+
+// the Gauss-Newton step was not taken: the bracket [alpha_lo, alpha_hi] and the first alpha (pn2_0, ppq_0: the probe at alpha = 0)
+__device__ inline void exact_begin(SolverState* st, double pn2_0, double ppq_0) {
+  st->alpha_hi = st->gh_norm / st->Delta;
+  if (st->full_rank) {
+    const double pn = sqrt(pn2_0), phi = pn - st->Delta, dphi = -ppq_0 / pn;
+    st->alpha_lo = -phi / dphi;
+  } else {
+    st->alpha_lo = 0.0;
+    if (st->tr_alpha == 0.0) st->tr_alpha = fmax(1e-3 * st->alpha_hi, sqrt(st->alpha_lo * st->alpha_hi));
+  }
+}
+// top of an iteration: an alpha outside the bracket is reset into it
+__device__ inline void exact_reset(SolverState* st) {
+  if (st->tr_alpha < st->alpha_lo || st->tr_alpha > st->alpha_hi) st->tr_alpha = fmax(1e-3 * st->alpha_hi, sqrt(st->alpha_lo * st->alpha_hi));
+}
+// one Newton step on phi at tr_alpha; true when |phi| < rtol Delta (the search ends)
+__device__ inline bool exact_newton(SolverState* st, double pn2, double ppq) {
+  const double pn = sqrt(pn2), phi = pn - st->Delta, dphi = -ppq / pn;
+  if (phi < 0.0) st->alpha_hi = st->tr_alpha;
+  const double ratio = phi / dphi;
+  st->alpha_lo = fmax(st->alpha_lo, st->tr_alpha - ratio);
+  st->tr_alpha -= (phi + st->Delta) * ratio / st->Delta;
+  return fabs(phi) < EXACT_RTOL * st->Delta;
+}
+// the step step_h = beta gn, gn = (A + alpha I)^-1 g_h: predicted reduction -(0.5 step_h^T A step_h + g_h^T step_h) from the quadratic
+// forms of gn (ann = gn^T A gn, dot = g_h . gn)
+__device__ inline void exact_step(SolverState* st, double beta, double gn_norm, double ann, double dot) {
+  st->alpha = 0.0; st->beta = beta;
+  st->step_h_norm = fabs(beta) * gn_norm;
+  st->predicted = -(0.5 * beta * beta * ann + beta * dot);
 }
 
 }  // namespace mcba

@@ -559,19 +559,27 @@ class Engine:
     return e[:self.N]
 
   # ---- the solve --------------------------------------------------------------------------------
-  def solve(self, ftol=1e-8, xtol=1e-8, gtol=1e-8, f_scale=1.0, max_nfev=100, loss="linear"):
+  def solve(self, ftol=1e-8, xtol=1e-8, gtol=1e-8, f_scale=1.0, max_nfev=100, loss="linear", tr_solver="lsmr"):
+    """tr_solver: "lsmr" (default) the Gauss-Newton direction and the step in the 2-D subspace span{g, gn}, as scipy's trf with
+    tr_solver='lsmr' but with the direction solved exactly; "exact" the full trust-region subproblem, scipy's tr_solver='exact'
+    (one rank only: NotImplementedError on several)."""
     if loss not in nat.LOSS_IDS:
       raise ValueError(f"`loss` must be one of {list(nat.LOSS_IDS)} or a callable.")
+    if tr_solver not in nat.TR_SOLVERS:
+      raise ValueError(f"`tr_solver` must be one of {list(nat.TR_SOLVERS)}.")
+    self._ck(self.lib.mcba_set_trust_region(self.h, nat.TR_SOLVERS[tr_solver]))
     opts = nat.SolveOpts(ftol, xtol, gtol, f_scale, int(max_nfev), nat.LOSS_IDS[loss])
     res = nat.SolveResult()
     cap = int(max_nfev) + 2
     log = (nat.LogRow * cap)()
     self._ck(self.lib.mcba_solve(self.h, C.byref(opts), C.byref(res), log, cap))
     rows = [(r.iteration, r.nfev, r.cost, r.cost_reduction, r.step_norm, r.optimality) for r in log[:res.n_log]]
+    alpha_iterations = C.c_int32()
+    self._ck(self.lib.mcba_last_alpha_iterations(self.h, C.byref(alpha_iterations)))
     return SolveInfo(cost=res.cost, initial_cost=res.initial_cost, optimality=res.optimality, nfev=res.nfev,
                      njev=res.njev, status=res.status, message=nat.STATUS_MESSAGES.get(res.status, ""),
                      device_ms=res.device_ms, kernel_launches=res.kernel_launches, log=rows,
-                     chol_retries=res.chol_retries)
+                     chol_retries=res.chol_retries, alpha_iterations=alpha_iterations.value)
 
   # ---- measurement hooks ------------------------------------------------------------------------
   def bench_launch(self, which, repeats=1):

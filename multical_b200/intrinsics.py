@@ -201,7 +201,8 @@ def calibrate_views(boards, cam_views, image_sizes, model="standard", fix_aspect
   """One calibrateCameraExtended (model "fisheye": one cv2.fisheye.calibrate) for each camera's list of views (calibration_points
   entries, any order): returns per camera a struct of the intrinsics [fx fy cx cy skew dist...], the views' rtvecs (board wrt camera),
   per-view RMS, total RMS, K0 and the solve summary.  camera_ids: how errors name the cameras (default: their position in cam_views).
-  fixed: bool[5+nd], the intrinsics held at K0's values (fixed_of_flags; None: all free)."""
+  fixed: bool[5+nd], the intrinsics held at K0's values (fixed_of_flags; None: all free).  solve_opts go to Engine.solve: ftol, xtol,
+  gtol, max_nfev, and tr_solver ("lsmr" or "exact")."""
   eng = engine or intrinsics_engine()
   opts = dict(ftol=1e-10, xtol=1e-10, gtol=1e-10, max_nfev=100)
   opts.update(solve_opts)

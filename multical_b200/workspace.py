@@ -35,23 +35,25 @@ def calibrate_single(boards, detected_points, image_sizes, camera_model, intrins
 
 
 def calibrate(calib: Calibration, camera_poses=True, motion=True, board_poses=True, cameras=False, boards=False,
-              loss="linear", tolerance=1e-4, num_adjustments=3, quantile=0.75, auto_scale=None, outlier_threshold=5.0) -> Calibration:
-  """workspace.py:228-247: same arguments, defaults and order of operations."""
+              loss="linear", tolerance=1e-4, num_adjustments=3, quantile=0.75, auto_scale=None, outlier_threshold=5.0,
+              tr_solver="lsmr") -> Calibration:
+  """workspace.py:228-247: same arguments, defaults and order of operations; tr_solver as Calibration.bundle_adjust."""
   calib = calib.enable(cameras=cameras, boards=boards, camera_poses=camera_poses, motion=motion, board_poses=board_poses)
   return calib.adjust_outliers(
-    loss=loss, tolerance=tolerance, num_adjustments=num_adjustments,
+    loss=loss, tolerance=tolerance, num_adjustments=num_adjustments, tr_solver=tr_solver,
     select_outliers=select_threshold(quantile=quantile, factor=outlier_threshold),
     select_scale=select_threshold(quantile=quantile, factor=auto_scale) if auto_scale is not None else None)
 
 
 def optimize(calib: Calibration, iter=3, loss="linear", outlier_quantile=0.75, outlier_threshold=5.0, auto_scale=None,
-             fix_intrinsic=False, fix_camera_poses=False, fix_board_poses=False, fix_motion=False, adjust_board=False) -> Calibration:
+             fix_intrinsic=False, fix_camera_poses=False, fix_board_poses=False, fix_motion=False, adjust_board=False,
+             tr_solver="lsmr") -> Calibration:
   """config/workspace.py:47-58 with the fields of OptimizerOpts (config/arguments.py:53-69) as keyword arguments.  Like the reference's
   `optimize`, the `iter` option is NOT forwarded: Workspace.calibrate runs its own default of 3 adjustments."""
   del iter
   return calibrate(calib, loss=loss, boards=adjust_board, cameras=not fix_intrinsic, camera_poses=not fix_camera_poses,
                    board_poses=not fix_board_poses, motion=not fix_motion, auto_scale=auto_scale,
-                   outlier_threshold=outlier_threshold, quantile=outlier_quantile)
+                   outlier_threshold=outlier_threshold, quantile=outlier_quantile, tr_solver=tr_solver)
 
 
 def pose_table(point_table, boards, cameras, exclude_bad_poses=True, pose_error_limit=1.0):
