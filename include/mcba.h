@@ -29,6 +29,7 @@ extern "C" {
 
 typedef struct mcba_ctx mcba_ctx;
 
+/* MCBA_ERR_CUDA: a CUDA call failed, or a host allocation did (the message says which) */
 enum { MCBA_OK = 0, MCBA_ERR_ARG = 1, MCBA_ERR_CUDA = 2, MCBA_ERR_STATE = 3, MCBA_ERR_NCCL = 4,
        MCBA_ERR_NONFINITE = 5, MCBA_ERR_UNSUPPORTED = 6,
        MCBA_ERR_DEGENERATE = 7 /* input too degenerate for the estimate asked for (mcba_hand_eye_vote) */ };

@@ -13,6 +13,8 @@
 #include <functional>
 #include <type_traits>
 #include <memory>
+#include <new>
+#include <exception>
 #include <vector>
 
 #include "../../include/mcba.h"
@@ -34,6 +36,10 @@ using namespace mcba;
 namespace {
 
 thread_local std::string g_create_error;
+
+// A refusal or a CUDA error on the host: thrown by CK / CKL / REQUIRE, turned into a status and mcba_last_error's text only where an
+// entry point returns (guarded)
+struct Failure { int code; std::string msg; };
 
 template <typename T>
 struct DevBuf {
@@ -212,21 +218,37 @@ struct mcba_ctx {
 #define CK(call)                                                                                   \
   do {                                                                                             \
     cudaError_t e_ = (call);                                                                       \
-    if (e_ != cudaSuccess) {                                                                       \
-      ctx->err = std::string(#call) + ": " + cudaGetErrorString(e_);                               \
-      return MCBA_ERR_CUDA;                                                                        \
-    }                                                                                              \
+    if (e_ != cudaSuccess) throw Failure{MCBA_ERR_CUDA, std::string(#call) + ": " + cudaGetErrorString(e_)}; \
   } while (0)
 #define CKL()                                                                                      \
   do {                                                                                             \
     ctx->launches++;                                                                               \
     cudaError_t e_ = cudaGetLastError();                                                           \
-    if (e_ != cudaSuccess) { ctx->err = std::string("kernel launch: ") + cudaGetErrorString(e_); return MCBA_ERR_CUDA; } \
+    if (e_ != cudaSuccess) throw Failure{MCBA_ERR_CUDA, std::string("kernel launch: ") + cudaGetErrorString(e_)}; \
   } while (0)
+// a macro, not a function: the message is built only when the check fails (it runs inside per-element loops)
 #define REQUIRE(cond, code, msg)                                                                   \
-  do { if (!(cond)) { ctx->err = msg; return code; } } while (0)
+  do { if (!(cond)) throw Failure{code, msg}; } while (0)
 
 namespace {
+
+// body() with whatever it throws as a status, its message in err: every C++ exception stops here, none crosses the C ABI
+template <typename Fn>
+int guarded(std::string& err, Fn&& body) {
+  try { body(); return MCBA_OK; }
+  catch (const Failure& f) { err = f.msg; return f.code; }
+  catch (const std::bad_alloc&) { err = "host allocation failed (std::bad_alloc)"; }
+  catch (const std::exception& e) { err = std::string("host exception: ") + e.what(); }
+  catch (...) { err = "unknown host exception"; }
+  return MCBA_ERR_CUDA;
+}
+
+// the boundary of an entry point: a null context, then the context's device, then the body
+template <typename Fn>
+int api(mcba_ctx* ctx, Fn&& body) {
+  if (!ctx) return MCBA_ERR_ARG;
+  return guarded(ctx->err, [&] { CK(cudaSetDevice(ctx->device)); body(); });
+}
 
 // full parameter state -> block-structured vector x (internal order)
 __global__ void k_gather_params(DeviceProblem p, double* x, const double* cam_rt, const double* board_rt, const double* frame_rt, const double* intr) {
@@ -250,7 +272,7 @@ __global__ void k_trial_state(DeviceProblem p, const double* x, double* trial, i
 int trial_items(const DeviceProblem& P) { return P.C + P.B + P.F * P.npf + P.C + P.B * P.P + 2; }
 
 template <int MODE>
-int launch_views(mcba_ctx* ctx, const DeviceProblem& P, const ViewKernelArgs& a) {
+void launch_views(mcba_ctx* ctx, const DeviceProblem& P, const ViewKernelArgs& a) {
   const int blocks = std::max(1, std::min((P.V + VIEW_WARPS - 1) / VIEW_WARPS, ctx->num_sms * 8));
   const int th = VIEW_WARPS * 32;
   cudaStream_t s = ctx->stream;
@@ -259,7 +281,6 @@ int launch_views(mcba_ctx* ctx, const DeviceProblem& P, const ViewKernelArgs& a)
     k_views<MODEL, MODE, ROLL><<<blocks, th, 0, s>>>(P, a);
   });
   CKL();
-  return MCBA_OK;
 }
 
 // ---------------------------------------------------------------- linearisation (linearize.cuh)
@@ -272,8 +293,8 @@ size_t lin_smem_for(const DeviceProblem& P, int warps) {
   return bytes;
 }
 // one launch: H_ff, g_f, W_f, frame costs and the per-CTA records of the shared blocks at the (trial or current) state
-int launch_linearize(mcba_ctx* ctx, const DeviceProblem& P, int loss, double f_scale) {
-  if (P.F == 0) return MCBA_OK;
+void launch_linearize(mcba_ctx* ctx, const DeviceProblem& P, int loss, double f_scale) {
+  if (P.F == 0) return;
   LinArgs a{}; a.loss = loss; a.f_scale = f_scale; a.split = ctx->lin_split;
   a.Hff = ctx->Hff.p; a.g = ctx->g.p; a.W = ctx->W.p; a.spart = ctx->spart.p; a.frame_cost = ctx->frame_cost.p;
   const size_t sm = lin_smem_for(P, ctx->lin_warps);
@@ -284,10 +305,9 @@ int launch_linearize(mcba_ctx* ctx, const DeviceProblem& P, int loss, double f_s
     k_linearize<MODEL, ROLL><<<ctx->lin_grid, th, sm, s>>>(P, a);
   });
   CKL();
-  return MCBA_OK;
 }
 // per-CTA records -> H_ss, g_s, cost (stores, fixed summation order)
-int launch_reduce_shared(mcba_ctx* ctx, const DeviceProblem& P) {
+void launch_reduce_shared(mcba_ctx* ctx, const DeviceProblem& P) {
   ReduceArgs r{}; r.spart = ctx->spart.p; r.nparts = P.F > 0 ? ctx->lin_grid : 0; r.Hss = ctx->Hss.p; r.g = ctx->g.p; r.bpart = ctx->bpart.p;
   r.frame_cost = ctx->frame_cost.p; r.F = P.F; r.cost_out = ctx->lin_cost.p; r.cam_counter = ctx->cam_counter.p; r.sred = ctx->sred.p;
   const size_t sm = sizeof(double) * reduce_smem_doubles(P.T, P.D);
@@ -295,7 +315,6 @@ int launch_reduce_shared(mcba_ctx* ctx, const DeviceProblem& P) {
   if (P.motion == MOTION_ROLLING) k_reduce_shared<2><<<grid, RED_THREADS, sm, ctx->stream>>>(P, r);
   else k_reduce_shared<1><<<grid, RED_THREADS, sm, ctx->stream>>>(P, r);
   CKL();
-  return MCBA_OK;
 }
 
 // DeviceProblem view whose parameter pointers are the trial state
@@ -305,25 +324,24 @@ DeviceProblem with_state(const mcba_ctx* ctx, bool trial) {
   return P;
 }
 
-int prepare(mcba_ctx* ctx, const DeviceProblem& P) {
+void prepare(mcba_ctx* ctx, const DeviceProblem& P) {
   const int np = P.C + P.B + P.F * P.npf + (P.motion == MOTION_HAND_EYE ? 2 : 0);
   k_prepare<<<(np + 127) / 128, 128, 0, ctx->stream>>>(P, P.cam_rt, P.board_rt, P.frame_rt);
   CKL();
-  return MCBA_OK;
 }
 
 // The normal equations and the cost at the (trial or current) state, whose pose tables must already describe it: k_linearize, its per-CTA
 // records -> H_ss, g_s, cost (k_reduce_shared), then boards=True: the board-point blocks on top (k_point_blocks), then hand-eye: the
 // hand-eye rows and columns from the frame blocks (k_fold_hand_eye, last: it reads the point rows of W_f)
-int linearize(mcba_ctx* ctx, int loss, double f_scale, bool trial = false) {
+void linearize(mcba_ctx* ctx, int loss, double f_scale, bool trial = false) {
   DeviceProblem P = with_state(ctx, trial);
   cudaStream_t s = ctx->stream;
-  int r = launch_linearize(ctx, P, loss, f_scale); if (r) return r;
+  launch_linearize(ctx, P, loss, f_scale);
   if (P.off_pt >= 0) {         // k_point_blocks adds the point rows / columns (atomics): they start at zero
     CK(cudaMemsetAsync(ctx->Hss.p, 0, sizeof(double) * (size_t)P.n_s * P.n_s, s));
     CK(cudaMemsetAsync(ctx->g.p, 0, sizeof(double) * (size_t)std::max(P.n_s, 1), s));
   }
-  r = launch_reduce_shared(ctx, P); if (r) return r;
+  launch_reduce_shared(ctx, P);
   if (P.off_pt >= 0 && P.V > 0) {
     ViewKernelArgs a{}; a.loss = loss; a.f_scale = f_scale;
     const int blocks = std::max(1, std::min((P.V + VIEW_WARPS - 1) / VIEW_WARPS, ctx->num_sms * 8));
@@ -337,37 +355,33 @@ int linearize(mcba_ctx* ctx, int loss, double f_scale, bool trial = false) {
     k_fold_hand_eye<<<P.n_s + 1, FOLD_THREADS, 0, s>>>(P, ctx->Hff.p, ctx->W.p, ctx->Hss.p, ctx->g.p);
     CKL();
   }
-  return MCBA_OK;
 }
 
 // cost at the (trial or current) state -> eval_cost
-int trial_cost(mcba_ctx* ctx, int loss, double f_scale, bool trial) {
+void trial_cost(mcba_ctx* ctx, int loss, double f_scale, bool trial) {
   DeviceProblem P = with_state(ctx, trial);
   ViewKernelArgs a{}; a.loss = loss; a.f_scale = f_scale; a.view_cost = ctx->view_cost.p;
-  int r = launch_views<MODE_COST>(ctx, P, a); if (r) return r;
+  launch_views<MODE_COST>(ctx, P, a);
   k_sum_partials<<<1, 1024, 0, ctx->stream>>>(ctx->view_cost.p, P.V, 1, 1, ctx->eval_cost.p); CKL();
-  return MCBA_OK;
 }
 
 // ---------------------------------------------------------------- the device-resident trust-region loop (lm_kernel.cuh)
 // trial parameter state := current state
-int copy_state_to_trial(mcba_ctx* ctx) {
+void copy_state_to_trial(mcba_ctx* ctx) {
   CK(cudaMemcpyAsync(ctx->trial.p, ctx->params.p, sizeof(double) * ctx->layout.len, cudaMemcpyDeviceToDevice, ctx->stream));
-  return MCBA_OK;
 }
 
 // push vector x (internal order) into the trial state and rebuild the pose tables, as k_lm builds its trial states; trial == false:
 // the trial state then becomes the current one.  The current state is only read, never updated in place: the derived hand-eye frame
 // poses read he_rt while other items write its new value.
-int set_state_from_x(mcba_ctx* ctx, const double* x, bool trial) {
+void set_state_from_x(mcba_ctx* ctx, const double* x, bool trial) {
   // make_trial_item writes every entry but he_rt of a problem without hand-eye and frame_rt of a hand-eye problem (derived frames):
   // those come from the copy
-  int r = copy_state_to_trial(ctx); if (r) return r;
+  copy_state_to_trial(ctx);
   const int items = trial_items(ctx->P);
   k_trial_state<<<(items + 127) / 128, 128, 0, ctx->stream>>>(ctx->P, x, ctx->trial.p, items);
   CKL();
   if (!trial) CK(cudaMemcpyAsync(ctx->params.p, ctx->trial.p, sizeof(double) * ctx->layout.len, cudaMemcpyDeviceToDevice, ctx->stream));
-  return MCBA_OK;
 }
 
 LmArgs make_lm_args(mcba_ctx* ctx, int log_cap) {
@@ -391,7 +405,7 @@ LmArgs make_lm_args(mcba_ctx* ctx, int log_cap) {
   return a;
 }
 
-int launch_lm(mcba_ctx* ctx, const LmArgs& a) {
+void launch_lm(mcba_ctx* ctx, const LmArgs& a) {
   const size_t sm = sizeof(double) * lm_smem_doubles(ctx->P.n_s, ctx->P.fb);
   LmArgs args = a;
 #ifdef MCBA_SIMT_BUILD
@@ -409,16 +423,15 @@ int launch_lm(mcba_ctx* ctx, const LmArgs& a) {
   CK(cudaLaunchCooperativeKernel(fn, dim3(ctx->lm_grid), dim3(LM_THREADS), params, sm, ctx->stream));
   ctx->launches++;
 #endif
-  return MCBA_OK;
 }
 
 // one pass of the loop body: linearise the trial state, then accept / solve / step (k_lm)
-int lm_body(mcba_ctx* ctx, int loss, double f_scale, const LmArgs& a) {
-  int r = linearize(ctx, loss, f_scale, true); if (r) return r;
-  return launch_lm(ctx, a);
+void lm_body(mcba_ctx* ctx, int loss, double f_scale, const LmArgs& a) {
+  linearize(ctx, loss, f_scale, true);
+  launch_lm(ctx, a);
 }
 
-int run_lm_loop(mcba_ctx* ctx, int loss, double f_scale, int log_cap) {
+void run_lm_loop(mcba_ctx* ctx, int loss, double f_scale, int log_cap) {
   cudaStream_t s = ctx->stream;
   LmArgs a = make_lm_args(ctx, log_cap);
 #ifndef MCBA_SIMT_BUILD
@@ -446,11 +459,14 @@ int run_lm_loop(mcba_ctx* ctx, int loss, double f_scale, int log_cap) {
       CK(cudaStreamSynchronize(s));
       CK(cudaStreamBeginCaptureToGraph(cap, body, nullptr, nullptr, 0, cudaStreamCaptureModeRelaxed));
       ctx->stream = cap;
-      int r = lm_body(ctx, loss, f_scale, a);
-      ctx->stream = s;
-      cudaError_t e = cudaStreamEndCapture(cap, nullptr);
-      if (r) return r;
-      if (e != cudaSuccess) { ctx->err = std::string("graph capture of the loop body: ") + cudaGetErrorString(e); return MCBA_ERR_CUDA; }
+      struct Capture {       // on every path, a throw from the body included: the context's stream back, the capture ended
+        mcba_ctx* ctx; cudaStream_t s, cap; bool open = true;
+        cudaError_t end() { open = false; ctx->stream = s; return cudaStreamEndCapture(cap, nullptr); }
+        ~Capture() { if (open) end(); }
+      } capture{ctx, s, cap};
+      lm_body(ctx, loss, f_scale, a);
+      const cudaError_t e = capture.end();
+      REQUIRE(e == cudaSuccess, MCBA_ERR_CUDA, std::string("graph capture of the loop body: ") + cudaGetErrorString(e));
       CK(cudaGraphInstantiate(&ctx->sg.exec, g, 0));
       ctx->sg.key = key; ctx->sg.stream = s;
       ctx->sg.body_launches = ctx->launches - before;
@@ -458,14 +474,14 @@ int run_lm_loop(mcba_ctx* ctx, int loss, double f_scale, int log_cap) {
     ctx->launches = before;
     CK(cudaGraphLaunch(ctx->sg.exec, s));
     ctx->graph_launched = true;
-    return MCBA_OK;
+    return;
   }
 #endif
   // host-driven loop (the SIMT interpreter build; MCBA_GRAPH=0): same kernels, one state read per body
   ctx->graph_launched = false;
   SolverState h{};
   for (int it = 0; it < 2 * (log_cap + 8); it++) {      // (tr_solver='exact': a rejected trial costs a second pass, a relinearisation)
-    int r = lm_body(ctx, loss, f_scale, a); if (r) return r;
+    lm_body(ctx, loss, f_scale, a);
     CK(cudaMemcpyAsync(&h, ctx->state.p, sizeof(h), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
     if (ctx->profiling) {
@@ -478,20 +494,18 @@ int run_lm_loop(mcba_ctx* ctx, int loss, double f_scale, int log_cap) {
     }
     if (h.done) break;
   }
-  return MCBA_OK;
 }
 
-// the current and trial parameter state of `desc` (kept when they already fit: a re-selected table keeps its state); board_pts, if not
-// null, receives where the uploads write the board points
-int alloc_state(mcba_ctx* ctx, const mcba_problem_desc* desc, double** board_pts) {
+// the current and trial parameter state of `desc` (kept when they already fit: a re-selected table keeps its state); returns where the
+// uploads write the board points
+double* alloc_state(mcba_ctx* ctx, const mcba_problem_desc* desc) {
   ctx->layout = state_layout(*desc);
   CK(ctx->params.alloc(ctx->layout.len)); CK(ctx->trial.alloc(ctx->layout.len));
-  if (board_pts) *board_pts = ctx->params.p + ctx->layout.pts;
-  return MCBA_OK;
+  return ctx->params.p + ctx->layout.pts;
 }
 
 // dimensions, variable layout, permutation and every solver buffer that depends on (C,F,B,P,N,V)
-int setup_problem(mcba_ctx* ctx, const mcba_problem_desc* desc, int64_t N, int V, bool keep_state = false) {
+void setup_problem(mcba_ctx* ctx, const mcba_problem_desc* desc, int64_t N, int V, bool keep_state = false) {
   const int C = desc->C, F = desc->F, B = desc->B, Pn = desc->P;
   DeviceProblem& P = ctx->P;
   P = DeviceProblem{};
@@ -532,7 +546,7 @@ int setup_problem(mcba_ctx* ctx, const mcba_problem_desc* desc, int64_t N, int V
   }
 
   const size_t fbs = (size_t)std::max(P.fb, 6);      // doubles per frame in frame_rt and in the per-frame solver blocks
-  { int r = alloc_state(ctx, desc, nullptr); if (r) return r; }
+  alloc_state(ctx, desc);
   CK(ctx->cam_T.alloc(C)); CK(ctx->frame_T.alloc((size_t)std::max(F, 1) * P.npf)); CK(ctx->board_T.alloc(B));
   CK(ctx->img_h.alloc(C)); CK(ctx->he_T.alloc(2)); CK(ctx->arm_T.alloc(std::max(F, 1)));
   // solver buffers
@@ -633,7 +647,6 @@ int setup_problem(mcba_ctx* ctx, const mcba_problem_desc* desc, int64_t N, int V
   set_state_pointers(P, ctx->params.p, ctx->layout);
   P.cam_T = ctx->cam_T.p; P.frame_T = ctx->frame_T.p; P.board_T = ctx->board_T.p;
   P.img_h = ctx->img_h.p; P.he_T = ctx->he_T.p; P.arm_T = ctx->arm_T.p;
-  return MCBA_OK;
 }
 // MCBA_PROF=1: host wall clock at checkpoints of the upload path, on stderr (no synchronisation is added: it times what the host waits for)
 struct UploadClock {
@@ -641,20 +654,19 @@ struct UploadClock {
   explicit UploadClock(bool enabled) : on(enabled), t0(std::chrono::steady_clock::now()) {}
   void mark(const char* what) { if (on) fprintf(stderr, "[upload] %-28s %8.3f ms\n", what, std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count()); }
 };
-int check_desc(mcba_ctx* ctx, const mcba_problem_desc* desc) {
+void check_desc(const mcba_problem_desc* desc) {
   REQUIRE(desc->C > 0 && desc->F >= 0 && desc->B > 0 && desc->P > 0, MCBA_ERR_ARG, "bad problem dimensions");
   REQUIRE(desc->P <= 65535, MCBA_ERR_UNSUPPORTED, "more than 65535 points per board");
   REQUIRE(desc->model >= 0 && desc->model <= 4, MCBA_ERR_ARG, "unknown camera model");
   REQUIRE(!((desc->optimize & MCBA_MOTION_ROLLING) && (desc->optimize & MCBA_MOTION_HAND_EYE)), MCBA_ERR_ARG, "more than one motion model");
   REQUIRE((int64_t)desc->C * desc->F * desc->B * desc->P < ((int64_t)1 << 31), MCBA_ERR_UNSUPPORTED, "more than 2^31 table entries per rank");
-  return MCBA_OK;
 }
 
-// pack the resident dense table (ctx->dense_pts) under a device mask into the frame-major corner arrays the kernels read
-// points_ready: event after which dense_pts holds the observations (they may still be in flight on the copy stream while the views are
-// counted and scanned), or null
-int pack_dense(mcba_ctx* ctx, const mcba_problem_desc* desc, const uint8_t* d_mask, bool keep_state, int64_t* n_corners,
-               const uint8_t* d_view_valid = nullptr, cudaEvent_t points_ready = nullptr, bool points_f32 = false) {
+// pack the resident dense table (ctx->dense_pts) under a device mask into the frame-major corner arrays the kernels read; returns the
+// number of corners.  points_ready: event after which dense_pts holds the observations (they may still be in flight on the copy stream
+// while the views are counted and scanned), or null
+int64_t pack_dense(mcba_ctx* ctx, const mcba_problem_desc* desc, const uint8_t* d_mask, bool keep_state,
+                   const uint8_t* d_view_valid = nullptr, cudaEvent_t points_ready = nullptr, bool points_f32 = false) {
   const int C = desc->C, F = desc->F, B = desc->B, Pn = desc->P;
   const int nv = C * F * B;
   cudaStream_t s = ctx->stream;
@@ -687,13 +699,12 @@ int pack_dense(mcba_ctx* ctx, const mcba_problem_desc* desc, const uint8_t* d_ma
     CK(cudaMemsetAsync(ctx->view_start.p, 0, sizeof(int), s)); CK(cudaMemsetAsync(ctx->frame_view_start.p, 0, sizeof(int) * (F + 1), s));
   }
   clk.mark("pack: scatter issued");
-  { int r = setup_problem(ctx, desc, N, V, keep_state); if (r) return r; }
+  setup_problem(ctx, desc, N, V, keep_state);
   clk.mark("pack: setup_problem done");
   CK(cudaStreamSynchronize(s));
   clk.mark("pack: final synchronise");
-  if (n_corners) *n_corners = N;
   ctx->uploaded = true;
-  return MCBA_OK;
+  return N;
 }
 
 }  // namespace
@@ -706,45 +717,46 @@ int mcba_version(void) { return 100; }
 const char* mcba_last_error(const mcba_ctx* ctx) { return ctx ? ctx->err.c_str() : g_create_error.c_str(); }
 
 int mcba_create(int device, mcba_ctx** out) {
-  if (!out) return MCBA_ERR_ARG;
-  *out = nullptr;
-  int count = 0;
-  cudaError_t e = cudaGetDeviceCount(&count);
-  if (e != cudaSuccess || count == 0) { g_create_error = std::string("no CUDA device: ") + cudaGetErrorString(e); return MCBA_ERR_CUDA; }
-  if (device < 0 || device >= count) { g_create_error = "device ordinal out of range"; return MCBA_ERR_ARG; }
-  e = cudaSetDevice(device);
-  if (e != cudaSuccess) { g_create_error = cudaGetErrorString(e); return MCBA_ERR_CUDA; }
-  cudaDeviceProp prop;
-  e = cudaGetDeviceProperties(&prop, device);
-  if (e != cudaSuccess) { g_create_error = cudaGetErrorString(e); return MCBA_ERR_CUDA; }
-  if (prop.major != 9 || prop.minor != 0) { g_create_error = "libmcba is built for sm_90a only (found sm_" + std::to_string(prop.major * 10 + prop.minor) + ")"; return MCBA_ERR_CUDA; }
-  mcba_ctx* ctx = new mcba_ctx();
-  ctx->device = device;
-  ctx->num_sms = prop.multiProcessorCount;
-  if (cudaStreamCreateWithFlags(&ctx->own_stream, cudaStreamNonBlocking) != cudaSuccess) { g_create_error = "cudaStreamCreate failed"; delete ctx; return MCBA_ERR_CUDA; }
-  ctx->stream = ctx->own_stream;
-  { const char* e = getenv("MCBA_GRAPH"); if (e && std::string(e) == "0") ctx->use_graph = false; }
-  { const char* e = getenv("MCBA_PROF"); if (e && std::string(e) == "1") { ctx->profiling = true; ctx->use_graph = false; } }
-  for (int model = MODEL_STANDARD; model <= MODEL_TILTED; model++)
-    for (bool roll : {false, true})
-      with_model(model, roll, [](auto M, auto R) {
-        cudaFuncSetAttribute(k_linearize<decltype(M)::value, decltype(R)::value>, cudaFuncAttributeMaxDynamicSharedMemorySize, LIN_SMEM_MAX);
+  return guarded(g_create_error, [&] {
+    REQUIRE(out, MCBA_ERR_ARG, "null output pointer");
+    *out = nullptr;
+    int count = 0;
+    cudaError_t e = cudaGetDeviceCount(&count);
+    REQUIRE(e == cudaSuccess && count > 0, MCBA_ERR_CUDA, std::string("no CUDA device: ") + cudaGetErrorString(e));
+    REQUIRE(device >= 0 && device < count, MCBA_ERR_ARG, "device ordinal out of range");
+    e = cudaSetDevice(device);
+    REQUIRE(e == cudaSuccess, MCBA_ERR_CUDA, cudaGetErrorString(e));
+    cudaDeviceProp prop;
+    e = cudaGetDeviceProperties(&prop, device);
+    REQUIRE(e == cudaSuccess, MCBA_ERR_CUDA, cudaGetErrorString(e));
+    REQUIRE(prop.major == 9 && prop.minor == 0, MCBA_ERR_CUDA, "libmcba is built for sm_90a only (found sm_" + std::to_string(prop.major * 10 + prop.minor) + ")");
+    std::unique_ptr<mcba_ctx> ctx(new mcba_ctx());
+    ctx->device = device;
+    ctx->num_sms = prop.multiProcessorCount;
+    REQUIRE(cudaStreamCreateWithFlags(&ctx->own_stream, cudaStreamNonBlocking) == cudaSuccess, MCBA_ERR_CUDA, "cudaStreamCreate failed");
+    ctx->stream = ctx->own_stream;
+    { const char* e = getenv("MCBA_GRAPH"); if (e && std::string(e) == "0") ctx->use_graph = false; }
+    { const char* e = getenv("MCBA_PROF"); if (e && std::string(e) == "1") { ctx->profiling = true; ctx->use_graph = false; } }
+    for (int model = MODEL_STANDARD; model <= MODEL_TILTED; model++)
+      for (bool roll : {false, true})
+        with_model(model, roll, [](auto M, auto R) {
+          cudaFuncSetAttribute(k_linearize<decltype(M)::value, decltype(R)::value>, cudaFuncAttributeMaxDynamicSharedMemorySize, LIN_SMEM_MAX);
+        });
+    cudaFuncSetAttribute(k_reduce_shared<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaFuncSetAttribute(k_reduce_shared<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaFuncSetAttribute(k_lm<6, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaFuncSetAttribute(k_lm<12, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaFuncSetAttribute(k_lm<6, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaFuncSetAttribute(k_lm<12, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaFuncSetAttribute(k_pose_align<PI_SMALL_THREADS, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, PI_SMALL_MAX * PI_ROW_BYTES);
+    for (int model = MODEL_STANDARD; model <= MODEL_TILTED; model++)
+      with_model(model, false, [](auto M, auto) {
+        cudaFuncSetAttribute(k_rectify_map<decltype(M)::value>, cudaFuncAttributeMaxDynamicSharedMemorySize, RECT_SMEM_MAX);
+        cudaFuncSetAttribute(k_triangulate<decltype(M)::value, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             (int)tri_smem((MCBA_TRI_MAX_CAMERAS + 31) / 32));
       });
-  cudaFuncSetAttribute(k_reduce_shared<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-  cudaFuncSetAttribute(k_reduce_shared<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-  cudaFuncSetAttribute(k_lm<6, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-  cudaFuncSetAttribute(k_lm<12, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-  cudaFuncSetAttribute(k_lm<6, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-  cudaFuncSetAttribute(k_lm<12, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-  cudaFuncSetAttribute(k_pose_align<PI_SMALL_THREADS, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, PI_SMALL_MAX * PI_ROW_BYTES);
-  for (int model = MODEL_STANDARD; model <= MODEL_TILTED; model++)
-    with_model(model, false, [](auto M, auto) {
-      cudaFuncSetAttribute(k_rectify_map<decltype(M)::value>, cudaFuncAttributeMaxDynamicSharedMemorySize, RECT_SMEM_MAX);
-      cudaFuncSetAttribute(k_triangulate<decltype(M)::value, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                           (int)tri_smem((MCBA_TRI_MAX_CAMERAS + 31) / 32));
-    });
-  *out = ctx;
-  return MCBA_OK;
+    *out = ctx.release();
+  });
 }
 
 void mcba_destroy(mcba_ctx* ctx) {
@@ -773,63 +785,64 @@ void mcba_destroy(mcba_ctx* ctx) {
 }
 
 int mcba_set_stream(mcba_ctx* ctx, void* stream) {
-  if (!ctx) return MCBA_ERR_ARG;
-  CK(cudaSetDevice(ctx->device));
-  CK(cudaStreamSynchronize(ctx->stream));          // nothing of ours may still be in flight on the stream we leave
-  ctx->stream = (cudaStream_t)stream;              // NULL is the legacy default stream (what torch reports as stream 0)
-  return MCBA_OK;
+  return api(ctx, [&] {
+    CK(cudaStreamSynchronize(ctx->stream));          // nothing of ours may still be in flight on the stream we leave
+    ctx->stream = (cudaStream_t)stream;              // NULL is the legacy default stream (what torch reports as stream 0)
+  });
 }
 
 int mcba_comm_unique_id(mcba_ctx* ctx, char out_id[128]) {
   // kept for the shape of the API (rank 0 makes an id, the host broadcasts it): the exchanges of a solve run inside the solver kernel over
   // NVLink peer mappings (mcba_peer_export / mcba_peer_import), there is no library communicator to create
-  if (!ctx || !out_id) return MCBA_ERR_ARG;
-  memset(out_id, 0, 128);
-  snprintf(out_id, 128, "mcba-peer-group");
-  return MCBA_OK;
+  return api(ctx, [&] {
+    REQUIRE(out_id, MCBA_ERR_ARG, "null id buffer");
+    memset(out_id, 0, 128);
+    snprintf(out_id, 128, "mcba-peer-group");
+  });
 }
 
 int mcba_comm_init(mcba_ctx* ctx, const char id_[128], int rank, int world) {
-  if (!ctx || !id_) return MCBA_ERR_ARG;
-  REQUIRE(world >= 1 && world <= PEER_MAX_WORLD && rank >= 0 && rank < world, MCBA_ERR_ARG, "bad rank/world (1..16 ranks)");
-  ctx->rank = rank; ctx->world = world; ctx->peer_ready = false;
-  return MCBA_OK;
+  return api(ctx, [&] {
+    REQUIRE(id_, MCBA_ERR_ARG, "null id");
+    REQUIRE(world >= 1 && world <= PEER_MAX_WORLD && rank >= 0 && rank < world, MCBA_ERR_ARG, "bad rank/world (1..16 ranks)");
+    ctx->rank = rank; ctx->world = world; ctx->peer_ready = false;
+  });
 }
 
 int mcba_peer_export(mcba_ctx* ctx, int64_t cap_doubles, char out_handle[64]) {
-  if (!ctx || !out_handle) return MCBA_ERR_ARG;
-  REQUIRE(ctx->world > 1 && ctx->world <= PEER_MAX_WORLD, MCBA_ERR_STATE, "peer buffers need an initialised communicator with 2..16 ranks");
-  REQUIRE(cap_doubles > 0 && cap_doubles < ((int64_t)1 << 30), MCBA_ERR_ARG, "bad peer slot capacity");
-  REQUIRE(sizeof(cudaIpcMemHandle_t) == 64, MCBA_ERR_UNSUPPORTED, "unexpected cudaIpcMemHandle_t size");
-  CK(cudaSetDevice(ctx->device));
-  if (ctx->peer_own) { cudaFree(ctx->peer_own); ctx->peer_own = nullptr; }
-  ctx->peer_ready = false; ctx->peer_cap = (int)cap_doubles;
-  const size_t bytes = peer_buffer_doubles(ctx->world, ctx->peer_cap) * sizeof(double);
-  CK(cudaMalloc(&ctx->peer_own, bytes));
-  CK(cudaMemset(ctx->peer_own, 0, bytes));
-  CK(cudaDeviceSynchronize());
-  cudaIpcMemHandle_t h;
-  CK(cudaIpcGetMemHandle(&h, ctx->peer_own));
-  memcpy(out_handle, &h, 64);
-  return MCBA_OK;
+  return api(ctx, [&] {
+    REQUIRE(out_handle, MCBA_ERR_ARG, "null handle buffer");
+    REQUIRE(ctx->world > 1 && ctx->world <= PEER_MAX_WORLD, MCBA_ERR_STATE, "peer buffers need an initialised communicator with 2..16 ranks");
+    REQUIRE(cap_doubles > 0 && cap_doubles < ((int64_t)1 << 30), MCBA_ERR_ARG, "bad peer slot capacity");
+    REQUIRE(sizeof(cudaIpcMemHandle_t) == 64, MCBA_ERR_UNSUPPORTED, "unexpected cudaIpcMemHandle_t size");
+    if (ctx->peer_own) { cudaFree(ctx->peer_own); ctx->peer_own = nullptr; }
+    ctx->peer_ready = false; ctx->peer_cap = (int)cap_doubles;
+    const size_t bytes = peer_buffer_doubles(ctx->world, ctx->peer_cap) * sizeof(double);
+    CK(cudaMalloc(&ctx->peer_own, bytes));
+    CK(cudaMemset(ctx->peer_own, 0, bytes));
+    CK(cudaDeviceSynchronize());
+    cudaIpcMemHandle_t h;
+    CK(cudaIpcGetMemHandle(&h, ctx->peer_own));
+    memcpy(out_handle, &h, 64);
+  });
 }
 
 int mcba_peer_import(mcba_ctx* ctx, const char* handles /* world x 64 bytes, rank order */) {
-  if (!ctx || !handles) return MCBA_ERR_ARG;
-  REQUIRE(ctx->peer_own != nullptr, MCBA_ERR_STATE, "mcba_peer_export has not been called");
-  CK(cudaSetDevice(ctx->device));
-  for (int r = 0; r < ctx->world; r++) {
-    if (r == ctx->rank) { ctx->peer_base[r] = ctx->peer_own; continue; }
-    cudaIpcMemHandle_t h; memcpy(&h, handles + (size_t)r * 64, 64);
-    void* p = nullptr;
-    CK(cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess));
-    ctx->peer_base[r] = (double*)p; ctx->peer_opened.push_back(p);
-  }
-  // sequence number of the in-kernel exchanges (lm_kernel.cuh): starts at zero on every rank, advanced on the device
-  CK(ctx->peer_seq_dev.alloc(1));
-  CK(cudaMemset(ctx->peer_seq_dev.p, 0, sizeof(unsigned long long)));
-  ctx->peer_ready = true;
-  return MCBA_OK;
+  return api(ctx, [&] {
+    REQUIRE(handles, MCBA_ERR_ARG, "null handles");
+    REQUIRE(ctx->peer_own != nullptr, MCBA_ERR_STATE, "mcba_peer_export has not been called");
+    for (int r = 0; r < ctx->world; r++) {
+      if (r == ctx->rank) { ctx->peer_base[r] = ctx->peer_own; continue; }
+      cudaIpcMemHandle_t h; memcpy(&h, handles + (size_t)r * 64, 64);
+      void* p = nullptr;
+      CK(cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess));
+      ctx->peer_base[r] = (double*)p; ctx->peer_opened.push_back(p);
+    }
+    // sequence number of the in-kernel exchanges (lm_kernel.cuh): starts at zero on every rank, advanced on the device
+    CK(ctx->peer_seq_dev.alloc(1));
+    CK(cudaMemset(ctx->peer_seq_dev.p, 0, sizeof(unsigned long long)));
+    ctx->peer_ready = true;
+  });
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -846,8 +859,8 @@ bool all_finite(const double* p, size_t n) {
 
 // The caller's detection lists: list w = (c*F+f)*B+b of the C*F*B views holds point ids det_ids[det_start[w]:det_start[w+1]] in [0, P) and
 // their pixel corners det_xy (a CSR layout); the boards' id grids, when given, are at most 64 x 64.
-int check_detections(mcba_ctx* ctx, const mcba_problem_desc* desc, const int64_t* det_start, const int32_t* det_ids, const double* det_xy,
-                     const int32_t* board_grid) {
+void check_detections(const mcba_problem_desc* desc, const int64_t* det_start, const int32_t* det_ids, const double* det_xy,
+                      const int32_t* board_grid) {
   const int nv = desc->C * desc->F * desc->B;
   const int64_t total = det_start[nv];
   REQUIRE(det_start[0] == 0 && total >= 0 && total < ((int64_t)1 << 31), MCBA_ERR_ARG, "bad detection offsets");
@@ -857,12 +870,11 @@ int check_detections(mcba_ctx* ctx, const mcba_problem_desc* desc, const int64_t
   for (int b = 0; board_grid && b < desc->B; b++)
     REQUIRE(board_grid[5 * b] > 0 && board_grid[5 * b + 1] > 0 && board_grid[5 * b + 2] > 0 && board_grid[5 * b] <= 64 && board_grid[5 * b + 1] <= 64,
             MCBA_ERR_UNSUPPORTED, "id grids are limited to 64 x 64 (bit masks of the occupied rows / columns)");
-  return MCBA_OK;
 }
 
 // detection lists in that layout -> ctx->pnp, with the id grids and the board points when given (the point table needs the lists only)
-int stage_detections(mcba_ctx* ctx, const mcba_problem_desc* desc, const int64_t* det_start, const int32_t* det_ids, const double* det_xy,
-                     const int32_t* board_grid, const double* board_points) {
+void stage_detections(mcba_ctx* ctx, const mcba_problem_desc* desc, const int64_t* det_start, const int32_t* det_ids, const double* det_xy,
+                      const int32_t* board_grid, const double* board_points) {
   const int nv = desc->C * desc->F * desc->B, B = desc->B, Pn = desc->P;
   const int64_t total = det_start[nv];
   cudaStream_t s = ctx->stream;
@@ -882,11 +894,10 @@ int stage_detections(mcba_ctx* ctx, const mcba_problem_desc* desc, const int64_t
     CK(pb.bp.alloc((size_t)B * Pn * 3));
     CK(cudaMemcpyAsync(pb.bp.p, board_points, sizeof(double) * (size_t)B * Pn * 3, cudaMemcpyHostToDevice, s));
   }
-  return MCBA_OK;
 }
 
 // k_pnp_views over the staged lists: one warp per list, poses under the intrinsics intr [C][kint] (device) of camera model `model`
-int launch_pnp(mcba_ctx* ctx, const mcba_problem_desc* desc, int model, int kint, const double* intr) {
+void launch_pnp(mcba_ctx* ctx, const mcba_problem_desc* desc, int model, int kint, const double* intr) {
   auto& pb = ctx->pnp;
   PnpArgs a{};
   a.C = desc->C; a.F = desc->F; a.B = desc->B; a.P = desc->P; a.model = model; a.kint = kint; a.nv = desc->C * desc->F * desc->B;
@@ -899,7 +910,6 @@ int launch_pnp(mcba_ctx* ctx, const mcba_problem_desc* desc, int model, int kint
     k_pnp_views<MODEL><<<blocks, PNP_WARPS * 32, 0, ctx->stream>>>(a);
   });
   CKL();
-  return MCBA_OK;
 }
 
 // Every upload starts here: whatever it refuses, and however late, it leaves no problem rather than a stale one (the entry points that
@@ -908,33 +918,31 @@ void drop_problem(mcba_ctx* ctx) {
   ctx->uploaded = false; ctx->table = false; ctx->table_selected = -1; ctx->errors_current = false;
 }
 
-// the dense table and the parameter state of `desc`; *board_pts receives where the board points go
-int begin_intake(mcba_ctx* ctx, const mcba_problem_desc* desc, bool points_f32, double** board_pts) {
+// the dense table and the parameter state of `desc`; returns where the board points go
+double* begin_intake(mcba_ctx* ctx, const mcba_problem_desc* desc, bool points_f32) {
   const size_t dense = std::max<size_t>((size_t)desc->C * desc->F * desc->B * desc->P, 1);
   CK(ctx->valid_mask.alloc(dense));
   if (points_f32) CK(ctx->dense_pts32.alloc(dense)); else CK(ctx->dense_pts.alloc(dense));
-  return alloc_state(ctx, desc, board_pts);
+  return alloc_state(ctx, desc);
 }
 
 // A dense host table -> ctx->valid_mask (and ctx->view_valid), its points -> dense_pts or dense_pts32, the board points -> the state.
-// *points_ready: the event after which the points are on the device, or null.
-int stage_dense(mcba_ctx* ctx, const mcba_problem_desc* desc, const uint8_t* valid, const uint8_t* view_valid, const void* points,
-                int32_t point_type, const double* board_points, cudaEvent_t* points_ready) {
-  if (!ctx || !desc) return MCBA_ERR_ARG;
+// Returns the event after which the points are on the device, or null.
+cudaEvent_t stage_dense(mcba_ctx* ctx, const mcba_problem_desc* desc, const uint8_t* valid, const uint8_t* view_valid, const void* points,
+                        int32_t point_type, const double* board_points) {
+  REQUIRE(desc, MCBA_ERR_ARG, "null problem description");
   drop_problem(ctx);
-  CK(cudaSetDevice(ctx->device));
-  { int r = check_desc(ctx, desc); if (r) return r; }
+  check_desc(desc);
   REQUIRE(valid && points && board_points, MCBA_ERR_ARG, "null dense table");
   REQUIRE(point_type == MCBA_POINTS_F64 || point_type == MCBA_POINTS_F32, MCBA_ERR_ARG, "unknown point type");
   const bool points_f32 = point_type == MCBA_POINTS_F32;
   const int nv = desc->C * desc->F * desc->B;
   const size_t dense = (size_t)nv * desc->P;
-  double* bpts = nullptr;
-  { int r = begin_intake(ctx, desc, points_f32, &bpts); if (r) return r; }
+  double* bpts = begin_intake(ctx, desc, points_f32);
   if (view_valid) CK(ctx->view_valid.alloc((size_t)std::max(nv, 1)));
   cudaStream_t s = ctx->stream;
   UploadClock clk(ctx->profiling);
-  *points_ready = nullptr;
+  cudaEvent_t points_ready = nullptr;
   // the mask (1 B/point) goes first on the solver's stream; the observations (16 B/point) follow on the copy stream while the views
   // are counted and scanned, and the scatter waits for them
   if (dense) CK(cudaMemcpyAsync(ctx->valid_mask.p, valid, dense, cudaMemcpyHostToDevice, s));
@@ -949,24 +957,22 @@ int stage_dense(mcba_ctx* ctx, const mcba_problem_desc* desc, const uint8_t* val
     if (points_f32) CK(cudaMemcpyAsync(ctx->dense_pts32.p, points, dense * sizeof(float2), cudaMemcpyHostToDevice, ctx->copy_stream));
     else CK(cudaMemcpyAsync(ctx->dense_pts.p, points, dense * sizeof(double2), cudaMemcpyHostToDevice, ctx->copy_stream));
     CK(cudaEventRecord(ctx->copy_done, ctx->copy_stream));
-    *points_ready = ctx->copy_done;
+    points_ready = ctx->copy_done;
     clk.mark("upload: copies issued");
   }
-  return MCBA_OK;
+  return points_ready;
 }
 
-// the staged table becomes the resident one: inliers = valid, pack `valid`, remember the description
-int table_finish(mcba_ctx* ctx, const mcba_problem_desc* desc, cudaEvent_t points_ready, int64_t* n_valid) {
+// the staged table becomes the resident one: inliers = valid, pack `valid`, remember the description; returns the number of corners
+int64_t table_finish(mcba_ctx* ctx, const mcba_problem_desc* desc, cudaEvent_t points_ready) {
   const size_t dense = (size_t)desc->C * desc->F * desc->B * desc->P;
   CK(ctx->inlier_mask.alloc(std::max<size_t>(dense, 1)));
   if (dense) CK(cudaMemcpyAsync(ctx->inlier_mask.p, ctx->valid_mask.p, dense, cudaMemcpyDeviceToDevice, ctx->stream));
   ctx->table_desc = *desc;
-  int64_t n = 0;
-  { int r = pack_dense(ctx, desc, ctx->valid_mask.p, false, &n, nullptr, points_ready); if (r) return r; }
+  const int64_t n = pack_dense(ctx, desc, ctx->valid_mask.p, false, nullptr, points_ready);
   ctx->table = true; ctx->table_selected = MCBA_TABLE_VALID;
   ctx->n_valid = n; ctx->n_inliers = n;
-  if (n_valid) *n_valid = n;
-  return MCBA_OK;
+  return n;
 }
 
 size_t table_dense(const mcba_ctx* ctx) {
@@ -974,24 +980,25 @@ size_t table_dense(const mcba_ctx* ctx) {
   return (size_t)d.C * d.F * d.B * d.P;
 }
 
-int sort_errors(mcba_ctx* ctx, const double* in, double* out, int64_t n) {
+void sort_errors(mcba_ctx* ctx, const double* in, double* out, int64_t n) {
   size_t bytes = 0;
   CK(cub::DeviceRadixSort::SortKeys(nullptr, bytes, in, out, n, 0, 64, ctx->stream));
   CK(ctx->sort_tmp.alloc(bytes));
   bytes = ctx->sort_tmp.n;
   CK(cub::DeviceRadixSort::SortKeys(ctx->sort_tmp.p, bytes, in, out, n, 0, 64, ctx->stream));
   ctx->launches += 4;
-  return MCBA_OK;
 }
 
 }  // namespace
 
 int mcba_upload_dense(mcba_ctx* ctx, const mcba_problem_desc* desc, const uint8_t* valid, const uint8_t* view_valid, const void* points,
                       int32_t point_type, const double* board_points, int64_t* n_corners) {
-  cudaEvent_t ready = nullptr;
-  { int r = stage_dense(ctx, desc, valid, view_valid, points, point_type, board_points, &ready); if (r) return r; }
-  return pack_dense(ctx, desc, ctx->valid_mask.p, false, n_corners, view_valid ? ctx->view_valid.p : nullptr, ready,
-                    point_type == MCBA_POINTS_F32);
+  return api(ctx, [&] {
+    cudaEvent_t ready = stage_dense(ctx, desc, valid, view_valid, points, point_type, board_points);
+    const int64_t n = pack_dense(ctx, desc, ctx->valid_mask.p, false, view_valid ? ctx->view_valid.p : nullptr, ready,
+                                 point_type == MCBA_POINTS_F32);
+    if (n_corners) *n_corners = n;
+  });
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -999,69 +1006,72 @@ int mcba_upload_dense(mcba_ctx* ctx, const mcba_problem_desc* desc, const uint8_
 
 int mcba_table_upload(mcba_ctx* ctx, const mcba_problem_desc* desc, const uint8_t* valid, const double* points,
                       const double* board_points, int64_t* n_valid) {
-  cudaEvent_t ready = nullptr;
-  { int r = stage_dense(ctx, desc, valid, nullptr, points, MCBA_POINTS_F64, board_points, &ready); if (r) return r; }
-  return table_finish(ctx, desc, ready, n_valid);
+  return api(ctx, [&] {
+    cudaEvent_t ready = stage_dense(ctx, desc, valid, nullptr, points, MCBA_POINTS_F64, board_points);
+    const int64_t n = table_finish(ctx, desc, ready);
+    if (n_valid) *n_valid = n;
+  });
 }
 
 int mcba_table_from_detections(mcba_ctx* ctx, const mcba_problem_desc* desc, const int64_t* det_start, const int32_t* det_ids,
                                const double* det_xy, const double* board_points, int64_t* n_valid) {
-  if (!ctx || !desc) return MCBA_ERR_ARG;
-  drop_problem(ctx);
-  CK(cudaSetDevice(ctx->device));
-  { int r = check_desc(ctx, desc); if (r) return r; }
-  REQUIRE(det_start && board_points, MCBA_ERR_ARG, "null argument");
-  { int r = check_detections(ctx, desc, det_start, det_ids, det_xy, nullptr); if (r) return r; }
-  const int nv = desc->C * desc->F * desc->B;
-  {   // a table entry holds one corner
-    std::vector<int> list_of((size_t)desc->P, -1);
-    for (int w = 0; w < nv; w++)
-      for (int64_t i = det_start[w]; i < det_start[w + 1]; i++) {
-        REQUIRE(list_of[det_ids[i]] != w, MCBA_ERR_ARG, "detection list " + std::to_string(w) + " repeats point id " + std::to_string(det_ids[i]));
-        list_of[det_ids[i]] = w;
-      }
-  }
-  const size_t dense = (size_t)nv * desc->P;
-  cudaStream_t s = ctx->stream;
-  double* bpts = nullptr;
-  { int r = begin_intake(ctx, desc, false, &bpts); if (r) return r; }
-  CK(cudaMemcpyAsync(bpts, board_points, sizeof(double) * (size_t)desc->B * desc->P * 3, cudaMemcpyHostToDevice, s));
-  { int r = stage_detections(ctx, desc, det_start, det_ids, det_xy, nullptr, nullptr); if (r) return r; }
-  if (dense) {
-    CK(cudaMemsetAsync(ctx->valid_mask.p, 0, dense, s));
-    CK(cudaMemsetAsync(ctx->dense_pts.p, 0, dense * sizeof(double2), s));    // fill_sparse leaves zeros where nothing was detected
-  }
-  if (det_start[nv] > 0) {      // the ids were checked above: k_table_fill's range guard never writes its flag
-    auto& pb = ctx->pnp;
-    k_table_fill<<<(unsigned)(((size_t)nv * 32 + 255) / 256), 256, 0, s>>>(pb.start.p, pb.ids.p, pb.xy.p, nv, desc->P, ctx->valid_mask.p, ctx->dense_pts.p, nullptr); CKL();
-  }
-  return table_finish(ctx, desc, nullptr, n_valid);
+  return api(ctx, [&] {
+    REQUIRE(desc, MCBA_ERR_ARG, "null problem description");
+    drop_problem(ctx);
+    check_desc(desc);
+    REQUIRE(det_start && board_points, MCBA_ERR_ARG, "null argument");
+    check_detections(desc, det_start, det_ids, det_xy, nullptr);
+    const int nv = desc->C * desc->F * desc->B;
+    {   // a table entry holds one corner
+      std::vector<int> list_of((size_t)desc->P, -1);
+      for (int w = 0; w < nv; w++)
+        for (int64_t i = det_start[w]; i < det_start[w + 1]; i++) {
+          REQUIRE(list_of[det_ids[i]] != w, MCBA_ERR_ARG, "detection list " + std::to_string(w) + " repeats point id " + std::to_string(det_ids[i]));
+          list_of[det_ids[i]] = w;
+        }
+    }
+    const size_t dense = (size_t)nv * desc->P;
+    cudaStream_t s = ctx->stream;
+    double* bpts = begin_intake(ctx, desc, false);
+    CK(cudaMemcpyAsync(bpts, board_points, sizeof(double) * (size_t)desc->B * desc->P * 3, cudaMemcpyHostToDevice, s));
+    stage_detections(ctx, desc, det_start, det_ids, det_xy, nullptr, nullptr);
+    if (dense) {
+      CK(cudaMemsetAsync(ctx->valid_mask.p, 0, dense, s));
+      CK(cudaMemsetAsync(ctx->dense_pts.p, 0, dense * sizeof(double2), s));    // fill_sparse leaves zeros where nothing was detected
+    }
+    if (det_start[nv] > 0) {      // the ids were checked above: k_table_fill's range guard never writes its flag
+      auto& pb = ctx->pnp;
+      k_table_fill<<<(unsigned)(((size_t)nv * 32 + 255) / 256), 256, 0, s>>>(pb.start.p, pb.ids.p, pb.xy.p, nv, desc->P, ctx->valid_mask.p, ctx->dense_pts.p, nullptr); CKL();
+    }
+    const int64_t n = table_finish(ctx, desc, nullptr);
+    if (n_valid) *n_valid = n;
+  });
 }
 
 // Batched board-pose initialisation (pnp_kernels.cuh): one warp per detection list.  Independent of the uploaded problem.
 int mcba_pnp_views(mcba_ctx* ctx, const mcba_problem_desc* desc, const int64_t* det_start, const int32_t* det_ids, const double* det_xy,
                    const double* board_points, const double* intrinsics, const int32_t* board_grid,
                    double* poses, double* errors, int32_t* num_points, uint8_t* valid) {
-  if (!ctx || !desc) return MCBA_ERR_ARG;
-  CK(cudaSetDevice(ctx->device));
-  { int r = check_desc(ctx, desc); if (r) return r; }
-  REQUIRE(det_start && board_points && intrinsics && board_grid && poses && errors && num_points && valid, MCBA_ERR_ARG, "null argument");
-  const int nv = desc->C * desc->F * desc->B;
-  if (nv == 0) return MCBA_OK;
-  { int r = check_detections(ctx, desc, det_start, det_ids, det_xy, board_grid); if (r) return r; }
-  const int kint = 5 + model_nd(desc->model);
-  cudaStream_t s = ctx->stream;
-  auto& pb = ctx->pnp;
-  { int r = stage_detections(ctx, desc, det_start, det_ids, det_xy, board_grid, board_points); if (r) return r; }
-  CK(pb.in.alloc((size_t)desc->C * kint));
-  CK(cudaMemcpyAsync(pb.in.p, intrinsics, sizeof(double) * (size_t)desc->C * kint, cudaMemcpyHostToDevice, s));
-  { int r = launch_pnp(ctx, desc, desc->model, kint, pb.in.p); if (r) return r; }
-  CK(cudaMemcpyAsync(poses, pb.pose.p, sizeof(double) * 16 * (size_t)nv, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(errors, pb.err.p, sizeof(double) * (size_t)nv, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(num_points, pb.n.p, sizeof(int32_t) * (size_t)nv, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(valid, pb.ok.p, (size_t)nv, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  return MCBA_OK;
+  return api(ctx, [&] {
+    REQUIRE(desc, MCBA_ERR_ARG, "null problem description");
+    check_desc(desc);
+    REQUIRE(det_start && board_points && intrinsics && board_grid && poses && errors && num_points && valid, MCBA_ERR_ARG, "null argument");
+    const int nv = desc->C * desc->F * desc->B;
+    if (nv == 0) return;
+    check_detections(desc, det_start, det_ids, det_xy, board_grid);
+    const int kint = 5 + model_nd(desc->model);
+    cudaStream_t s = ctx->stream;
+    auto& pb = ctx->pnp;
+    stage_detections(ctx, desc, det_start, det_ids, det_xy, board_grid, board_points);
+    CK(pb.in.alloc((size_t)desc->C * kint));
+    CK(cudaMemcpyAsync(pb.in.p, intrinsics, sizeof(double) * (size_t)desc->C * kint, cudaMemcpyHostToDevice, s));
+    launch_pnp(ctx, desc, desc->model, kint, pb.in.p);
+    CK(cudaMemcpyAsync(poses, pb.pose.p, sizeof(double) * 16 * (size_t)nv, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(errors, pb.err.p, sizeof(double) * (size_t)nv, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(num_points, pb.n.p, sizeof(int32_t) * (size_t)nv, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(valid, pb.ok.p, (size_t)nv, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+  });
 }
 
 // Initialisation of single-camera intrinsic calibration (intrinsics_kernels.cuh): one homography per used view, K0 per camera
@@ -1069,145 +1079,144 @@ int mcba_pnp_views(mcba_ctx* ctx, const mcba_problem_desc* desc, const int64_t* 
 int mcba_intrinsic_init(mcba_ctx* ctx, const mcba_problem_desc* desc, const int64_t* det_start, const int32_t* det_ids, const double* det_xy,
                         const double* board_points, const int32_t* board_grid, const int32_t* image_sizes, const uint8_t* view_use,
                         double* intrinsics, double* poses, uint8_t* ok) {
-  if (!ctx || !desc) return MCBA_ERR_ARG;
-  CK(cudaSetDevice(ctx->device));
-  { int r = check_desc(ctx, desc); if (r) return r; }
-  REQUIRE(det_start && board_points && board_grid && image_sizes && view_use && intrinsics && poses && ok, MCBA_ERR_ARG, "null argument");
-  const int C = desc->C, F = desc->F, B = desc->B, Pn = desc->P, nv = C * F * B;
-  const bool fisheye = desc->model == MODEL_FISHEYE;
-  const int kint = 5 + model_nd(desc->model);
-  { int r = check_detections(ctx, desc, det_start, det_ids, det_xy, board_grid); if (r) return r; }
-  for (int c = 0; c < C; c++) REQUIRE(image_sizes[2 * c] > 0 && image_sizes[2 * c + 1] > 0, MCBA_ERR_ARG, "image sizes must be positive");
-  // OpenCV estimates an initial camera matrix only for planar targets (all object points at z = 0)
-  for (size_t i = 0; i < (size_t)B * Pn; i++)
-    REQUIRE(board_points[3 * i + 2] == 0.0, MCBA_ERR_UNSUPPORTED, "non-planar board (z != 0): the initial camera matrix needs planar targets");
-  // used views grouped by camera, board-major inside a camera (the order of calibration_points, camera.py:229-235); the detection lists
-  // of unused views are emptied, so that k_pnp_views sees only the used ones
-  std::vector<int32_t> used, cam_start((size_t)C + 1, 0);
-  for (int c = 0; c < C; c++) {
-    for (int b = 0; b < B; b++) for (int f = 0; f < F; f++) { const int w = (c * F + f) * B + b; if (view_use[w]) used.push_back(w); }
-    cam_start[(size_t)c + 1] = (int32_t)used.size();
-  }
-  std::vector<int64_t> start((size_t)nv + 1, 0);
-  std::vector<int32_t> ids; std::vector<double> xy;
-  for (int w = 0; w < nv; w++) {
-    if (view_use[w]) {
-      ids.insert(ids.end(), det_ids + det_start[w], det_ids + det_start[w + 1]);
-      xy.insert(xy.end(), det_xy + 2 * det_start[w], det_xy + 2 * det_start[w + 1]);
+  return api(ctx, [&] {
+    REQUIRE(desc, MCBA_ERR_ARG, "null problem description");
+    check_desc(desc);
+    REQUIRE(det_start && board_points && board_grid && image_sizes && view_use && intrinsics && poses && ok, MCBA_ERR_ARG, "null argument");
+    const int C = desc->C, F = desc->F, B = desc->B, Pn = desc->P, nv = C * F * B;
+    const bool fisheye = desc->model == MODEL_FISHEYE;
+    const int kint = 5 + model_nd(desc->model);
+    check_detections(desc, det_start, det_ids, det_xy, board_grid);
+    for (int c = 0; c < C; c++) REQUIRE(image_sizes[2 * c] > 0 && image_sizes[2 * c + 1] > 0, MCBA_ERR_ARG, "image sizes must be positive");
+    // OpenCV estimates an initial camera matrix only for planar targets (all object points at z = 0)
+    for (size_t i = 0; i < (size_t)B * Pn; i++)
+      REQUIRE(board_points[3 * i + 2] == 0.0, MCBA_ERR_UNSUPPORTED, "non-planar board (z != 0): the initial camera matrix needs planar targets");
+    // used views grouped by camera, board-major inside a camera (the order of calibration_points, camera.py:229-235); the detection lists
+    // of unused views are emptied, so that k_pnp_views sees only the used ones
+    std::vector<int32_t> used, cam_start((size_t)C + 1, 0);
+    for (int c = 0; c < C; c++) {
+      for (int b = 0; b < B; b++) for (int f = 0; f < F; f++) { const int w = (c * F + f) * B + b; if (view_use[w]) used.push_back(w); }
+      cam_start[(size_t)c + 1] = (int32_t)used.size();
     }
-    start[(size_t)w + 1] = (int64_t)ids.size();
-  }
-  const int n_used = (int)used.size();
-  cudaStream_t s = ctx->stream;
-  auto& pb = ctx->pnp; auto& ib = ctx->intrinsic;
-  { int r = stage_detections(ctx, desc, start.data(), ids.data(), xy.data(), board_grid, board_points); if (r) return r; }
-  CK(ib.used.alloc((size_t)std::max(n_used, 1))); CK(ib.cam_start.alloc((size_t)C + 1)); CK(ib.size.alloc((size_t)C * 2));
-  CK(ib.H.alloc((size_t)std::max(n_used, 1) * 9)); CK(ib.hok.alloc((size_t)std::max(n_used, 1))); CK(ib.k0.alloc((size_t)C * kint));
-  if (n_used) CK(cudaMemcpyAsync(ib.used.p, used.data(), sizeof(int32_t) * used.size(), cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(ib.cam_start.p, cam_start.data(), sizeof(int32_t) * cam_start.size(), cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(ib.size.p, image_sizes, sizeof(int32_t) * (size_t)C * 2, cudaMemcpyHostToDevice, s));
-  if (fisheye) {
-    if (C) { k_fisheye_k0<<<(C + 127) / 128, 128, 0, s>>>(C, kint, ib.size.p, ib.k0.p); CKL(); }
-  } else {
-    if (n_used) {
-      HomographyArgs h{};
-      h.n_used = n_used; h.B = B; h.P = Pn; h.used = ib.used.p; h.det_start = pb.start.p; h.det_ids = pb.ids.p; h.det_xy = pb.xy.p;
-      h.board_pts = pb.bp.p; h.H = ib.H.p; h.ok = ib.hok.p;
-      k_view_homography<<<(n_used + HOMOG_WARPS - 1) / HOMOG_WARPS, HOMOG_WARPS * 32, 0, s>>>(h); CKL();
+    std::vector<int64_t> start((size_t)nv + 1, 0);
+    std::vector<int32_t> ids; std::vector<double> xy;
+    for (int w = 0; w < nv; w++) {
+      if (view_use[w]) {
+        ids.insert(ids.end(), det_ids + det_start[w], det_ids + det_start[w + 1]);
+        xy.insert(xy.end(), det_xy + 2 * det_start[w], det_xy + 2 * det_start[w + 1]);
+      }
+      start[(size_t)w + 1] = (int64_t)ids.size();
     }
-    ZhangArgs z{};
-    z.kint = kint; z.fix_aspect = (desc->optimize & MCBA_OPT_FIX_ASPECT) ? 1 : 0; z.cam_start = ib.cam_start.p; z.image_size = ib.size.p;
-    z.H = ib.H.p; z.ok = ib.hok.p; z.intr = ib.k0.p;
-    k_zhang_init<<<C, ZHANG_THREADS, 0, s>>>(z); CKL();
-  }
-  if (nv) {
-    // zero distortion: the pinhole K0, or the fisheye K0 whose undistortion is exact at k = 0
-    { int r = launch_pnp(ctx, desc, fisheye ? MODEL_FISHEYE : MODEL_STANDARD, kint, ib.k0.p); if (r) return r; }
-    CK(cudaMemcpyAsync(poses, pb.pose.p, sizeof(double) * 16 * (size_t)nv, cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(ok, pb.ok.p, (size_t)nv, cudaMemcpyDeviceToHost, s));
-  }
-  CK(cudaMemcpyAsync(intrinsics, ib.k0.p, sizeof(double) * (size_t)C * kint, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  return MCBA_OK;
+    const int n_used = (int)used.size();
+    cudaStream_t s = ctx->stream;
+    auto& pb = ctx->pnp; auto& ib = ctx->intrinsic;
+    stage_detections(ctx, desc, start.data(), ids.data(), xy.data(), board_grid, board_points);
+    CK(ib.used.alloc((size_t)std::max(n_used, 1))); CK(ib.cam_start.alloc((size_t)C + 1)); CK(ib.size.alloc((size_t)C * 2));
+    CK(ib.H.alloc((size_t)std::max(n_used, 1) * 9)); CK(ib.hok.alloc((size_t)std::max(n_used, 1))); CK(ib.k0.alloc((size_t)C * kint));
+    if (n_used) CK(cudaMemcpyAsync(ib.used.p, used.data(), sizeof(int32_t) * used.size(), cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(ib.cam_start.p, cam_start.data(), sizeof(int32_t) * cam_start.size(), cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(ib.size.p, image_sizes, sizeof(int32_t) * (size_t)C * 2, cudaMemcpyHostToDevice, s));
+    if (fisheye) {
+      if (C) { k_fisheye_k0<<<(C + 127) / 128, 128, 0, s>>>(C, kint, ib.size.p, ib.k0.p); CKL(); }
+    } else {
+      if (n_used) {
+        HomographyArgs h{};
+        h.n_used = n_used; h.B = B; h.P = Pn; h.used = ib.used.p; h.det_start = pb.start.p; h.det_ids = pb.ids.p; h.det_xy = pb.xy.p;
+        h.board_pts = pb.bp.p; h.H = ib.H.p; h.ok = ib.hok.p;
+        k_view_homography<<<(n_used + HOMOG_WARPS - 1) / HOMOG_WARPS, HOMOG_WARPS * 32, 0, s>>>(h); CKL();
+      }
+      ZhangArgs z{};
+      z.kint = kint; z.fix_aspect = (desc->optimize & MCBA_OPT_FIX_ASPECT) ? 1 : 0; z.cam_start = ib.cam_start.p; z.image_size = ib.size.p;
+      z.H = ib.H.p; z.ok = ib.hok.p; z.intr = ib.k0.p;
+      k_zhang_init<<<C, ZHANG_THREADS, 0, s>>>(z); CKL();
+    }
+    if (nv) {
+      // zero distortion: the pinhole K0, or the fisheye K0 whose undistortion is exact at k = 0
+      launch_pnp(ctx, desc, fisheye ? MODEL_FISHEYE : MODEL_STANDARD, kint, ib.k0.p);
+      CK(cudaMemcpyAsync(poses, pb.pose.p, sizeof(double) * 16 * (size_t)nv, cudaMemcpyDeviceToHost, s));
+      CK(cudaMemcpyAsync(ok, pb.ok.p, (size_t)nv, cudaMemcpyDeviceToHost, s));
+    }
+    CK(cudaMemcpyAsync(intrinsics, ib.k0.p, sizeof(double) * (size_t)C * kint, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+  });
 }
 
 // Initialisation of stereo calibration (stereo_kernels.cuh): per-view poses of both cameras by k_pnp_views under the given intrinsics,
 // then the median relative pose.  Independent of the uploaded problem.
 int mcba_stereo_init(mcba_ctx* ctx, const mcba_problem_desc* desc, const int64_t* det_start, const int32_t* det_ids, const double* det_xy,
                      const double* board_points, const double* intrinsics, double* rt0, double* left_poses, uint8_t* ok) {
-  if (!ctx || !desc) return MCBA_ERR_ARG;
-  CK(cudaSetDevice(ctx->device));
-  { int r = check_desc(ctx, desc); if (r) return r; }
-  REQUIRE(desc->C == 2 && desc->B == 1 && desc->F > 0, MCBA_ERR_ARG, "a stereo pair is 2 cameras, 1 board and at least one view");
-  REQUIRE(det_start && board_points && intrinsics && rt0 && left_poses && ok, MCBA_ERR_ARG, "null argument");
-  const int F = desc->F, Pn = desc->P;
-  const int kint = 5 + model_nd(desc->model);
-  const int32_t grid[5] = {1, 1, 1, 0, 0};           // the views are chosen already: no minimum-detections rule on the device
-  { int r = check_detections(ctx, desc, det_start, det_ids, det_xy, grid); if (r) return r; }
-  REQUIRE(all_finite(intrinsics, 2 * (size_t)kint), MCBA_ERR_NONFINITE, "non-finite camera parameter");
-  // the per-view poses are the planar PnP of k_pnp_views
-  for (size_t i = 0; i < (size_t)Pn; i++)
-    REQUIRE(board_points[3 * i + 2] == 0.0, MCBA_ERR_UNSUPPORTED, "non-planar object points (z != 0): the initial view poses need planar targets");
-  for (int c = 0; c < 2; c++)
-    for (int f = 0; f < F; f++) {
-      const int64_t n = det_start[c * F + f + 1] - det_start[c * F + f];
-      REQUIRE(n >= 4, MCBA_ERR_DEGENERATE, "view " + std::to_string(f) + " has " + std::to_string(n) + " points: a view pose needs at least 4");
-    }
-  cudaStream_t s = ctx->stream;
-  auto& pb = ctx->pnp; auto& sb = ctx->stereo;
-  { int r = stage_detections(ctx, desc, det_start, det_ids, det_xy, grid, board_points); if (r) return r; }
-  CK(pb.in.alloc((size_t)2 * kint));
-  CK(cudaMemcpyAsync(pb.in.p, intrinsics, sizeof(double) * 2 * (size_t)kint, cudaMemcpyHostToDevice, s));
-  { int r = launch_pnp(ctx, desc, desc->model, kint, pb.in.p); if (r) return r; }
-  CK(sb.rel.alloc((size_t)6 * F)); CK(sb.sorted.alloc((size_t)6 * F)); CK(sb.rt0.alloc(6)); CK(sb.both.alloc((size_t)F));
-  StereoStartArgs a{};
-  a.F = F; a.poses = pb.pose.p; a.ok = pb.ok.p; a.rel = sb.rel.p; a.sorted = sb.sorted.p; a.rt0 = sb.rt0.p; a.both = sb.both.p;
-  k_stereo_start<<<1, STEREO_THREADS, 0, s>>>(a); CKL();
-  CK(cudaMemcpyAsync(rt0, sb.rt0.p, sizeof(double) * 6, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(left_poses, pb.pose.p, sizeof(double) * 16 * (size_t)F, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(ok, sb.both.p, (size_t)F, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  return MCBA_OK;
+  return api(ctx, [&] {
+    REQUIRE(desc, MCBA_ERR_ARG, "null problem description");
+    check_desc(desc);
+    REQUIRE(desc->C == 2 && desc->B == 1 && desc->F > 0, MCBA_ERR_ARG, "a stereo pair is 2 cameras, 1 board and at least one view");
+    REQUIRE(det_start && board_points && intrinsics && rt0 && left_poses && ok, MCBA_ERR_ARG, "null argument");
+    const int F = desc->F, Pn = desc->P;
+    const int kint = 5 + model_nd(desc->model);
+    const int32_t grid[5] = {1, 1, 1, 0, 0};           // the views are chosen already: no minimum-detections rule on the device
+    check_detections(desc, det_start, det_ids, det_xy, grid);
+    REQUIRE(all_finite(intrinsics, 2 * (size_t)kint), MCBA_ERR_NONFINITE, "non-finite camera parameter");
+    // the per-view poses are the planar PnP of k_pnp_views
+    for (size_t i = 0; i < (size_t)Pn; i++)
+      REQUIRE(board_points[3 * i + 2] == 0.0, MCBA_ERR_UNSUPPORTED, "non-planar object points (z != 0): the initial view poses need planar targets");
+    for (int c = 0; c < 2; c++)
+      for (int f = 0; f < F; f++) {
+        const int64_t n = det_start[c * F + f + 1] - det_start[c * F + f];
+        REQUIRE(n >= 4, MCBA_ERR_DEGENERATE, "view " + std::to_string(f) + " has " + std::to_string(n) + " points: a view pose needs at least 4");
+      }
+    cudaStream_t s = ctx->stream;
+    auto& pb = ctx->pnp; auto& sb = ctx->stereo;
+    stage_detections(ctx, desc, det_start, det_ids, det_xy, grid, board_points);
+    CK(pb.in.alloc((size_t)2 * kint));
+    CK(cudaMemcpyAsync(pb.in.p, intrinsics, sizeof(double) * 2 * (size_t)kint, cudaMemcpyHostToDevice, s));
+    launch_pnp(ctx, desc, desc->model, kint, pb.in.p);
+    CK(sb.rel.alloc((size_t)6 * F)); CK(sb.sorted.alloc((size_t)6 * F)); CK(sb.rt0.alloc(6)); CK(sb.both.alloc((size_t)F));
+    StereoStartArgs a{};
+    a.F = F; a.poses = pb.pose.p; a.ok = pb.ok.p; a.rel = sb.rel.p; a.sorted = sb.sorted.p; a.rt0 = sb.rt0.p; a.both = sb.both.p;
+    k_stereo_start<<<1, STEREO_THREADS, 0, s>>>(a); CKL();
+    CK(cudaMemcpyAsync(rt0, sb.rt0.p, sizeof(double) * 6, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(left_poses, pb.pose.p, sizeof(double) * 16 * (size_t)F, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(ok, sb.both.p, (size_t)F, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+  });
 }
 
 // Per-view sums of squared pixel errors and corner counts of the packed problem at the current parameters (intrinsics_kernels.cuh)
 int mcba_view_errors(mcba_ctx* ctx, double* sumsq, int64_t* count) {
-  if (!ctx || !sumsq || !count) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
-  CK(cudaSetDevice(ctx->device));
-  DeviceProblem P = with_state(ctx, false);
-  const size_t nv = (size_t)P.C * P.F * P.B;
-  if (nv == 0) return MCBA_OK;
-  int r = prepare(ctx, P); if (r) return r;
-  DevBuf<double> ds; DevBuf<int64_t> dn;
-  CK(ds.alloc(nv)); CK(dn.alloc(nv));
-  cudaStream_t s = ctx->stream;
-  CK(cudaMemsetAsync(ds.p, 0, sizeof(double) * nv, s)); CK(cudaMemsetAsync(dn.p, 0, sizeof(int64_t) * nv, s));
-  if (P.V > 0) {
-    ViewKernelArgs a{}; a.loss = MCBA_LOSS_LINEAR; a.f_scale = 1.0; a.view_cost = ctx->view_cost.p;
-    r = launch_views<MODE_COST>(ctx, P, a); if (r) return r;
-    k_view_sumsq<<<(P.V + 255) / 256, 256, 0, s>>>(P, ctx->view_cost.p, ds.p, dn.p);
-    CKL();
-  }
-  CK(cudaMemcpyAsync(sumsq, ds.p, sizeof(double) * nv, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(count, dn.p, sizeof(int64_t) * nv, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  return MCBA_OK;
+  return api(ctx, [&] {
+    REQUIRE(sumsq && count, MCBA_ERR_ARG, "null argument");
+    REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
+    DeviceProblem P = with_state(ctx, false);
+    const size_t nv = (size_t)P.C * P.F * P.B;
+    if (nv == 0) return;
+    prepare(ctx, P);
+    DevBuf<double> ds; DevBuf<int64_t> dn;
+    CK(ds.alloc(nv)); CK(dn.alloc(nv));
+    cudaStream_t s = ctx->stream;
+    CK(cudaMemsetAsync(ds.p, 0, sizeof(double) * nv, s)); CK(cudaMemsetAsync(dn.p, 0, sizeof(int64_t) * nv, s));
+    if (P.V > 0) {
+      ViewKernelArgs a{}; a.loss = MCBA_LOSS_LINEAR; a.f_scale = 1.0; a.view_cost = ctx->view_cost.p;
+      launch_views<MODE_COST>(ctx, P, a);
+      k_view_sumsq<<<(P.V + 255) / 256, 256, 0, s>>>(P, ctx->view_cost.p, ds.p, dn.p);
+      CKL();
+    }
+    CK(cudaMemcpyAsync(sumsq, ds.p, sizeof(double) * nv, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(count, dn.p, sizeof(int64_t) * nv, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+  });
 }
 
 namespace {
 
-int check_pose_dims(mcba_ctx* ctx, int32_t C, int32_t F, int32_t B) {
+void check_pose_dims(int32_t C, int32_t F, int32_t B) {
   REQUIRE(C > 0 && F > 0 && B > 0, MCBA_ERR_ARG, "bad pose table dimensions");
   REQUIRE((int64_t)C * F * B < ((int64_t)1 << 31), MCBA_ERR_UNSUPPORTED, "more than 2^31 views");
-  return MCBA_OK;
 }
 
 // Uploads the pose table, gathers the rows of every item (start: CSR row offsets, one segment per item) and runs align_transforms_robust
 // on each (pose_init_kernels.cuh): items above PI_SMALL_MAX rows on the large-item kernel, the rest on the shared-memory one.  Leaves
 // t [items][4][4], n_inl [items] and inl [rows] on the device.  vecs (host, [rows][6]) selects the cluster-only mode instead of rows.
-int run_pose_align(mcba_ctx* ctx, int C, int F, int B, const double* poses, const uint8_t* valid, const double* cam, const double* board,
-                   const std::vector<PoseRow>& rows, const std::vector<int64_t>& start, const double* vecs) {
+void run_pose_align(mcba_ctx* ctx, int C, int F, int B, const double* poses, const uint8_t* valid, const double* cam, const double* board,
+                    const std::vector<PoseRow>& rows, const std::vector<int64_t>& start, const double* vecs) {
   auto& pb = ctx->pinit;
   cudaStream_t s = ctx->stream;
   const int n_items = (int)start.size() - 1;
@@ -1255,7 +1264,7 @@ int run_pose_align(mcba_ctx* ctx, int C, int F, int B, const double* poses, cons
     const int64_t R = start[i + 1] - start[i];
     if (R > 0 && R <= PI_SMALL_MAX) { order.push_back(i); small_max = std::max(small_max, (int)R); }
   }
-  if (order.empty()) return MCBA_OK;
+  if (order.empty()) return;
   CK(cudaMemcpyAsync(pb.items.p, order.data(), sizeof(int32_t) * order.size(), cudaMemcpyHostToDevice, s));
   if (n_large) {
     CK(pb.work.alloc((size_t)n_rows * PI_ROW_BYTES));
@@ -1267,7 +1276,6 @@ int run_pose_align(mcba_ctx* ctx, int C, int F, int B, const double* poses, cons
     a.items = pb.items.p + n_large;
     k_pose_align<PI_SMALL_THREADS, false><<<n_small, PI_SMALL_THREADS, (size_t)small_max * PI_ROW_BYTES, s>>>(a); CKL();
   }
-  return MCBA_OK;
 }
 
 }  // namespace
@@ -1275,179 +1283,173 @@ int run_pose_align(mcba_ctx* ctx, int C, int F, int B, const double* poses, cons
 // Relative poses of estimate_relative_poses (axis 0) / estimate_relative_poses_inv (axis 2), every (parent, child) pair in one launch chain
 int mcba_pose_pairs(mcba_ctx* ctx, int32_t C, int32_t F, int32_t B, const double* poses, const uint8_t* valid, int32_t axis,
                     const int32_t* pairs, int32_t n_pairs, double* t, uint8_t* inliers, int32_t* n_inliers) {
-  if (!ctx) return MCBA_ERR_ARG;
-  CK(cudaSetDevice(ctx->device));
-  { int r = check_pose_dims(ctx, C, F, B); if (r) return r; }
-  REQUIRE(poses && valid, MCBA_ERR_ARG, "null pose table");
-  REQUIRE(axis == 0 || axis == 2, MCBA_ERR_ARG, "axis must be 0 (cameras) or 2 (boards)");
-  REQUIRE(n_pairs >= 0, MCBA_ERR_ARG, "negative pair count");
-  REQUIRE(n_pairs == 0 || (pairs && t && inliers && n_inliers), MCBA_ERR_ARG, "null argument");
-  const int n = axis == 0 ? C : B;
-  const int64_t R = axis == 0 ? (int64_t)F * B : (int64_t)C * F;
-  REQUIRE((int64_t)n_pairs * R < ((int64_t)1 << 31), MCBA_ERR_UNSUPPORTED, "more than 2^31 rows");
-  for (int k = 0; k < n_pairs; k++)
-    REQUIRE(pairs[2 * k] >= 0 && pairs[2 * k] < n && pairs[2 * k + 1] >= 0 && pairs[2 * k + 1] < n && pairs[2 * k] != pairs[2 * k + 1],
-            MCBA_ERR_ARG, "pair index out of range");
-  if (n_pairs == 0) return MCBA_OK;
-  REQUIRE(all_finite(poses, 16 * (size_t)C * F * B), MCBA_ERR_NONFINITE, "non-finite pose in the table");
-  std::vector<PoseRow> rows((size_t)n_pairs * R);
-  std::vector<int64_t> start((size_t)n_pairs + 1);
-  for (int k = 0; k < n_pairs; k++) {
-    const int p = pairs[2 * k], q = pairs[2 * k + 1];
-    start[k] = k * R;
-    PoseRow* o = rows.data() + k * R;
-    if (axis == 0) {           // rows (f, b), f-major, of table[p] and table[q]
-      for (int64_t r = 0; r < R; r++) o[r] = PoseRow{PI_ROW_PAIR, (int32_t)(p * R + r), (int32_t)(q * R + r), 0};
-    } else {                   // rows (c, f), c-major, of the inverted table[:, :, p] and [:, :, q]
-      for (int64_t r = 0; r < R; r++) o[r] = PoseRow{PI_ROW_PAIR_INV, (int32_t)(r * B + p), (int32_t)(r * B + q), 0};
+  return api(ctx, [&] {
+    check_pose_dims(C, F, B);
+    REQUIRE(poses && valid, MCBA_ERR_ARG, "null pose table");
+    REQUIRE(axis == 0 || axis == 2, MCBA_ERR_ARG, "axis must be 0 (cameras) or 2 (boards)");
+    REQUIRE(n_pairs >= 0, MCBA_ERR_ARG, "negative pair count");
+    REQUIRE(n_pairs == 0 || (pairs && t && inliers && n_inliers), MCBA_ERR_ARG, "null argument");
+    const int n = axis == 0 ? C : B;
+    const int64_t R = axis == 0 ? (int64_t)F * B : (int64_t)C * F;
+    REQUIRE((int64_t)n_pairs * R < ((int64_t)1 << 31), MCBA_ERR_UNSUPPORTED, "more than 2^31 rows");
+    for (int k = 0; k < n_pairs; k++)
+      REQUIRE(pairs[2 * k] >= 0 && pairs[2 * k] < n && pairs[2 * k + 1] >= 0 && pairs[2 * k + 1] < n && pairs[2 * k] != pairs[2 * k + 1],
+              MCBA_ERR_ARG, "pair index out of range");
+    if (n_pairs == 0) return;
+    REQUIRE(all_finite(poses, 16 * (size_t)C * F * B), MCBA_ERR_NONFINITE, "non-finite pose in the table");
+    std::vector<PoseRow> rows((size_t)n_pairs * R);
+    std::vector<int64_t> start((size_t)n_pairs + 1);
+    for (int k = 0; k < n_pairs; k++) {
+      const int p = pairs[2 * k], q = pairs[2 * k + 1];
+      start[k] = k * R;
+      PoseRow* o = rows.data() + k * R;
+      if (axis == 0) {           // rows (f, b), f-major, of table[p] and table[q]
+        for (int64_t r = 0; r < R; r++) o[r] = PoseRow{PI_ROW_PAIR, (int32_t)(p * R + r), (int32_t)(q * R + r), 0};
+      } else {                   // rows (c, f), c-major, of the inverted table[:, :, p] and [:, :, q]
+        for (int64_t r = 0; r < R; r++) o[r] = PoseRow{PI_ROW_PAIR_INV, (int32_t)(r * B + p), (int32_t)(r * B + q), 0};
+      }
     }
-  }
-  start[n_pairs] = (int64_t)n_pairs * R;
-  { int r = run_pose_align(ctx, C, F, B, poses, valid, nullptr, nullptr, rows, start, nullptr); if (r) return r; }
-  auto& pb = ctx->pinit;
-  cudaStream_t s = ctx->stream;
-  CK(cudaMemcpyAsync(t, pb.t.p, sizeof(double) * 16 * n_pairs, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(n_inliers, pb.n_inl.p, sizeof(int32_t) * n_pairs, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(inliers, pb.inl.p, (size_t)n_pairs * R, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  return MCBA_OK;
+    start[n_pairs] = (int64_t)n_pairs * R;
+    run_pose_align(ctx, C, F, B, poses, valid, nullptr, nullptr, rows, start, nullptr);
+    auto& pb = ctx->pinit;
+    cudaStream_t s = ctx->stream;
+    CK(cudaMemcpyAsync(t, pb.t.p, sizeof(double) * 16 * n_pairs, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(n_inliers, pb.n_inl.p, sizeof(int32_t) * n_pairs, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(inliers, pb.inl.p, (size_t)n_pairs * R, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+  });
 }
 
 // Rig poses of initialise_poses (tables.py:370-375): per frame, align_transforms_robust over the (camera, board) rows, times = inv(t)
 int mcba_pose_times(mcba_ctx* ctx, int32_t C, int32_t F, int32_t B, const double* poses, const uint8_t* valid, const double* cam_poses,
                     const uint8_t* cam_valid, const double* board_poses, const uint8_t* board_valid, double* times, uint8_t* times_valid) {
-  if (!ctx) return MCBA_ERR_ARG;
-  CK(cudaSetDevice(ctx->device));
-  { int r = check_pose_dims(ctx, C, F, B); if (r) return r; }
-  REQUIRE(poses && valid, MCBA_ERR_ARG, "null pose table");
-  REQUIRE(cam_poses && cam_valid && board_poses && board_valid && times && times_valid, MCBA_ERR_ARG, "null argument");
-  REQUIRE(all_finite(poses, 16 * (size_t)C * F * B) && all_finite(cam_poses, 16 * (size_t)C) && all_finite(board_poses, 16 * (size_t)B),
-          MCBA_ERR_NONFINITE, "non-finite pose");
-  std::vector<PoseRow> rows;
-  std::vector<int64_t> start(1, 0);
-  std::vector<int32_t> frame_of;
-  for (int f = 0; f < F; f++) {
-    const size_t r0 = rows.size();
-    for (int c = 0; c < C; c++) for (int b = 0; b < B; b++) {
-      const int v = (c * F + f) * B + b;
-      if (cam_valid[c] && valid[v] && board_valid[b]) rows.push_back(PoseRow{PI_ROW_FRAME, v, 0, 0});
+  return api(ctx, [&] {
+    check_pose_dims(C, F, B);
+    REQUIRE(poses && valid, MCBA_ERR_ARG, "null pose table");
+    REQUIRE(cam_poses && cam_valid && board_poses && board_valid && times && times_valid, MCBA_ERR_ARG, "null argument");
+    REQUIRE(all_finite(poses, 16 * (size_t)C * F * B) && all_finite(cam_poses, 16 * (size_t)C) && all_finite(board_poses, 16 * (size_t)B),
+            MCBA_ERR_NONFINITE, "non-finite pose");
+    std::vector<PoseRow> rows;
+    std::vector<int64_t> start(1, 0);
+    std::vector<int32_t> frame_of;
+    for (int f = 0; f < F; f++) {
+      const size_t r0 = rows.size();
+      for (int c = 0; c < C; c++) for (int b = 0; b < B; b++) {
+        const int v = (c * F + f) * B + b;
+        if (cam_valid[c] && valid[v] && board_valid[b]) rows.push_back(PoseRow{PI_ROW_FRAME, v, 0, 0});
+      }
+      if (rows.size() > r0) { start.push_back((int64_t)rows.size()); frame_of.push_back(f); }
     }
-    if (rows.size() > r0) { start.push_back((int64_t)rows.size()); frame_of.push_back(f); }
-  }
-  for (int f = 0; f < F; f++) {
-    times_valid[f] = 0;
-    for (int k = 0; k < 16; k++) times[16 * (size_t)f + k] = (k % 5 == 0) ? 1.0 : 0.0;
-  }
-  if (frame_of.empty()) return MCBA_OK;
-  { int r = run_pose_align(ctx, C, F, B, poses, valid, cam_poses, board_poses, rows, start, nullptr); if (r) return r; }
-  std::vector<double> t(16 * frame_of.size());
-  CK(cudaMemcpyAsync(t.data(), ctx->pinit.t.p, sizeof(double) * t.size(), cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  for (size_t k = 0; k < frame_of.size(); k++) {
-    double* o = times + 16 * (size_t)frame_of[k];
-    pi_inv34(t.data() + 16 * k, o);
-    o[12] = 0.0; o[13] = 0.0; o[14] = 0.0; o[15] = 1.0;
-    times_valid[frame_of[k]] = 1;
-  }
-  return MCBA_OK;
+    for (int f = 0; f < F; f++) {
+      times_valid[f] = 0;
+      for (int k = 0; k < 16; k++) times[16 * (size_t)f + k] = (k % 5 == 0) ? 1.0 : 0.0;
+    }
+    if (frame_of.empty()) return;
+    run_pose_align(ctx, C, F, B, poses, valid, cam_poses, board_poses, rows, start, nullptr);
+    std::vector<double> t(16 * frame_of.size());
+    CK(cudaMemcpyAsync(t.data(), ctx->pinit.t.p, sizeof(double) * t.size(), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    for (size_t k = 0; k < frame_of.size(); k++) {
+      double* o = times + 16 * (size_t)frame_of[k];
+      pi_inv34(t.data() + 16 * k, o);
+      o[12] = 0.0; o[13] = 0.0; o[14] = 0.0; o[15] = 1.0;
+      times_valid[frame_of[k]] = 1;
+    }
+  });
 }
 
 // mean_robust's cluster alone (transform/common.py:6-13): per set of 6-vectors, the mask of the largest Ward cluster
 int mcba_pose_cluster(mcba_ctx* ctx, int32_t n_sets, const int64_t* set_start, const double* vecs, uint8_t* mask) {
-  if (!ctx) return MCBA_ERR_ARG;
-  CK(cudaSetDevice(ctx->device));
-  REQUIRE(n_sets >= 0 && (n_sets == 0 || set_start), MCBA_ERR_ARG, "null set offsets");
-  if (n_sets == 0) return MCBA_OK;
-  REQUIRE(set_start[0] == 0, MCBA_ERR_ARG, "set offsets must start at 0");
-  for (int k = 0; k < n_sets; k++) REQUIRE(set_start[k + 1] >= set_start[k], MCBA_ERR_ARG, "set offsets must not decrease");
-  const int64_t N = set_start[n_sets];
-  REQUIRE(N < ((int64_t)1 << 31), MCBA_ERR_UNSUPPORTED, "more than 2^31 vectors");
-  REQUIRE(N == 0 || (vecs && mask), MCBA_ERR_ARG, "null argument");
-  if (N == 0) return MCBA_OK;
-  REQUIRE(all_finite(vecs, 6 * (size_t)N), MCBA_ERR_NONFINITE, "non-finite vector");
-  std::vector<int64_t> start(set_start, set_start + n_sets + 1);
-  { int r = run_pose_align(ctx, 1, 1, 1, nullptr, nullptr, nullptr, nullptr, {}, start, vecs); if (r) return r; }
-  CK(cudaMemcpyAsync(mask, ctx->pinit.inl.p, (size_t)N, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  return MCBA_OK;
+  return api(ctx, [&] {
+    REQUIRE(n_sets >= 0 && (n_sets == 0 || set_start), MCBA_ERR_ARG, "null set offsets");
+    if (n_sets == 0) return;
+    REQUIRE(set_start[0] == 0, MCBA_ERR_ARG, "set offsets must start at 0");
+    for (int k = 0; k < n_sets; k++) REQUIRE(set_start[k + 1] >= set_start[k], MCBA_ERR_ARG, "set offsets must not decrease");
+    const int64_t N = set_start[n_sets];
+    REQUIRE(N < ((int64_t)1 << 31), MCBA_ERR_UNSUPPORTED, "more than 2^31 vectors");
+    REQUIRE(N == 0 || (vecs && mask), MCBA_ERR_ARG, "null argument");
+    if (N == 0) return;
+    REQUIRE(all_finite(vecs, 6 * (size_t)N), MCBA_ERR_NONFINITE, "non-finite vector");
+    std::vector<int64_t> start(set_start, set_start + n_sets + 1);
+    run_pose_align(ctx, 1, 1, 1, nullptr, nullptr, nullptr, nullptr, {}, start, vecs);
+    CK(cudaMemcpyAsync(mask, ctx->pinit.inl.p, (size_t)N, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+  });
 }
 
 // One cv2.calibrateRobotWorldHandEye(SHAH) of HandEye.master_slave_pair (hand_eye/hand_eye.py:82-107) per quadruple, one CTA each
 int mcba_hand_eye_quads(mcba_ctx* ctx, int32_t C, int32_t F, int32_t B, const double* poses, const uint8_t* valid, int32_t n_quads,
                         const int32_t* quads, double* X, double* Z, int32_t* n_images, uint8_t* ok) {
-  if (!ctx) return MCBA_ERR_ARG;
-  CK(cudaSetDevice(ctx->device));
-  { int r = check_pose_dims(ctx, C, F, B); if (r) return r; }
-  REQUIRE(poses && valid, MCBA_ERR_ARG, "null pose table");
-  REQUIRE(n_quads >= 0, MCBA_ERR_ARG, "negative quadruple count");
-  REQUIRE(n_quads == 0 || (quads && X && Z && n_images && ok), MCBA_ERR_ARG, "null argument");
-  for (int k = 0; k < n_quads; k++) {
-    const int32_t* q = quads + 4 * (size_t)k;
-    REQUIRE(q[0] >= 0 && q[0] < C && q[1] >= 0 && q[1] < C && q[2] >= 0 && q[2] < B && q[3] >= 0 && q[3] < B, MCBA_ERR_ARG,
-            "quadruple index out of range");
-    REQUIRE(q[0] != q[1], MCBA_ERR_ARG, "quadruple with master == slave");
-  }
-  if (n_quads == 0) return MCBA_OK;
-  REQUIRE(all_finite(poses, 16 * (size_t)C * F * B), MCBA_ERR_NONFINITE, "non-finite pose in the table");
-  auto& hb = ctx->heinit;
-  cudaStream_t s = ctx->stream;
-  const size_t nv = (size_t)C * F * B, nq = (size_t)n_quads;
-  CK(hb.poses.alloc(16 * nv)); CK(hb.valid.alloc(nv));
-  CK(hb.quads.alloc(4 * nq)); CK(hb.X.alloc(16 * nq)); CK(hb.Z.alloc(16 * nq)); CK(hb.n_images.alloc(nq)); CK(hb.ok.alloc(nq));
-  CK(cudaMemcpyAsync(hb.poses.p, poses, sizeof(double) * 16 * nv, cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(hb.valid.p, valid, nv, cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(hb.quads.p, quads, sizeof(int32_t) * 4 * nq, cudaMemcpyHostToDevice, s));
-  HandEyeArgs a{C, F, B, hb.poses.p, hb.valid.p, hb.quads.p, hb.X.p, hb.Z.p, hb.n_images.p, hb.ok.p};
-  k_he_quads<<<n_quads, HE_THREADS, 0, s>>>(a); CKL();
-  CK(cudaMemcpyAsync(X, hb.X.p, sizeof(double) * 16 * nq, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(Z, hb.Z.p, sizeof(double) * 16 * nq, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(n_images, hb.n_images.p, sizeof(int32_t) * nq, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(ok, hb.ok.p, nq, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  return MCBA_OK;
+  return api(ctx, [&] {
+    check_pose_dims(C, F, B);
+    REQUIRE(poses && valid, MCBA_ERR_ARG, "null pose table");
+    REQUIRE(n_quads >= 0, MCBA_ERR_ARG, "negative quadruple count");
+    REQUIRE(n_quads == 0 || (quads && X && Z && n_images && ok), MCBA_ERR_ARG, "null argument");
+    for (int k = 0; k < n_quads; k++) {
+      const int32_t* q = quads + 4 * (size_t)k;
+      REQUIRE(q[0] >= 0 && q[0] < C && q[1] >= 0 && q[1] < C && q[2] >= 0 && q[2] < B && q[3] >= 0 && q[3] < B, MCBA_ERR_ARG,
+              "quadruple index out of range");
+      REQUIRE(q[0] != q[1], MCBA_ERR_ARG, "quadruple with master == slave");
+    }
+    if (n_quads == 0) return;
+    REQUIRE(all_finite(poses, 16 * (size_t)C * F * B), MCBA_ERR_NONFINITE, "non-finite pose in the table");
+    auto& hb = ctx->heinit;
+    cudaStream_t s = ctx->stream;
+    const size_t nv = (size_t)C * F * B, nq = (size_t)n_quads;
+    CK(hb.poses.alloc(16 * nv)); CK(hb.valid.alloc(nv));
+    CK(hb.quads.alloc(4 * nq)); CK(hb.X.alloc(16 * nq)); CK(hb.Z.alloc(16 * nq)); CK(hb.n_images.alloc(nq)); CK(hb.ok.alloc(nq));
+    CK(cudaMemcpyAsync(hb.poses.p, poses, sizeof(double) * 16 * nv, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(hb.valid.p, valid, nv, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(hb.quads.p, quads, sizeof(int32_t) * 4 * nq, cudaMemcpyHostToDevice, s));
+    HandEyeArgs a{C, F, B, hb.poses.p, hb.valid.p, hb.quads.p, hb.X.p, hb.Z.p, hb.n_images.p, hb.ok.p};
+    k_he_quads<<<n_quads, HE_THREADS, 0, s>>>(a); CKL();
+    CK(cudaMemcpyAsync(X, hb.X.p, sizeof(double) * 16 * nq, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(Z, hb.Z.p, sizeof(double) * 16 * nq, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(n_images, hb.n_images.p, sizeof(int32_t) * nq, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(ok, hb.ok.p, nq, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+  });
 }
 
 // probabilistic_guess (hand_eye/helper.py:5-18) for every set: gaussian_kde densities at the points, and the argmax
 int mcba_hand_eye_vote(mcba_ctx* ctx, int32_t n_sets, const int64_t* set_start, const double* points, double* density, int32_t* best) {
-  if (!ctx) return MCBA_ERR_ARG;
-  CK(cudaSetDevice(ctx->device));
-  REQUIRE(n_sets >= 0 && (n_sets == 0 || (set_start && best)), MCBA_ERR_ARG, "null set offsets");
-  if (n_sets == 0) return MCBA_OK;
-  REQUIRE(set_start[0] == 0, MCBA_ERR_ARG, "set offsets must start at 0");
-  for (int k = 0; k < n_sets; k++) REQUIRE(set_start[k + 1] >= set_start[k], MCBA_ERR_ARG, "set offsets must not decrease");
-  const int64_t N = set_start[n_sets];
-  REQUIRE(N < ((int64_t)1 << 31), MCBA_ERR_UNSUPPORTED, "more than 2^31 points");
-  REQUIRE(points && density, MCBA_ERR_ARG, "null argument");
-  for (int k = 0; k < n_sets; k++)
-    REQUIRE(set_start[k + 1] - set_start[k] > 3, MCBA_ERR_DEGENERATE,
-            "set " + std::to_string(k) + " has " + std::to_string(set_start[k + 1] - set_start[k]) +
-            " points: a 3-D kernel density estimate needs at least 4");
-  REQUIRE(all_finite(points, 3 * (size_t)N), MCBA_ERR_NONFINITE, "non-finite point");
-  auto& hb = ctx->heinit;
-  cudaStream_t s = ctx->stream;
-  CK(hb.start.alloc((size_t)n_sets + 1)); CK(hb.points.alloc(3 * (size_t)N)); CK(hb.density.alloc((size_t)N));
-  CK(hb.best.alloc((size_t)n_sets));
-  CK(cudaMemcpyAsync(hb.start.p, set_start, sizeof(int64_t) * (n_sets + 1), cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(hb.points.p, points, sizeof(double) * 3 * N, cudaMemcpyHostToDevice, s));
-  HandEyeVoteArgs a{n_sets, hb.start.p, hb.points.p, hb.density.p, hb.best.p};
-  k_he_vote<<<(n_sets + HE_VOTE_WARPS - 1) / HE_VOTE_WARPS, 32 * HE_VOTE_WARPS, 0, s>>>(a); CKL();
-  CK(cudaMemcpyAsync(density, hb.density.p, sizeof(double) * N, cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(best, hb.best.p, sizeof(int32_t) * n_sets, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  for (int k = 0; k < n_sets; k++)
-    REQUIRE(best[k] >= 0, MCBA_ERR_DEGENERATE, "set " + std::to_string(k) + " has a singular covariance");
-  return MCBA_OK;
+  return api(ctx, [&] {
+    REQUIRE(n_sets >= 0 && (n_sets == 0 || (set_start && best)), MCBA_ERR_ARG, "null set offsets");
+    if (n_sets == 0) return;
+    REQUIRE(set_start[0] == 0, MCBA_ERR_ARG, "set offsets must start at 0");
+    for (int k = 0; k < n_sets; k++) REQUIRE(set_start[k + 1] >= set_start[k], MCBA_ERR_ARG, "set offsets must not decrease");
+    const int64_t N = set_start[n_sets];
+    REQUIRE(N < ((int64_t)1 << 31), MCBA_ERR_UNSUPPORTED, "more than 2^31 points");
+    REQUIRE(points && density, MCBA_ERR_ARG, "null argument");
+    for (int k = 0; k < n_sets; k++)
+      REQUIRE(set_start[k + 1] - set_start[k] > 3, MCBA_ERR_DEGENERATE,
+              "set " + std::to_string(k) + " has " + std::to_string(set_start[k + 1] - set_start[k]) +
+              " points: a 3-D kernel density estimate needs at least 4");
+    REQUIRE(all_finite(points, 3 * (size_t)N), MCBA_ERR_NONFINITE, "non-finite point");
+    auto& hb = ctx->heinit;
+    cudaStream_t s = ctx->stream;
+    CK(hb.start.alloc((size_t)n_sets + 1)); CK(hb.points.alloc(3 * (size_t)N)); CK(hb.density.alloc((size_t)N));
+    CK(hb.best.alloc((size_t)n_sets));
+    CK(cudaMemcpyAsync(hb.start.p, set_start, sizeof(int64_t) * (n_sets + 1), cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(hb.points.p, points, sizeof(double) * 3 * N, cudaMemcpyHostToDevice, s));
+    HandEyeVoteArgs a{n_sets, hb.start.p, hb.points.p, hb.density.p, hb.best.p};
+    k_he_vote<<<(n_sets + HE_VOTE_WARPS - 1) / HE_VOTE_WARPS, 32 * HE_VOTE_WARPS, 0, s>>>(a); CKL();
+    CK(cudaMemcpyAsync(density, hb.density.p, sizeof(double) * N, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(best, hb.best.p, sizeof(int32_t) * n_sets, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    for (int k = 0; k < n_sets; k++)
+      REQUIRE(best[k] >= 0, MCBA_ERR_DEGENERATE, "set " + std::to_string(k) + " has a singular covariance");
+  });
 }
 
 namespace {
 
 // the camera of the undistortion entries: [fx fy cx cy skew dist...] with 5 + nd values of `model`
-int check_camera(mcba_ctx* ctx, int32_t model, const double* camera) {
+void check_camera(int32_t model, const double* camera) {
   REQUIRE(model >= MODEL_STANDARD && model <= MODEL_TILTED, MCBA_ERR_ARG, "unknown camera model");
   REQUIRE(camera, MCBA_ERR_ARG, "null camera");
   REQUIRE(all_finite(camera, 5 + (size_t)model_nd(model)), MCBA_ERR_NONFINITE, "non-finite camera parameter");
   REQUIRE(camera[0] != 0.0 && camera[1] != 0.0, MCBA_ERR_ARG, "zero focal length");
-  return MCBA_OK;
 }
 
 UndistortCamera make_camera(int model, const double* camera, int w, int h) {
@@ -1460,23 +1462,22 @@ UndistortCamera make_camera(int model, const double* camera, int w, int h) {
 }
 
 // the bicubic weight table, built on the context stream at first use
-int ensure_cubic_table(mcba_ctx* ctx) {
+void ensure_cubic_table(mcba_ctx* ctx) {
   auto& U = ctx->und;
-  if (U.tab_ready) return MCBA_OK;
+  if (U.tab_ready) return;
   CK(U.tab.alloc(16 * (size_t)UND_TAB_ENTRIES));
   k_cubic_table<<<(UND_TAB_ENTRIES + UND_THREADS - 1) / UND_THREADS, UND_THREADS, 0, ctx->stream>>>(U.tab.p); CKL();
   U.tab_ready = true;
-  return MCBA_OK;
 }
 
 // the resident fixed-point map of a key, computed on ctx->stream by launch(float map or null, org, idx) when it is not resident yet (or
 // when the float map is asked for).  The key is the camera vector for an undistortion map, the camera vector followed by R and P for a
 // rectification map: its length tells the two apart.
-int resident_map(mcba_ctx* ctx, int model, const double* key, size_t nk, int w, int h, float* map_out,
-                 const std::function<void(float2*, uint32_t*, uint16_t*)>& launch, mcba_ctx::UndistortMap** out) {
+mcba_ctx::UndistortMap* resident_map(mcba_ctx* ctx, int model, const double* key, size_t nk, int w, int h, float* map_out,
+                                     const std::function<void(float2*, uint32_t*, uint16_t*)>& launch) {
   auto& U = ctx->und;
   cudaStream_t s = ctx->stream;
-  { int r = ensure_cubic_table(ctx); if (r) return r; }
+  ensure_cubic_table(ctx);
   const size_t npx = (size_t)w * h;
   mcba_ctx::UndistortMap* m = nullptr;
   for (auto& e : U.maps)
@@ -1505,24 +1506,24 @@ int resident_map(mcba_ctx* ctx, int model, const double* key, size_t nk, int w, 
     }
   }
   m->used = ++U.tick;
-  *out = m;
-  return MCBA_OK;
+  return m;
 }
 
 // the resident undistortion map of a camera (k_undistort_map)
-int undistortion_map(mcba_ctx* ctx, int model, const double* camera, int w, int h, float* map_out, mcba_ctx::UndistortMap** out) {
+mcba_ctx::UndistortMap* undistortion_map(mcba_ctx* ctx, int model, const double* camera, int w, int h, float* map_out) {
   const UndistortCamera c = make_camera(model, camera, w, h);
   const dim3 grid((w + UND_THREADS - 1) / UND_THREADS, h);
   cudaStream_t s = ctx->stream;
   return resident_map(ctx, model, camera, 5 + (size_t)model_nd(model), w, h, map_out, [&](float2* f, uint32_t* org, uint16_t* idx) {
     with_model(model, false, [&](auto M, auto) { k_undistort_map<decltype(M)::value><<<grid, UND_THREADS, 0, s>>>(c, f, org, idx); });
-  }, out);
+  });
 }
 
 // rr = P R and ir = rr^-1 (row-major 3x3) for the rectification entries; a singular or non-finite P R fails with MCBA_ERR_ARG
-int make_rectify_camera(mcba_ctx* ctx, int model, const double* camera, const double* R, const double* P, int w, int h, RectifyCamera& rc) {
+RectifyCamera make_rectify_camera(int model, const double* camera, const double* R, const double* P, int w, int h) {
   REQUIRE(R && P, MCBA_ERR_ARG, "null R or P");
   REQUIRE(all_finite(R, 9) && all_finite(P, 9), MCBA_ERR_NONFINITE, "non-finite R or P");
+  RectifyCamera rc;
   rc.cam = make_camera(model, camera, w, h);
   for (int i = 0; i < 3; i++)
     for (int j = 0; j < 3; j++) rc.rr[3 * i + j] = P[3 * i] * R[j] + P[3 * i + 1] * R[3 + j] + P[3 * i + 2] * R[6 + j];
@@ -1544,17 +1545,16 @@ int make_rectify_camera(mcba_ctx* ctx, int model, const double* camera, const do
   for (int i = 0; i < 3; i++)
     for (int j = 0; j < 3; j++) rc.ir[3 * i + j] = I[i][j] / A[i][i];
   REQUIRE(all_finite(rc.ir, 9), MCBA_ERR_ARG, "P R is singular");
-  return MCBA_OK;
+  return rc;
 }
 
 // shared memory of a k_rectify_map CTA
 size_t rectify_smem(int model, int w) { return 3 * sizeof(double) * (size_t)rectify_walk_len(model, w); }
 
 // the resident rectification map of a camera under (R, P) (k_rectify_map)
-int rectification_map(mcba_ctx* ctx, int model, const double* camera, const double* R, const double* P, int w, int h, float* map_out,
-                      mcba_ctx::UndistortMap** out) {
-  RectifyCamera rc;
-  { int r = make_rectify_camera(ctx, model, camera, R, P, w, h, rc); if (r) return r; }
+mcba_ctx::UndistortMap* rectification_map(mcba_ctx* ctx, int model, const double* camera, const double* R, const double* P, int w, int h,
+                                          float* map_out) {
+  const RectifyCamera rc = make_rectify_camera(model, camera, R, P, w, h);
   const size_t smem = rectify_smem(model, w);
   REQUIRE(smem <= (size_t)RECT_SMEM_MAX, MCBA_ERR_ARG, "map too wide for one row's walk in shared memory");
   const size_t nk = 5 + (size_t)model_nd(model);
@@ -1563,14 +1563,14 @@ int rectification_map(mcba_ctx* ctx, int model, const double* camera, const doub
   cudaStream_t s = ctx->stream;
   return resident_map(ctx, model, key.data(), key.size(), w, h, map_out, [&](float2* f, uint32_t* org, uint16_t* idx) {
     with_model(model, false, [&](auto M, auto) { k_rectify_map<decltype(M)::value><<<h, UND_THREADS, smem, s>>>(rc, f, org, idx); });
-  }, out);
+  });
 }
 
 // cv2.remap(src[i], map, None, INTER_CUBIC) for n images through the resident map m of (width, height), host to host.  Chunks of images
 // go through pinned staging on UND_STREAMS streams in turn: while the host copies one chunk into its staging buffer, earlier chunks are
 // in flight (copy in, k_remap_cubic, copy out) on the other streams.
-int remap_images(mcba_ctx* ctx, const mcba_ctx::UndistortMap* m, int32_t width, int32_t height, int32_t n, int32_t src_width,
-                 int32_t src_height, int32_t channels, const uint8_t* const* src, uint8_t* const* dst) {
+void remap_images(mcba_ctx* ctx, const mcba_ctx::UndistortMap* m, int32_t width, int32_t height, int32_t n, int32_t src_width,
+                  int32_t src_height, int32_t channels, const uint8_t* const* src, uint8_t* const* dst) {
   auto& U = ctx->und;
   const size_t in_bytes = (size_t)src_width * src_height * channels, out_bytes = (size_t)width * height * channels;
   const size_t chunk_bytes = (size_t)8 << 20;
@@ -1599,18 +1599,17 @@ int remap_images(mcba_ctx* ctx, const mcba_ctx::UndistortMap* m, int32_t width, 
   RemapArgs a{};
   a.org = m->org.p; a.idx = m->idx.p; a.tab = U.tab.p; a.ws = src_width; a.hs = src_height; a.wm = width; a.hm = height;
   std::vector<int> pending(n_slots, -1);                    // chunk whose results a slot holds
-  auto drain = [&](int slot) -> int {
+  auto drain = [&](int slot) {
     const int ck = pending[slot];
-    if (ck < 0) return MCBA_OK;
+    if (ck < 0) return;
     CK(cudaEventSynchronize(U.done[slot]));
     const int first = ck * per_chunk, cnt = std::min(per_chunk, n - first);
     for (int j = 0; j < cnt; j++) std::memcpy(dst[first + j], U.host_out[slot] + j * out_bytes, out_bytes);
     pending[slot] = -1;
-    return MCBA_OK;
   };
   for (int ck = 0; ck < n_chunks; ck++) {
     const int slot = ck % n_slots, first = ck * per_chunk, cnt = std::min(per_chunk, n - first);
-    { int r = drain(slot); if (r) return r; }
+    drain(slot);
     for (int j = 0; j < cnt; j++) std::memcpy(U.host_in[slot] + j * in_bytes, src[first + j], in_bytes);
     cudaStream_t s = U.st[slot];
     CK(cudaMemcpyAsync(U.dev_in[slot].p, U.host_in[slot], cnt * in_bytes, cudaMemcpyHostToDevice, s));
@@ -1623,35 +1622,31 @@ int remap_images(mcba_ctx* ctx, const mcba_ctx::UndistortMap* m, int32_t width, 
     CK(cudaEventRecord(U.done[slot], s));
     pending[slot] = ck;
   }
-  for (int k = 0; k < n_slots; k++) { int r = drain((n_chunks + k) % n_slots); if (r) return r; }
-  return MCBA_OK;
+  for (int k = 0; k < n_slots; k++) drain((n_chunks + k) % n_slots);
 }
 
 // the checks every image entry makes before its map is looked up
-int check_images(mcba_ctx* ctx, int32_t width, int32_t height, int32_t n, int32_t src_width, int32_t src_height, int32_t channels,
-                 int32_t dtype, const uint8_t* const* src, uint8_t* const* dst) {
+void check_images(int32_t width, int32_t height, int32_t n, int32_t src_width, int32_t src_height, int32_t channels,
+                  int32_t dtype, const uint8_t* const* src, uint8_t* const* dst) {
   REQUIRE(dtype == MCBA_IMAGE_UINT8, MCBA_ERR_ARG, "unsupported image dtype: only 8-bit unsigned images are remapped");
   REQUIRE(channels == 1 || channels == 3, MCBA_ERR_ARG, "unsupported channel count: 1 or 3 channels are remapped");
   REQUIRE(width > 0 && height > 0 && height <= 65535, MCBA_ERR_ARG, "map size out of range");
   REQUIRE(src_width > 0 && src_height > 0, MCBA_ERR_ARG, "empty source image");
   REQUIRE(n >= 0, MCBA_ERR_ARG, "negative image count");
-  if (n == 0) return MCBA_OK;
+  if (n == 0) return;
   REQUIRE(src && dst, MCBA_ERR_ARG, "null image list");
   for (int i = 0; i < n; i++) REQUIRE(src[i] && dst[i], MCBA_ERR_ARG, "null image " + std::to_string(i));
-  return MCBA_OK;
 }
 
 // point entries: copy in, one thread per point, copy out.  R and P (both or neither) make it the rectification of the points.
-int run_points(mcba_ctx* ctx, bool project, int32_t model, const double* camera, int64_t n, const double* in, double* out,
-               const double* R = nullptr, const double* P = nullptr) {
-  if (!ctx) return MCBA_ERR_ARG;
-  CK(cudaSetDevice(ctx->device));
-  { int r = check_camera(ctx, model, camera); if (r) return r; }
+void run_points(mcba_ctx* ctx, bool project, int32_t model, const double* camera, int64_t n, const double* in, double* out,
+                const double* R = nullptr, const double* P = nullptr) {
+  check_camera(model, camera);
   const bool rectify = R || P;
   RectifyCamera rc;
-  if (rectify) { int r = make_rectify_camera(ctx, model, camera, R, P, 0, 0, rc); if (r) return r; }
+  if (rectify) rc = make_rectify_camera(model, camera, R, P, 0, 0);
   REQUIRE(n >= 0, MCBA_ERR_ARG, "negative point count");
-  if (n == 0) return MCBA_OK;
+  if (n == 0) return;
   REQUIRE(in && out, MCBA_ERR_ARG, "null argument");
   auto& U = ctx->und;
   cudaStream_t s = ctx->stream;
@@ -1669,88 +1664,82 @@ int run_points(mcba_ctx* ctx, bool project, int32_t model, const double* camera,
   CKL();
   CK(cudaMemcpyAsync(out, U.pout.p, sizeof(double) * 2 * n, cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
-  return MCBA_OK;
 }
 
 }  // namespace
 
 // initUndistortRectifyMap(K, dist, None, K, (width, height)) of one camera, kept resident for mcba_undistort_images
 int mcba_undistort_map(mcba_ctx* ctx, int32_t model, const double* camera, int32_t width, int32_t height, float* map) {
-  if (!ctx) return MCBA_ERR_ARG;
-  CK(cudaSetDevice(ctx->device));
-  { int r = check_camera(ctx, model, camera); if (r) return r; }
-  REQUIRE(width > 0 && height > 0 && height <= 65535, MCBA_ERR_ARG, "map size out of range");
-  mcba_ctx::UndistortMap* m = nullptr;
-  int r = undistortion_map(ctx, model, camera, width, height, map, &m);
-  if (r) return r;
-  CK(cudaStreamSynchronize(ctx->stream));
-  return MCBA_OK;
+  return api(ctx, [&] {
+    check_camera(model, camera);
+    REQUIRE(width > 0 && height > 0 && height <= 65535, MCBA_ERR_ARG, "map size out of range");
+    undistortion_map(ctx, model, camera, width, height, map);
+    CK(cudaStreamSynchronize(ctx->stream));
+  });
 }
 
 // cv2.remap(src[i], map, None, INTER_CUBIC) for n images of one camera through its undistortion map, host to host (remap_images)
 int mcba_undistort_images(mcba_ctx* ctx, int32_t model, const double* camera, int32_t width, int32_t height, int32_t n,
                           int32_t src_width, int32_t src_height, int32_t channels, int32_t dtype, const uint8_t* const* src,
                           uint8_t* const* dst) {
-  if (!ctx) return MCBA_ERR_ARG;
-  CK(cudaSetDevice(ctx->device));
-  { int r = check_camera(ctx, model, camera); if (r) return r; }
-  { int r = check_images(ctx, width, height, n, src_width, src_height, channels, dtype, src, dst); if (r || n == 0) return r; }
-  mcba_ctx::UndistortMap* m = nullptr;
-  { int r = undistortion_map(ctx, model, camera, width, height, nullptr, &m); if (r) return r; }
-  return remap_images(ctx, m, width, height, n, src_width, src_height, channels, src, dst);
+  return api(ctx, [&] {
+    check_camera(model, camera);
+    check_images(width, height, n, src_width, src_height, channels, dtype, src, dst);
+    if (n == 0) return;
+    const mcba_ctx::UndistortMap* m = undistortion_map(ctx, model, camera, width, height, nullptr);
+    remap_images(ctx, m, width, height, n, src_width, src_height, channels, src, dst);
+  });
 }
 
 // initUndistortRectifyMap(K, dist, R, P, (width, height)) of one camera, kept resident for mcba_rectify_images
 int mcba_rectify_map(mcba_ctx* ctx, int32_t model, const double* camera, const double* R, const double* P, int32_t width, int32_t height,
                      float* map) {
-  if (!ctx) return MCBA_ERR_ARG;
-  CK(cudaSetDevice(ctx->device));
-  { int r = check_camera(ctx, model, camera); if (r) return r; }
-  REQUIRE(width > 0 && height > 0 && height <= 65535, MCBA_ERR_ARG, "map size out of range");
-  mcba_ctx::UndistortMap* m = nullptr;
-  int r = rectification_map(ctx, model, camera, R, P, width, height, map, &m);
-  if (r) return r;
-  CK(cudaStreamSynchronize(ctx->stream));
-  return MCBA_OK;
+  return api(ctx, [&] {
+    check_camera(model, camera);
+    REQUIRE(width > 0 && height > 0 && height <= 65535, MCBA_ERR_ARG, "map size out of range");
+    rectification_map(ctx, model, camera, R, P, width, height, map);
+    CK(cudaStreamSynchronize(ctx->stream));
+  });
 }
 
 // cv2.remap(src[i], map, None, INTER_CUBIC) for n images of one camera through its rectification map, host to host (remap_images)
 int mcba_rectify_images(mcba_ctx* ctx, int32_t model, const double* camera, const double* R, const double* P, int32_t width,
                         int32_t height, int32_t n, int32_t src_width, int32_t src_height, int32_t channels, int32_t dtype,
                         const uint8_t* const* src, uint8_t* const* dst) {
-  if (!ctx) return MCBA_ERR_ARG;
-  CK(cudaSetDevice(ctx->device));
-  { int r = check_camera(ctx, model, camera); if (r) return r; }
-  { int r = check_images(ctx, width, height, n, src_width, src_height, channels, dtype, src, dst); if (r || n == 0) return r; }
-  mcba_ctx::UndistortMap* m = nullptr;
-  { int r = rectification_map(ctx, model, camera, R, P, width, height, nullptr, &m); if (r) return r; }
-  return remap_images(ctx, m, width, height, n, src_width, src_height, channels, src, dst);
+  return api(ctx, [&] {
+    check_camera(model, camera);
+    check_images(width, height, n, src_width, src_height, channels, dtype, src, dst);
+    if (n == 0) return;
+    const mcba_ctx::UndistortMap* m = rectification_map(ctx, model, camera, R, P, width, height, nullptr);
+    remap_images(ctx, m, width, height, n, src_width, src_height, channels, src, dst);
+  });
 }
 
 int mcba_rectify_points(mcba_ctx* ctx, int32_t model, const double* camera, const double* R, const double* P, int64_t n,
                         const double* pixels, double* rectified) {
-  if (!ctx) return MCBA_ERR_ARG;
-  REQUIRE(R && P, MCBA_ERR_ARG, "null R or P");
-  return run_points(ctx, false, model, camera, n, pixels, rectified, R, P);
+  return api(ctx, [&] {
+    REQUIRE(R && P, MCBA_ERR_ARG, "null R or P");
+    run_points(ctx, false, model, camera, n, pixels, rectified, R, P);
+  });
 }
 
 int mcba_project_points(mcba_ctx* ctx, int32_t model, const double* camera, int64_t n, const double* points, double* pixels) {
-  return run_points(ctx, true, model, camera, n, points, pixels);
+  return api(ctx, [&] { run_points(ctx, true, model, camera, n, points, pixels); });
 }
 
 int mcba_undistort_points(mcba_ctx* ctx, int32_t model, const double* camera, int64_t n, const double* pixels, double* undistorted) {
-  return run_points(ctx, false, model, camera, n, pixels, undistorted);
+  return api(ctx, [&] { run_points(ctx, false, model, camera, n, pixels, undistorted); });
 }
 
 // the fixed-point bicubic weights k_remap_cubic reads, int32[1024][16]
 int mcba_remap_cubic_table(mcba_ctx* ctx, int32_t* table) {
-  if (!ctx || !table) return MCBA_ERR_ARG;
-  CK(cudaSetDevice(ctx->device));
-  auto& U = ctx->und;
-  { int r = ensure_cubic_table(ctx); if (r) return r; }
-  CK(cudaMemcpyAsync(table, U.tab.p, sizeof(int32_t) * 16 * UND_TAB_ENTRIES, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  return MCBA_OK;
+  return api(ctx, [&] {
+    REQUIRE(table, MCBA_ERR_ARG, "null table");
+    auto& U = ctx->und;
+    ensure_cubic_table(ctx);
+    CK(cudaMemcpyAsync(table, U.tab.p, sizeof(int32_t) * 16 * UND_TAB_ENTRIES, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+  });
 }
 
 namespace {
@@ -1764,634 +1753,630 @@ int64_t tri_chunk(int64_t N, size_t bytes) { return std::max<int64_t>(1, std::mi
 // launch, the points, flags and rms come out
 int mcba_triangulate(mcba_ctx* ctx, int32_t model, int32_t C, const double* cameras, const double* poses, int64_t N,
                      const double* pixels, const uint8_t* valid, double* points, uint8_t* ok, double* rms) {
-  if (!ctx) return MCBA_ERR_ARG;
-  CK(cudaSetDevice(ctx->device));
-  REQUIRE(model >= MODEL_STANDARD && model <= MODEL_TILTED, MCBA_ERR_ARG, "unknown camera model");
-  REQUIRE(C >= 1 && C <= MCBA_TRI_MAX_CAMERAS, MCBA_ERR_ARG, "camera count out of range (1 .. " + std::to_string(MCBA_TRI_MAX_CAMERAS) + ")");
-  REQUIRE(N >= 0, MCBA_ERR_ARG, "negative point count");
-  REQUIRE(cameras && poses, MCBA_ERR_ARG, "null cameras or poses");
-  const int kd = 5 + model_nd(model);
-  for (int c = 0; c < C; c++) {
-    int r = check_camera(ctx, model, cameras + (size_t)kd * c);
-    if (r) { ctx->err = "camera " + std::to_string(c) + ": " + ctx->err; return r; }
-  }
-  REQUIRE(all_finite(poses, 16 * (size_t)C), MCBA_ERR_NONFINITE, "non-finite camera pose");
-  if (N == 0) return MCBA_OK;
-  REQUIRE(pixels && valid && points && ok && rms, MCBA_ERR_ARG, "null argument");
-  auto& T = ctx->tri;
-  cudaStream_t s = ctx->stream;
-  std::vector<double> cams((size_t)TRI_KD * C, 0.0);
-  for (int c = 0; c < C; c++) std::copy(cameras + (size_t)kd * c, cameras + (size_t)kd * (c + 1), cams.begin() + (size_t)TRI_KD * c);
-  const int lanes = tri_lanes(C), nk = (C + lanes - 1) / lanes;
-  const int64_t chunk = tri_chunk(N, (size_t)C * (sizeof(double2) + 1) + 4 * sizeof(double) + 1);
-  CK(T.cams.alloc(cams.size())); CK(T.poses.alloc(16 * (size_t)C));
-  CK(T.px.alloc((size_t)C * chunk)); CK(T.valid.alloc((size_t)C * chunk));
-  CK(T.points.alloc(3 * (size_t)chunk)); CK(T.rms.alloc(chunk)); CK(T.ok.alloc(chunk));
-  CK(cudaMemcpyAsync(T.cams.p, cams.data(), sizeof(double) * cams.size(), cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(T.poses.p, poses, sizeof(double) * 16 * C, cudaMemcpyHostToDevice, s));
-  for (int64_t p0 = 0; p0 < N; p0 += chunk) {
-    const int64_t n = std::min(chunk, N - p0);
+  return api(ctx, [&] {
+    REQUIRE(model >= MODEL_STANDARD && model <= MODEL_TILTED, MCBA_ERR_ARG, "unknown camera model");
+    REQUIRE(C >= 1 && C <= MCBA_TRI_MAX_CAMERAS, MCBA_ERR_ARG, "camera count out of range (1 .. " + std::to_string(MCBA_TRI_MAX_CAMERAS) + ")");
+    REQUIRE(N >= 0, MCBA_ERR_ARG, "negative point count");
+    REQUIRE(cameras && poses, MCBA_ERR_ARG, "null cameras or poses");
+    const int kd = 5 + model_nd(model);
     for (int c = 0; c < C; c++) {
-      CK(cudaMemcpyAsync(T.px.p + (size_t)c * n, pixels + 2 * ((size_t)c * N + p0), sizeof(double2) * n, cudaMemcpyHostToDevice, s));
-      CK(cudaMemcpyAsync(T.valid.p + (size_t)c * n, valid + (size_t)c * N + p0, n, cudaMemcpyHostToDevice, s));
+      try {
+        check_camera(model, cameras + (size_t)kd * c);
+      } catch (Failure& f) {
+        f.msg = "camera " + std::to_string(c) + ": " + f.msg;
+        throw;
+      }
     }
-    TriArgs a{C, nk, n, T.cams.p, T.poses.p, T.px.p, T.valid.p, T.points.p, T.ok.p, T.rms.p};
-    const unsigned blocks = (unsigned)((n * lanes + TRI_THREADS - 1) / TRI_THREADS);
-    with_model(model, false, [&](auto M, auto) {
-      with_lanes(lanes, [&](auto L) {
-        k_triangulate<decltype(M)::value, decltype(L)::value><<<blocks, TRI_THREADS, tri_smem(nk), s>>>(a);
+    REQUIRE(all_finite(poses, 16 * (size_t)C), MCBA_ERR_NONFINITE, "non-finite camera pose");
+    if (N == 0) return;
+    REQUIRE(pixels && valid && points && ok && rms, MCBA_ERR_ARG, "null argument");
+    auto& T = ctx->tri;
+    cudaStream_t s = ctx->stream;
+    std::vector<double> cams((size_t)TRI_KD * C, 0.0);
+    for (int c = 0; c < C; c++) std::copy(cameras + (size_t)kd * c, cameras + (size_t)kd * (c + 1), cams.begin() + (size_t)TRI_KD * c);
+    const int lanes = tri_lanes(C), nk = (C + lanes - 1) / lanes;
+    const int64_t chunk = tri_chunk(N, (size_t)C * (sizeof(double2) + 1) + 4 * sizeof(double) + 1);
+    CK(T.cams.alloc(cams.size())); CK(T.poses.alloc(16 * (size_t)C));
+    CK(T.px.alloc((size_t)C * chunk)); CK(T.valid.alloc((size_t)C * chunk));
+    CK(T.points.alloc(3 * (size_t)chunk)); CK(T.rms.alloc(chunk)); CK(T.ok.alloc(chunk));
+    CK(cudaMemcpyAsync(T.cams.p, cams.data(), sizeof(double) * cams.size(), cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(T.poses.p, poses, sizeof(double) * 16 * C, cudaMemcpyHostToDevice, s));
+    for (int64_t p0 = 0; p0 < N; p0 += chunk) {
+      const int64_t n = std::min(chunk, N - p0);
+      for (int c = 0; c < C; c++) {
+        CK(cudaMemcpyAsync(T.px.p + (size_t)c * n, pixels + 2 * ((size_t)c * N + p0), sizeof(double2) * n, cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(T.valid.p + (size_t)c * n, valid + (size_t)c * N + p0, n, cudaMemcpyHostToDevice, s));
+      }
+      TriArgs a{C, nk, n, T.cams.p, T.poses.p, T.px.p, T.valid.p, T.points.p, T.ok.p, T.rms.p};
+      const unsigned blocks = (unsigned)((n * lanes + TRI_THREADS - 1) / TRI_THREADS);
+      with_model(model, false, [&](auto M, auto) {
+        with_lanes(lanes, [&](auto L) {
+          k_triangulate<decltype(M)::value, decltype(L)::value><<<blocks, TRI_THREADS, tri_smem(nk), s>>>(a);
+        });
       });
-    });
-    CKL();
-    CK(cudaMemcpyAsync(points + 3 * p0, T.points.p, sizeof(double) * 3 * n, cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(ok + p0, T.ok.p, n, cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(rms + p0, T.rms.p, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
-  }
-  CK(cudaStreamSynchronize(s));
-  return MCBA_OK;
+      CKL();
+      CK(cudaMemcpyAsync(points + 3 * p0, T.points.p, sizeof(double) * 3 * n, cudaMemcpyDeviceToHost, s));
+      CK(cudaMemcpyAsync(ok + p0, T.ok.p, n, cudaMemcpyDeviceToHost, s));
+      CK(cudaMemcpyAsync(rms + p0, T.rms.p, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
+    }
+    CK(cudaStreamSynchronize(s));
+  });
 }
 
 // cv2.triangulatePoints (k_triangulate_linear), chunk by chunk
 int mcba_triangulate_linear(mcba_ctx* ctx, const double* P1, const double* P2, int64_t N, const double* x1, const double* x2, double* out) {
-  if (!ctx) return MCBA_ERR_ARG;
-  CK(cudaSetDevice(ctx->device));
-  REQUIRE(P1 && P2, MCBA_ERR_ARG, "null projection matrix");
-  REQUIRE(all_finite(P1, 12) && all_finite(P2, 12), MCBA_ERR_NONFINITE, "non-finite projection matrix");
-  REQUIRE(N >= 0, MCBA_ERR_ARG, "negative point count");
-  if (N == 0) return MCBA_OK;
-  REQUIRE(x1 && x2 && out, MCBA_ERR_ARG, "null argument");
-  auto& T = ctx->tri;
-  cudaStream_t s = ctx->stream;
-  const int64_t chunk = tri_chunk(N, 8 * sizeof(double));
-  CK(T.lin.alloc(8 * (size_t)chunk));
-  TriLinearArgs a{};
-  for (int j = 0; j < 12; j++) { a.P[0][j] = P1[j]; a.P[1][j] = P2[j]; }
-  for (int64_t p0 = 0; p0 < N; p0 += chunk) {
-    const int64_t n = std::min(chunk, N - p0);
-    double* dx = T.lin.p;                            // [x1 x; x1 y; x2 x; x2 y] of the chunk, then [4][n] out
-    for (int r = 0; r < 2; r++) {
-      CK(cudaMemcpyAsync(dx + r * n, x1 + r * N + p0, sizeof(double) * n, cudaMemcpyHostToDevice, s));
-      CK(cudaMemcpyAsync(dx + (2 + r) * n, x2 + r * N + p0, sizeof(double) * n, cudaMemcpyHostToDevice, s));
+  return api(ctx, [&] {
+    REQUIRE(P1 && P2, MCBA_ERR_ARG, "null projection matrix");
+    REQUIRE(all_finite(P1, 12) && all_finite(P2, 12), MCBA_ERR_NONFINITE, "non-finite projection matrix");
+    REQUIRE(N >= 0, MCBA_ERR_ARG, "negative point count");
+    if (N == 0) return;
+    REQUIRE(x1 && x2 && out, MCBA_ERR_ARG, "null argument");
+    auto& T = ctx->tri;
+    cudaStream_t s = ctx->stream;
+    const int64_t chunk = tri_chunk(N, 8 * sizeof(double));
+    CK(T.lin.alloc(8 * (size_t)chunk));
+    TriLinearArgs a{};
+    for (int j = 0; j < 12; j++) { a.P[0][j] = P1[j]; a.P[1][j] = P2[j]; }
+    for (int64_t p0 = 0; p0 < N; p0 += chunk) {
+      const int64_t n = std::min(chunk, N - p0);
+      double* dx = T.lin.p;                            // [x1 x; x1 y; x2 x; x2 y] of the chunk, then [4][n] out
+      for (int r = 0; r < 2; r++) {
+        CK(cudaMemcpyAsync(dx + r * n, x1 + r * N + p0, sizeof(double) * n, cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(dx + (2 + r) * n, x2 + r * N + p0, sizeof(double) * n, cudaMemcpyHostToDevice, s));
+      }
+      a.n = n; a.x[0] = dx; a.x[1] = dx + 2 * n; a.out = dx + 4 * n;
+      k_triangulate_linear<<<(unsigned)((2 * n + TRI_THREADS - 1) / TRI_THREADS), TRI_THREADS, tri_smem(1), s>>>(a);
+      CKL();
+      for (int j = 0; j < 4; j++) CK(cudaMemcpyAsync(out + j * N + p0, a.out + j * n, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
     }
-    a.n = n; a.x[0] = dx; a.x[1] = dx + 2 * n; a.out = dx + 4 * n;
-    k_triangulate_linear<<<(unsigned)((2 * n + TRI_THREADS - 1) / TRI_THREADS), TRI_THREADS, tri_smem(1), s>>>(a);
-    CKL();
-    for (int j = 0; j < 4; j++) CK(cudaMemcpyAsync(out + j * N + p0, a.out + j * n, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
-  }
-  CK(cudaStreamSynchronize(s));
-  return MCBA_OK;
+    CK(cudaStreamSynchronize(s));
+  });
 }
 
 int mcba_table_download(mcba_ctx* ctx, uint8_t* valid, double* points) {
-  if (!ctx) return MCBA_ERR_ARG;
-  REQUIRE(ctx->table, MCBA_ERR_STATE, "no resident table (mcba_table_upload / mcba_table_from_detections)");
-  CK(cudaSetDevice(ctx->device));
-  const size_t dense = table_dense(ctx);
-  if (valid && dense) CK(cudaMemcpyAsync(valid, ctx->valid_mask.p, dense, cudaMemcpyDeviceToHost, ctx->stream));
-  if (points && dense) CK(cudaMemcpyAsync(points, ctx->dense_pts.p, dense * sizeof(double2), cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  return MCBA_OK;
+  return api(ctx, [&] {
+    REQUIRE(ctx->table, MCBA_ERR_STATE, "no resident table (mcba_table_upload / mcba_table_from_detections)");
+    const size_t dense = table_dense(ctx);
+    if (valid && dense) CK(cudaMemcpyAsync(valid, ctx->valid_mask.p, dense, cudaMemcpyDeviceToHost, ctx->stream));
+    if (points && dense) CK(cudaMemcpyAsync(points, ctx->dense_pts.p, dense * sizeof(double2), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+  });
 }
 
 int mcba_table_set_inliers(mcba_ctx* ctx, const uint8_t* mask) {
-  if (!ctx) return MCBA_ERR_ARG;
-  REQUIRE(ctx->table, MCBA_ERR_STATE, "no resident table (mcba_table_upload / mcba_table_from_detections)");
-  CK(cudaSetDevice(ctx->device));
-  const size_t dense = table_dense(ctx);
-  if (dense) {
-    if (mask) {
-      CK(cudaMemcpyAsync(ctx->inlier_mask.p, mask, dense, cudaMemcpyHostToDevice, ctx->stream));
-      k_mask_and<<<(unsigned)((dense + 255) / 256), 256, 0, ctx->stream>>>(ctx->inlier_mask.p, ctx->valid_mask.p, dense, ctx->inlier_mask.p); CKL();
-    } else {
-      CK(cudaMemcpyAsync(ctx->inlier_mask.p, ctx->valid_mask.p, dense, cudaMemcpyDeviceToDevice, ctx->stream));
+  return api(ctx, [&] {
+    REQUIRE(ctx->table, MCBA_ERR_STATE, "no resident table (mcba_table_upload / mcba_table_from_detections)");
+    const size_t dense = table_dense(ctx);
+    if (dense) {
+      if (mask) {
+        CK(cudaMemcpyAsync(ctx->inlier_mask.p, mask, dense, cudaMemcpyHostToDevice, ctx->stream));
+        k_mask_and<<<(unsigned)((dense + 255) / 256), 256, 0, ctx->stream>>>(ctx->inlier_mask.p, ctx->valid_mask.p, dense, ctx->inlier_mask.p); CKL();
+      } else {
+        CK(cudaMemcpyAsync(ctx->inlier_mask.p, ctx->valid_mask.p, dense, cudaMemcpyDeviceToDevice, ctx->stream));
+      }
     }
-  }
-  CK(cudaStreamSynchronize(ctx->stream));      // the host mask is borrowed only for the call
-  ctx->errors_current = false;
-  if (ctx->table_selected == MCBA_TABLE_INLIERS) ctx->table_selected = -1;     // the packed set no longer matches the mask
-  return MCBA_OK;
+    CK(cudaStreamSynchronize(ctx->stream));      // the host mask is borrowed only for the call
+    ctx->errors_current = false;
+    if (ctx->table_selected == MCBA_TABLE_INLIERS) ctx->table_selected = -1;     // the packed set no longer matches the mask
+  });
 }
 
 int mcba_table_get_inliers(mcba_ctx* ctx, uint8_t* mask) {
-  if (!ctx || !mask) return MCBA_ERR_ARG;
-  REQUIRE(ctx->table, MCBA_ERR_STATE, "no resident table (mcba_table_upload / mcba_table_from_detections)");
-  CK(cudaSetDevice(ctx->device));
-  const size_t dense = table_dense(ctx);
-  if (dense) CK(cudaMemcpyAsync(mask, ctx->inlier_mask.p, dense, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  return MCBA_OK;
+  return api(ctx, [&] {
+    REQUIRE(mask, MCBA_ERR_ARG, "null mask");
+    REQUIRE(ctx->table, MCBA_ERR_STATE, "no resident table (mcba_table_upload / mcba_table_from_detections)");
+    const size_t dense = table_dense(ctx);
+    if (dense) CK(cudaMemcpyAsync(mask, ctx->inlier_mask.p, dense, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+  });
 }
 
-int mcba_table_select(mcba_ctx* ctx, int which, int64_t* n_corners) {
-  if (!ctx) return MCBA_ERR_ARG;
+namespace {
+
+// the resident table's corners under `which` become the packed problem (kept when already selected); returns their number
+int64_t select_table(mcba_ctx* ctx, int which) {
   REQUIRE(ctx->table, MCBA_ERR_STATE, "no resident table (mcba_table_upload / mcba_table_from_detections)");
   REQUIRE(which == MCBA_TABLE_VALID || which == MCBA_TABLE_INLIERS, MCBA_ERR_ARG, "unknown table selection");
-  CK(cudaSetDevice(ctx->device));
-  int64_t n = ctx->P.N;
-  if (ctx->table_selected != which) {
-    ctx->errors_current = false;
-    const uint8_t* m = which == MCBA_TABLE_VALID ? ctx->valid_mask.p : ctx->inlier_mask.p;
-    ctx->table_selected = -1;      // until the packing succeeds
-    int r = pack_dense(ctx, &ctx->table_desc, m, true, &n); if (r) return r;
-    ctx->table_selected = which;
-    if (which == MCBA_TABLE_INLIERS) ctx->n_inliers = n;
-  }
-  if (n_corners) *n_corners = n;
-  return MCBA_OK;
+  if (ctx->table_selected == which) return ctx->P.N;
+  ctx->errors_current = false;
+  const uint8_t* m = which == MCBA_TABLE_VALID ? ctx->valid_mask.p : ctx->inlier_mask.p;
+  ctx->table_selected = -1;      // until the packing succeeds
+  const int64_t n = pack_dense(ctx, &ctx->table_desc, m, true);
+  ctx->table_selected = which;
+  if (which == MCBA_TABLE_INLIERS) ctx->n_inliers = n;
+  return n;
+}
+
+}  // namespace
+
+int mcba_table_select(mcba_ctx* ctx, int which, int64_t* n_corners) {
+  return api(ctx, [&] {
+    const int64_t n = select_table(ctx, which);
+    if (n_corners) *n_corners = n;
+  });
 }
 
 int mcba_table_errors(mcba_ctx* ctx, mcba_table_stats* stats) {
-  if (!ctx) return MCBA_ERR_ARG;
-  REQUIRE(ctx->table, MCBA_ERR_STATE, "no resident table (mcba_table_upload / mcba_table_from_detections)");
-  { int r = mcba_table_select(ctx, MCBA_TABLE_VALID, nullptr); if (r) return r; }
-  const DeviceProblem P = with_state(ctx, false);
-  cudaStream_t s = ctx->stream;
-  const int64_t N = P.N;
-  double sums[3] = {0.0, 0.0, 0.0};
-  if (N > 0) {
-    CK(ctx->err_valid.alloc((size_t)N)); CK(ctx->err_sorted.alloc((size_t)N));
-    CK(ctx->err_inl.alloc((size_t)N)); CK(ctx->err_inl_sorted.alloc((size_t)N));
-    CK(ctx->table_part.alloc((size_t)3 * P.V + 3));
-    { int r = prepare(ctx, P); if (r) return r; }
-    ViewKernelArgs a{}; a.err = ctx->err_valid.p;
-    { int r = launch_views<MODE_ERROR>(ctx, P, a); if (r) return r; }
-    const int blocks = std::max(1, std::min((P.V + TABLE_WARPS - 1) / TABLE_WARPS, ctx->num_sms * 8));
-    k_table_stats<<<blocks, TABLE_WARPS * 32, 0, s>>>(P, ctx->err_valid.p, ctx->inlier_mask.p, ctx->err_inl.p, ctx->table_part.p); CKL();
-    double* d_sums = ctx->table_part.p + (size_t)3 * P.V;
-    k_sum_partials<<<1, 1024, 0, s>>>(ctx->table_part.p, P.V, 3, 3, d_sums); CKL();
-    CK(cudaMemcpyAsync(sums, d_sums, sizeof(sums), cudaMemcpyDeviceToHost, s));
-    { int r = sort_errors(ctx, ctx->err_valid.p, ctx->err_sorted.p, N); if (r) return r; }
-    { int r = sort_errors(ctx, ctx->err_inl.p, ctx->err_inl_sorted.p, N); if (r) return r; }
-    CK(cudaStreamSynchronize(s));
-  }
-  ctx->n_valid = N; ctx->n_inliers = (int64_t)llround(sums[2]);
-  ctx->errors_current = true;
-  if (stats) { stats->n_valid = N; stats->n_inliers = ctx->n_inliers; stats->sumsq_valid = sums[0]; stats->sumsq_inliers = sums[1]; }
-  return MCBA_OK;
+  return api(ctx, [&] {
+    select_table(ctx, MCBA_TABLE_VALID);
+    const DeviceProblem P = with_state(ctx, false);
+    cudaStream_t s = ctx->stream;
+    const int64_t N = P.N;
+    double sums[3] = {0.0, 0.0, 0.0};
+    if (N > 0) {
+      CK(ctx->err_valid.alloc((size_t)N)); CK(ctx->err_sorted.alloc((size_t)N));
+      CK(ctx->err_inl.alloc((size_t)N)); CK(ctx->err_inl_sorted.alloc((size_t)N));
+      CK(ctx->table_part.alloc((size_t)3 * P.V + 3));
+      prepare(ctx, P);
+      ViewKernelArgs a{}; a.err = ctx->err_valid.p;
+      launch_views<MODE_ERROR>(ctx, P, a);
+      const int blocks = std::max(1, std::min((P.V + TABLE_WARPS - 1) / TABLE_WARPS, ctx->num_sms * 8));
+      k_table_stats<<<blocks, TABLE_WARPS * 32, 0, s>>>(P, ctx->err_valid.p, ctx->inlier_mask.p, ctx->err_inl.p, ctx->table_part.p); CKL();
+      double* d_sums = ctx->table_part.p + (size_t)3 * P.V;
+      k_sum_partials<<<1, 1024, 0, s>>>(ctx->table_part.p, P.V, 3, 3, d_sums); CKL();
+      CK(cudaMemcpyAsync(sums, d_sums, sizeof(sums), cudaMemcpyDeviceToHost, s));
+      sort_errors(ctx, ctx->err_valid.p, ctx->err_sorted.p, N);
+      sort_errors(ctx, ctx->err_inl.p, ctx->err_inl_sorted.p, N);
+      CK(cudaStreamSynchronize(s));
+    }
+    ctx->n_valid = N; ctx->n_inliers = (int64_t)llround(sums[2]);
+    ctx->errors_current = true;
+    if (stats) { stats->n_valid = N; stats->n_inliers = ctx->n_inliers; stats->sumsq_valid = sums[0]; stats->sumsq_inliers = sums[1]; }
+  });
 }
 
 int mcba_table_error_ranks(mcba_ctx* ctx, int which, const int64_t* ranks, int32_t n, double* out) {
-  if (!ctx || (n > 0 && (!ranks || !out))) return MCBA_ERR_ARG;
-  REQUIRE(ctx->table && ctx->errors_current, MCBA_ERR_STATE, "mcba_table_errors has not run since the parameters or the selection changed");
-  REQUIRE(which == MCBA_TABLE_VALID || which == MCBA_TABLE_INLIERS, MCBA_ERR_ARG, "unknown table selection");
-  if (n <= 0) return MCBA_OK;
-  CK(cudaSetDevice(ctx->device));
-  const int64_t count = which == MCBA_TABLE_VALID ? ctx->n_valid : ctx->n_inliers;
-  for (int i = 0; i < n; i++) REQUIRE(ranks[i] >= 0 && ranks[i] < count, MCBA_ERR_ARG, "error rank out of range");
-  CK(ctx->table_ranks.alloc((size_t)n)); CK(ctx->table_out.alloc((size_t)n));
-  CK(cudaMemcpyAsync(ctx->table_ranks.p, ranks, sizeof(int64_t) * n, cudaMemcpyHostToDevice, ctx->stream));
-  k_gather_ranks<<<(n + 127) / 128, 128, 0, ctx->stream>>>(which == MCBA_TABLE_VALID ? ctx->err_sorted.p : ctx->err_inl_sorted.p,
-                                                         ctx->table_ranks.p, n, ctx->table_out.p); CKL();
-  CK(cudaMemcpyAsync(out, ctx->table_out.p, sizeof(double) * n, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  return MCBA_OK;
+  return api(ctx, [&] {
+    REQUIRE(n <= 0 || (ranks && out), MCBA_ERR_ARG, "null ranks or output");
+    REQUIRE(ctx->table && ctx->errors_current, MCBA_ERR_STATE, "mcba_table_errors has not run since the parameters or the selection changed");
+    REQUIRE(which == MCBA_TABLE_VALID || which == MCBA_TABLE_INLIERS, MCBA_ERR_ARG, "unknown table selection");
+    if (n <= 0) return;
+    const int64_t count = which == MCBA_TABLE_VALID ? ctx->n_valid : ctx->n_inliers;
+    for (int i = 0; i < n; i++) REQUIRE(ranks[i] >= 0 && ranks[i] < count, MCBA_ERR_ARG, "error rank out of range");
+    CK(ctx->table_ranks.alloc((size_t)n)); CK(ctx->table_out.alloc((size_t)n));
+    CK(cudaMemcpyAsync(ctx->table_ranks.p, ranks, sizeof(int64_t) * n, cudaMemcpyHostToDevice, ctx->stream));
+    k_gather_ranks<<<(n + 127) / 128, 128, 0, ctx->stream>>>(which == MCBA_TABLE_VALID ? ctx->err_sorted.p : ctx->err_inl_sorted.p,
+                                                           ctx->table_ranks.p, n, ctx->table_out.p); CKL();
+    CK(cudaMemcpyAsync(out, ctx->table_out.p, sizeof(double) * n, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+  });
 }
 
 int mcba_table_count_below(mcba_ctx* ctx, int which, const double* thresholds, int32_t n, int64_t* counts) {
-  if (!ctx || (n > 0 && (!thresholds || !counts))) return MCBA_ERR_ARG;
-  REQUIRE(ctx->table && ctx->errors_current, MCBA_ERR_STATE, "mcba_table_errors has not run since the parameters or the selection changed");
-  REQUIRE(which == MCBA_TABLE_VALID || which == MCBA_TABLE_INLIERS, MCBA_ERR_ARG, "unknown table selection");
-  if (n <= 0) return MCBA_OK;
-  CK(cudaSetDevice(ctx->device));
-  const int64_t count = which == MCBA_TABLE_VALID ? ctx->n_valid : ctx->n_inliers;
-  CK(ctx->table_out.alloc((size_t)n)); CK(ctx->table_ranks.alloc((size_t)n));
-  CK(cudaMemcpyAsync(ctx->table_out.p, thresholds, sizeof(double) * n, cudaMemcpyHostToDevice, ctx->stream));
-  k_count_below<<<(n + 127) / 128, 128, 0, ctx->stream>>>(which == MCBA_TABLE_VALID ? ctx->err_sorted.p : ctx->err_inl_sorted.p, count,
-                                                        ctx->table_out.p, n, ctx->table_ranks.p); CKL();
-  CK(cudaMemcpyAsync(counts, ctx->table_ranks.p, sizeof(int64_t) * n, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  return MCBA_OK;
+  return api(ctx, [&] {
+    REQUIRE(n <= 0 || (thresholds && counts), MCBA_ERR_ARG, "null thresholds or counts");
+    REQUIRE(ctx->table && ctx->errors_current, MCBA_ERR_STATE, "mcba_table_errors has not run since the parameters or the selection changed");
+    REQUIRE(which == MCBA_TABLE_VALID || which == MCBA_TABLE_INLIERS, MCBA_ERR_ARG, "unknown table selection");
+    if (n <= 0) return;
+    const int64_t count = which == MCBA_TABLE_VALID ? ctx->n_valid : ctx->n_inliers;
+    CK(ctx->table_out.alloc((size_t)n)); CK(ctx->table_ranks.alloc((size_t)n));
+    CK(cudaMemcpyAsync(ctx->table_out.p, thresholds, sizeof(double) * n, cudaMemcpyHostToDevice, ctx->stream));
+    k_count_below<<<(n + 127) / 128, 128, 0, ctx->stream>>>(which == MCBA_TABLE_VALID ? ctx->err_sorted.p : ctx->err_inl_sorted.p, count,
+                                                          ctx->table_out.p, n, ctx->table_ranks.p); CKL();
+    CK(cudaMemcpyAsync(counts, ctx->table_ranks.p, sizeof(int64_t) * n, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+  });
 }
 
 int mcba_table_reject(mcba_ctx* ctx, double threshold, int64_t* n_valid, int64_t* n_keep) {
-  if (!ctx) return MCBA_ERR_ARG;
-  REQUIRE(ctx->table && ctx->errors_current && ctx->table_selected == MCBA_TABLE_VALID, MCBA_ERR_STATE,
-          "mcba_table_errors has not run since the parameters or the selection changed");
-  CK(cudaSetDevice(ctx->device));
-  const DeviceProblem& P = ctx->P;
-  cudaStream_t s = ctx->stream;
-  const size_t dense = table_dense(ctx);
-  double kept = 0.0;
-  if (dense) CK(cudaMemsetAsync(ctx->inlier_mask.p, 0, dense, s));
-  if (P.N > 0) {
-    const int blocks = std::max(1, std::min((P.V + TABLE_WARPS - 1) / TABLE_WARPS, ctx->num_sms * 8));
-    k_table_reject<<<blocks, TABLE_WARPS * 32, 0, s>>>(P, ctx->err_valid.p, threshold, ctx->inlier_mask.p, ctx->table_part.p); CKL();
-    double* d_sum = ctx->table_part.p + (size_t)3 * P.V;
-    k_sum_partials<<<1, 1024, 0, s>>>(ctx->table_part.p, P.V, 1, 1, d_sum); CKL();
-    CK(cudaMemcpyAsync(&kept, d_sum, sizeof(double), cudaMemcpyDeviceToHost, s));
-  }
-  CK(cudaStreamSynchronize(s));
-  ctx->n_inliers = (int64_t)llround(kept);
-  ctx->errors_current = false;           // the sorted inlier errors describe the previous mask
-  if (n_valid) *n_valid = P.N;
-  if (n_keep) *n_keep = ctx->n_inliers;
-  return MCBA_OK;
+  return api(ctx, [&] {
+    REQUIRE(ctx->table && ctx->errors_current && ctx->table_selected == MCBA_TABLE_VALID, MCBA_ERR_STATE,
+            "mcba_table_errors has not run since the parameters or the selection changed");
+    const DeviceProblem& P = ctx->P;
+    cudaStream_t s = ctx->stream;
+    const size_t dense = table_dense(ctx);
+    double kept = 0.0;
+    if (dense) CK(cudaMemsetAsync(ctx->inlier_mask.p, 0, dense, s));
+    if (P.N > 0) {
+      const int blocks = std::max(1, std::min((P.V + TABLE_WARPS - 1) / TABLE_WARPS, ctx->num_sms * 8));
+      k_table_reject<<<blocks, TABLE_WARPS * 32, 0, s>>>(P, ctx->err_valid.p, threshold, ctx->inlier_mask.p, ctx->table_part.p); CKL();
+      double* d_sum = ctx->table_part.p + (size_t)3 * P.V;
+      k_sum_partials<<<1, 1024, 0, s>>>(ctx->table_part.p, P.V, 1, 1, d_sum); CKL();
+      CK(cudaMemcpyAsync(&kept, d_sum, sizeof(double), cudaMemcpyDeviceToHost, s));
+    }
+    CK(cudaStreamSynchronize(s));
+    ctx->n_inliers = (int64_t)llround(kept);
+    ctx->errors_current = false;           // the sorted inlier errors describe the previous mask
+    if (n_valid) *n_valid = P.N;
+    if (n_keep) *n_keep = ctx->n_inliers;
+  });
 }
 
 int mcba_set_params(mcba_ctx* ctx, const double* cam_rt, const double* board_rt, const double* frame_rt, const double* intrinsics) {
-  if (!ctx) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
-  REQUIRE(cam_rt && board_rt && intrinsics && (frame_rt || ctx->P.F == 0 || ctx->P.fb == 0), MCBA_ERR_ARG, "null parameter array");
-  const DeviceProblem& P = ctx->P;
-  CK(cudaSetDevice(ctx->device));
-  ctx->errors_current = false;
-  CK(cudaMemcpyAsync(P.cam_rt, cam_rt, sizeof(double) * P.C * 6, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(P.board_rt, board_rt, sizeof(double) * P.B * 6, cudaMemcpyHostToDevice, ctx->stream));
-  if (P.F && P.fb) CK(cudaMemcpyAsync(P.frame_rt, frame_rt, sizeof(double) * P.F * P.fb, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(P.intr, intrinsics, sizeof(double) * P.C * P.kint, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  return MCBA_OK;
+  return api(ctx, [&] {
+    REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
+    REQUIRE(cam_rt && board_rt && intrinsics && (frame_rt || ctx->P.F == 0 || ctx->P.fb == 0), MCBA_ERR_ARG, "null parameter array");
+    const DeviceProblem& P = ctx->P;
+    ctx->errors_current = false;
+    CK(cudaMemcpyAsync(P.cam_rt, cam_rt, sizeof(double) * P.C * 6, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(P.board_rt, board_rt, sizeof(double) * P.B * 6, cudaMemcpyHostToDevice, ctx->stream));
+    if (P.F && P.fb) CK(cudaMemcpyAsync(P.frame_rt, frame_rt, sizeof(double) * P.F * P.fb, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(P.intr, intrinsics, sizeof(double) * P.C * P.kint, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+  });
 }
 
 // Same state as 4x4 pose matrices (PoseSet.poses): the rotation-vector conversions of transform/rtvec.py run on the device.
 // mats: f64[C+B+F][4][4] in the order cameras, boards, frames.
 int mcba_set_state_matrices(mcba_ctx* ctx, const double* mats, const double* intrinsics) {
-  if (!ctx) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
-  REQUIRE(mats && intrinsics, MCBA_ERR_ARG, "null parameter array");
-  const DeviceProblem& P = ctx->P;
-  CK(cudaSetDevice(ctx->device));
-  const int np = P.C + P.B + P.F;
-  ctx->errors_current = false;
-  CK(ctx->pose_mats.alloc((size_t)np * 16));
-  CK(cudaMemcpyAsync(ctx->pose_mats.p, mats, sizeof(double) * 16 * np, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(P.intr, intrinsics, sizeof(double) * P.C * P.kint, cudaMemcpyHostToDevice, ctx->stream));
-  k_matrices_to_state<<<(np + 127) / 128, 128, 0, ctx->stream>>>(P.C, P.B, P.F, ctx->pose_mats.p, P.cam_rt, P.board_rt, P.frame_rt, P.fb); CKL();
-  CK(cudaStreamSynchronize(ctx->stream));     // the host arrays are borrowed only for the call
-  return MCBA_OK;
+  return api(ctx, [&] {
+    REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
+    REQUIRE(mats && intrinsics, MCBA_ERR_ARG, "null parameter array");
+    const DeviceProblem& P = ctx->P;
+    const int np = P.C + P.B + P.F;
+    ctx->errors_current = false;
+    CK(ctx->pose_mats.alloc((size_t)np * 16));
+    CK(cudaMemcpyAsync(ctx->pose_mats.p, mats, sizeof(double) * 16 * np, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(P.intr, intrinsics, sizeof(double) * P.C * P.kint, cudaMemcpyHostToDevice, ctx->stream));
+    k_matrices_to_state<<<(np + 127) / 128, 128, 0, ctx->stream>>>(P.C, P.B, P.F, ctx->pose_mats.p, P.cam_rt, P.board_rt, P.frame_rt, P.fb); CKL();
+    CK(cudaStreamSynchronize(ctx->stream));     // the host arrays are borrowed only for the call
+  });
 }
 
 int mcba_get_state_matrices(mcba_ctx* ctx, double* mats, double* intrinsics) {
-  if (!ctx) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
-  const DeviceProblem& P = ctx->P;
-  CK(cudaSetDevice(ctx->device));
-  const int np = P.C + P.B + P.F;
-  if (mats) {
-    CK(ctx->pose_mats.alloc((size_t)np * 16));
-    const PoseT* derived = nullptr;
-    if (P.motion == MOTION_HAND_EYE) { int r = prepare(ctx, with_state(ctx, false)); if (r) return r; derived = P.frame_T; }
-    k_state_to_matrices<<<(np + 127) / 128, 128, 0, ctx->stream>>>(P.C, P.B, P.F, P.cam_rt, P.board_rt, P.frame_rt, ctx->pose_mats.p, P.fb, derived); CKL();
-    CK(cudaMemcpyAsync(mats, ctx->pose_mats.p, sizeof(double) * 16 * np, cudaMemcpyDeviceToHost, ctx->stream));
-  }
-  if (intrinsics) CK(cudaMemcpyAsync(intrinsics, P.intr, sizeof(double) * P.C * P.kint, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  return MCBA_OK;
+  return api(ctx, [&] {
+    REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
+    const DeviceProblem& P = ctx->P;
+    const int np = P.C + P.B + P.F;
+    if (mats) {
+      CK(ctx->pose_mats.alloc((size_t)np * 16));
+      const PoseT* derived = nullptr;
+      if (P.motion == MOTION_HAND_EYE) { prepare(ctx, with_state(ctx, false)); derived = P.frame_T; }
+      k_state_to_matrices<<<(np + 127) / 128, 128, 0, ctx->stream>>>(P.C, P.B, P.F, P.cam_rt, P.board_rt, P.frame_rt, ctx->pose_mats.p, P.fb, derived); CKL();
+      CK(cudaMemcpyAsync(mats, ctx->pose_mats.p, sizeof(double) * 16 * np, cudaMemcpyDeviceToHost, ctx->stream));
+    }
+    if (intrinsics) CK(cudaMemcpyAsync(intrinsics, P.intr, sizeof(double) * P.C * P.kint, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+  });
 }
 
 // RollingFrames (motion/rolling_frames.py:66-150): the frames of mcba_set_state_matrices are the start poses; the end poses
 // f64[F][4][4] and the image heights f64[C] that turn an observed row into the blend weight (rolling_times, 15-19) come here.
 int mcba_set_rolling(mcba_ctx* ctx, const double* end_pose_matrices, const double* image_heights) {
-  if (!ctx) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
-  const DeviceProblem& P = ctx->P;
-  REQUIRE(P.motion == MOTION_ROLLING, MCBA_ERR_STATE, "the problem was not uploaded with MCBA_MOTION_ROLLING");
-  REQUIRE((end_pose_matrices || P.F == 0) && image_heights, MCBA_ERR_ARG, "null parameter array");
-  for (int c = 0; c < P.C; c++) REQUIRE(image_heights[c] > 0, MCBA_ERR_ARG, "image heights must be positive");
-  CK(cudaSetDevice(ctx->device));
-  ctx->errors_current = false;
-  CK(cudaMemcpyAsync(ctx->img_h.p, image_heights, sizeof(double) * P.C, cudaMemcpyHostToDevice, ctx->stream));
-  if (P.F) {
-    CK(ctx->pose_mats.alloc((size_t)P.F * 16));
-    CK(cudaMemcpyAsync(ctx->pose_mats.p, end_pose_matrices, sizeof(double) * 16 * P.F, cudaMemcpyHostToDevice, ctx->stream));
-    // "cameras = 0, boards = 0, frames = F" view of the same kernel, writing the second half of every frame block
-    k_matrices_to_state<<<(P.F + 127) / 128, 128, 0, ctx->stream>>>(0, 0, P.F, ctx->pose_mats.p, nullptr, nullptr, P.frame_rt + 6, 12); CKL();
-  }
-  CK(cudaStreamSynchronize(ctx->stream));
-  return MCBA_OK;
+  return api(ctx, [&] {
+    REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
+    const DeviceProblem& P = ctx->P;
+    REQUIRE(P.motion == MOTION_ROLLING, MCBA_ERR_STATE, "the problem was not uploaded with MCBA_MOTION_ROLLING");
+    REQUIRE((end_pose_matrices || P.F == 0) && image_heights, MCBA_ERR_ARG, "null parameter array");
+    for (int c = 0; c < P.C; c++) REQUIRE(image_heights[c] > 0, MCBA_ERR_ARG, "image heights must be positive");
+    ctx->errors_current = false;
+    CK(cudaMemcpyAsync(ctx->img_h.p, image_heights, sizeof(double) * P.C, cudaMemcpyHostToDevice, ctx->stream));
+    if (P.F) {
+      CK(ctx->pose_mats.alloc((size_t)P.F * 16));
+      CK(cudaMemcpyAsync(ctx->pose_mats.p, end_pose_matrices, sizeof(double) * 16 * P.F, cudaMemcpyHostToDevice, ctx->stream));
+      // "cameras = 0, boards = 0, frames = F" view of the same kernel, writing the second half of every frame block
+      k_matrices_to_state<<<(P.F + 127) / 128, 128, 0, ctx->stream>>>(0, 0, P.F, ctx->pose_mats.p, nullptr, nullptr, P.frame_rt + 6, 12); CKL();
+    }
+    CK(cudaStreamSynchronize(ctx->stream));
+  });
 }
 
 int mcba_get_rolling(mcba_ctx* ctx, double* end_pose_matrices) {
-  if (!ctx || !end_pose_matrices) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
-  const DeviceProblem& P = ctx->P;
-  REQUIRE(P.motion == MOTION_ROLLING, MCBA_ERR_STATE, "the problem was not uploaded with MCBA_MOTION_ROLLING");
-  CK(cudaSetDevice(ctx->device));
-  if (P.F) {
-    CK(ctx->pose_mats.alloc((size_t)P.F * 16));
-    k_state_to_matrices<<<(P.F + 127) / 128, 128, 0, ctx->stream>>>(0, 0, P.F, nullptr, nullptr, P.frame_rt + 6, ctx->pose_mats.p, 12, nullptr); CKL();
-    CK(cudaMemcpyAsync(end_pose_matrices, ctx->pose_mats.p, sizeof(double) * 16 * P.F, cudaMemcpyDeviceToHost, ctx->stream));
-  }
-  CK(cudaStreamSynchronize(ctx->stream));
-  return MCBA_OK;
+  return api(ctx, [&] {
+    REQUIRE(end_pose_matrices, MCBA_ERR_ARG, "null parameter array");
+    REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
+    const DeviceProblem& P = ctx->P;
+    REQUIRE(P.motion == MOTION_ROLLING, MCBA_ERR_STATE, "the problem was not uploaded with MCBA_MOTION_ROLLING");
+    if (P.F) {
+      CK(ctx->pose_mats.alloc((size_t)P.F * 16));
+      k_state_to_matrices<<<(P.F + 127) / 128, 128, 0, ctx->stream>>>(0, 0, P.F, nullptr, nullptr, P.frame_rt + 6, ctx->pose_mats.p, 12, nullptr); CKL();
+      CK(cudaMemcpyAsync(end_pose_matrices, ctx->pose_mats.p, sizeof(double) * 16 * P.F, cudaMemcpyDeviceToHost, ctx->stream));
+    }
+    CK(cudaStreamSynchronize(ctx->stream));
+  });
 }
 
 // HandEye (motion/hand_eye.py:14-90): frame pose f = gripper_wrt_camera base_wrt_gripper[f] world_wrt_base; the arm poses are
 // constants, the two outer transforms are the 12 motion parameters.  The frames of mcba_set_state_matrices are ignored.
 int mcba_set_hand_eye(mcba_ctx* ctx, const double* base_wrt_gripper, const double* world_wrt_base, const double* gripper_wrt_camera) {
-  if (!ctx) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
-  const DeviceProblem& P = ctx->P;
-  REQUIRE(P.motion == MOTION_HAND_EYE, MCBA_ERR_STATE, "the problem was not uploaded with MCBA_MOTION_HAND_EYE");
-  REQUIRE((base_wrt_gripper || P.F == 0) && world_wrt_base && gripper_wrt_camera, MCBA_ERR_ARG, "null parameter array");
-  CK(cudaSetDevice(ctx->device));
-  ctx->errors_current = false;
-  std::vector<PoseT> arms((size_t)std::max(P.F, 1));
-  for (int f = 0; f < P.F; f++) {
-    const double* M = base_wrt_gripper + (size_t)16 * f;
-    PoseT t{};
-    for (int r = 0; r < 3; r++) { t.R[3 * r] = M[4 * r]; t.R[3 * r + 1] = M[4 * r + 1]; t.R[3 * r + 2] = M[4 * r + 2]; t.t[r] = M[4 * r + 3]; }
-    arms[(size_t)f] = t;
-  }
-  CK(cudaMemcpyAsync(ctx->arm_T.p, arms.data(), sizeof(PoseT) * arms.size(), cudaMemcpyHostToDevice, ctx->stream));
-  CK(ctx->pose_mats.alloc(32));
-  CK(cudaMemcpyAsync(ctx->pose_mats.p, world_wrt_base, sizeof(double) * 16, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(ctx->pose_mats.p + 16, gripper_wrt_camera, sizeof(double) * 16, cudaMemcpyHostToDevice, ctx->stream));
-  k_matrices_to_state<<<1, 128, 0, ctx->stream>>>(0, 0, 2, ctx->pose_mats.p, nullptr, nullptr, P.he_rt, 6); CKL();
-  CK(cudaStreamSynchronize(ctx->stream));
-  return MCBA_OK;
+  return api(ctx, [&] {
+    REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
+    const DeviceProblem& P = ctx->P;
+    REQUIRE(P.motion == MOTION_HAND_EYE, MCBA_ERR_STATE, "the problem was not uploaded with MCBA_MOTION_HAND_EYE");
+    REQUIRE((base_wrt_gripper || P.F == 0) && world_wrt_base && gripper_wrt_camera, MCBA_ERR_ARG, "null parameter array");
+    ctx->errors_current = false;
+    std::vector<PoseT> arms((size_t)std::max(P.F, 1));
+    for (int f = 0; f < P.F; f++) {
+      const double* M = base_wrt_gripper + (size_t)16 * f;
+      PoseT t{};
+      for (int r = 0; r < 3; r++) { t.R[3 * r] = M[4 * r]; t.R[3 * r + 1] = M[4 * r + 1]; t.R[3 * r + 2] = M[4 * r + 2]; t.t[r] = M[4 * r + 3]; }
+      arms[(size_t)f] = t;
+    }
+    CK(cudaMemcpyAsync(ctx->arm_T.p, arms.data(), sizeof(PoseT) * arms.size(), cudaMemcpyHostToDevice, ctx->stream));
+    CK(ctx->pose_mats.alloc(32));
+    CK(cudaMemcpyAsync(ctx->pose_mats.p, world_wrt_base, sizeof(double) * 16, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->pose_mats.p + 16, gripper_wrt_camera, sizeof(double) * 16, cudaMemcpyHostToDevice, ctx->stream));
+    k_matrices_to_state<<<1, 128, 0, ctx->stream>>>(0, 0, 2, ctx->pose_mats.p, nullptr, nullptr, P.he_rt, 6); CKL();
+    CK(cudaStreamSynchronize(ctx->stream));
+  });
 }
 
 int mcba_get_hand_eye(mcba_ctx* ctx, double* world_wrt_base, double* gripper_wrt_camera) {
-  if (!ctx) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
-  const DeviceProblem& P = ctx->P;
-  REQUIRE(P.motion == MOTION_HAND_EYE, MCBA_ERR_STATE, "the problem was not uploaded with MCBA_MOTION_HAND_EYE");
-  CK(cudaSetDevice(ctx->device));
-  CK(ctx->pose_mats.alloc(32));
-  k_state_to_matrices<<<1, 128, 0, ctx->stream>>>(0, 0, 2, nullptr, nullptr, P.he_rt, ctx->pose_mats.p, 6, nullptr); CKL();
-  if (world_wrt_base) CK(cudaMemcpyAsync(world_wrt_base, ctx->pose_mats.p, sizeof(double) * 16, cudaMemcpyDeviceToHost, ctx->stream));
-  if (gripper_wrt_camera) CK(cudaMemcpyAsync(gripper_wrt_camera, ctx->pose_mats.p + 16, sizeof(double) * 16, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  return MCBA_OK;
+  return api(ctx, [&] {
+    REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
+    const DeviceProblem& P = ctx->P;
+    REQUIRE(P.motion == MOTION_HAND_EYE, MCBA_ERR_STATE, "the problem was not uploaded with MCBA_MOTION_HAND_EYE");
+    CK(ctx->pose_mats.alloc(32));
+    k_state_to_matrices<<<1, 128, 0, ctx->stream>>>(0, 0, 2, nullptr, nullptr, P.he_rt, ctx->pose_mats.p, 6, nullptr); CKL();
+    if (world_wrt_base) CK(cudaMemcpyAsync(world_wrt_base, ctx->pose_mats.p, sizeof(double) * 16, cudaMemcpyDeviceToHost, ctx->stream));
+    if (gripper_wrt_camera) CK(cudaMemcpyAsync(gripper_wrt_camera, ctx->pose_mats.p + 16, sizeof(double) * 16, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+  });
 }
 
 // OpenCV's CALIB_FIX_* flags: intrinsic parameters held at their current values.  The mask lives in the problem descriptor that every
 // launch takes by value (and so in the key of the solve's cached graph); setup_problem clears it on every upload.
 int mcba_set_fixed_intrinsics(mcba_ctx* ctx, const uint8_t* fixed) {
-  if (!ctx) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
-  DeviceProblem& P = ctx->P;
-  uint32_t m = 0;
-  for (int i = 0; fixed && i < P.kint; i++) {
-    REQUIRE(fixed[i] <= 1, MCBA_ERR_ARG, "fixed intrinsics: every entry must be 0 or 1");
-    if (fixed[i]) m |= 1u << i;
-  }
-  REQUIRE(!P.fix_aspect || (m & 1u) == ((m >> 1) & 1u), MCBA_ERR_ARG,
-          "fixed intrinsics: under MCBA_OPT_FIX_ASPECT fy follows fx, so fx and fy are fixed together or not at all");
-  P.fixed_intr = m;
-  return MCBA_OK;
+  return api(ctx, [&] {
+    REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
+    DeviceProblem& P = ctx->P;
+    uint32_t m = 0;
+    for (int i = 0; fixed && i < P.kint; i++) {
+      REQUIRE(fixed[i] <= 1, MCBA_ERR_ARG, "fixed intrinsics: every entry must be 0 or 1");
+      if (fixed[i]) m |= 1u << i;
+    }
+    REQUIRE(!P.fix_aspect || (m & 1u) == ((m >> 1) & 1u), MCBA_ERR_ARG,
+            "fixed intrinsics: under MCBA_OPT_FIX_ASPECT fy follows fx, so fx and fy are fixed together or not at all");
+    P.fixed_intr = m;
+  });
 }
 
 // scipy's tr_solver: like the fixed-intrinsics mask a field of the problem descriptor (graph key; cleared by every upload)
 int mcba_set_trust_region(mcba_ctx* ctx, int32_t mode) {
-  if (!ctx) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
-  REQUIRE(mode == MCBA_TR_SUBSPACE || mode == MCBA_TR_EXACT, MCBA_ERR_ARG, "trust region: MCBA_TR_SUBSPACE or MCBA_TR_EXACT");
-  ctx->P.tr_exact = mode == MCBA_TR_EXACT ? 1 : 0;
-  return MCBA_OK;
+  return api(ctx, [&] {
+    REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
+    REQUIRE(mode == MCBA_TR_SUBSPACE || mode == MCBA_TR_EXACT, MCBA_ERR_ARG, "trust region: MCBA_TR_SUBSPACE or MCBA_TR_EXACT");
+    ctx->P.tr_exact = mode == MCBA_TR_EXACT ? 1 : 0;
+  });
 }
 
 int mcba_last_alpha_iterations(mcba_ctx* ctx, int32_t* total) {
-  if (!ctx || !total) return MCBA_ERR_ARG;
-  *total = ctx->last_alpha_iters;
-  return MCBA_OK;
+  return api(ctx, [&] {
+    REQUIRE(total, MCBA_ERR_ARG, "null argument");
+    *total = ctx->last_alpha_iters;
+  });
 }
 
 int mcba_get_params(mcba_ctx* ctx, double* cam_rt, double* board_rt, double* frame_rt, double* intrinsics) {
-  if (!ctx) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
-  const DeviceProblem& P = ctx->P;
-  CK(cudaSetDevice(ctx->device));
-  if (cam_rt) CK(cudaMemcpyAsync(cam_rt, P.cam_rt, sizeof(double) * P.C * 6, cudaMemcpyDeviceToHost, ctx->stream));
-  if (board_rt) CK(cudaMemcpyAsync(board_rt, P.board_rt, sizeof(double) * P.B * 6, cudaMemcpyDeviceToHost, ctx->stream));
-  if (frame_rt && P.F && P.fb) CK(cudaMemcpyAsync(frame_rt, P.frame_rt, sizeof(double) * P.F * P.fb, cudaMemcpyDeviceToHost, ctx->stream));
-  if (intrinsics) CK(cudaMemcpyAsync(intrinsics, P.intr, sizeof(double) * P.C * P.kint, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  return MCBA_OK;
+  return api(ctx, [&] {
+    REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
+    const DeviceProblem& P = ctx->P;
+    if (cam_rt) CK(cudaMemcpyAsync(cam_rt, P.cam_rt, sizeof(double) * P.C * 6, cudaMemcpyDeviceToHost, ctx->stream));
+    if (board_rt) CK(cudaMemcpyAsync(board_rt, P.board_rt, sizeof(double) * P.B * 6, cudaMemcpyDeviceToHost, ctx->stream));
+    if (frame_rt && P.F && P.fb) CK(cudaMemcpyAsync(frame_rt, P.frame_rt, sizeof(double) * P.F * P.fb, cudaMemcpyDeviceToHost, ctx->stream));
+    if (intrinsics) CK(cudaMemcpyAsync(intrinsics, P.intr, sizeof(double) * P.C * P.kint, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+  });
 }
 
 int mcba_num_params(mcba_ctx* ctx, int64_t* n) {
-  if (!ctx || !n) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
-  *n = ctx->P.n;
-  return MCBA_OK;
+  return api(ctx, [&] {
+    REQUIRE(n, MCBA_ERR_ARG, "null argument");
+    REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
+    *n = ctx->P.n;
+  });
 }
 
-static int read_x_canonical(mcba_ctx* ctx, double* x) {
+static void read_x_canonical(mcba_ctx* ctx, double* x) {
   const DeviceProblem& P = ctx->P;
-  if (P.n == 0) return MCBA_OK;
+  if (P.n == 0) return;
   k_gather_params<<<(P.n + 255) / 256, 256, 0, ctx->stream>>>(P, ctx->x.p, P.cam_rt, P.board_rt, P.frame_rt, P.intr); CKL();
   std::vector<double> h((size_t)P.n);
   CK(cudaMemcpyAsync(h.data(), ctx->x.p, sizeof(double) * P.n, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   for (int i = 0; i < P.n; i++) x[ctx->perm[(size_t)i]] = h[(size_t)i];
-  return MCBA_OK;
 }
-static int write_x_canonical(mcba_ctx* ctx, const double* x, double* dev_x) {
+static void write_x_canonical(mcba_ctx* ctx, const double* x, double* dev_x) {
   const DeviceProblem& P = ctx->P;
-  if (P.n == 0) return MCBA_OK;
+  if (P.n == 0) return;
   std::vector<double> h((size_t)P.n);
   for (int i = 0; i < P.n; i++) h[(size_t)i] = x[ctx->perm[(size_t)i]];
   CK(cudaMemcpyAsync(dev_x, h.data(), sizeof(double) * P.n, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  return MCBA_OK;
+}
+// the current state := x (canonical order)
+static void set_param_vec(mcba_ctx* ctx, const double* x) {
+  ctx->errors_current = false;
+  write_x_canonical(ctx, x, ctx->x.p);
+  set_state_from_x(ctx, ctx->x.p, false);
+  CK(cudaStreamSynchronize(ctx->stream));
 }
 
 int mcba_get_param_vec(mcba_ctx* ctx, double* x) {
-  if (!ctx || !x) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
-  CK(cudaSetDevice(ctx->device));
-  return read_x_canonical(ctx, x);
+  return api(ctx, [&] {
+    REQUIRE(x, MCBA_ERR_ARG, "null parameter vector");
+    REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
+    read_x_canonical(ctx, x);
+  });
 }
 
 int mcba_set_param_vec(mcba_ctx* ctx, const double* x) {
-  if (!ctx || !x) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
-  CK(cudaSetDevice(ctx->device));
-  ctx->errors_current = false;
-  int r = write_x_canonical(ctx, x, ctx->x.p); if (r) return r;
-  r = set_state_from_x(ctx, ctx->x.p, false); if (r) return r;
-  CK(cudaStreamSynchronize(ctx->stream));
-  return MCBA_OK;
+  return api(ctx, [&] {
+    REQUIRE(x, MCBA_ERR_ARG, "null parameter vector");
+    REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
+    set_param_vec(ctx, x);
+  });
 }
 
 int mcba_residuals(mcba_ctx* ctx, const double* x, double* r_out, double* cost) {
-  if (!ctx) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
-  CK(cudaSetDevice(ctx->device));
-  bool trial = false;
-  if (x) {
-    // evaluate at x without disturbing the stored parameters: trial state = current state overwritten by x
-    int r = write_x_canonical(ctx, x, ctx->x_new.p); if (r) return r;
-    r = set_state_from_x(ctx, ctx->x_new.p, true); if (r) return r;
-    trial = true;
-  } else {
-    int r = prepare(ctx, with_state(ctx, false)); if (r) return r;
-  }
-  DeviceProblem P = with_state(ctx, trial);
-  if (r_out && P.N > 0) {
-    DevBuf<double> dr; CK(dr.alloc((size_t)2 * P.N));
-    ViewKernelArgs a{}; a.resid = dr.p;
-    int r = launch_views<MODE_RESID>(ctx, P, a); if (r) return r;
-    CK(cudaMemcpyAsync(r_out, dr.p, sizeof(double) * 2 * P.N, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-  }
-  if (cost) {
-    int r = trial_cost(ctx, 0, 1.0, trial); if (r) return r;
-    CK(cudaMemcpyAsync(cost, ctx->eval_cost.p, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-  }
-  return MCBA_OK;
+  return api(ctx, [&] {
+    REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
+    bool trial = false;
+    if (x) {
+      // evaluate at x without disturbing the stored parameters: trial state = current state overwritten by x
+      write_x_canonical(ctx, x, ctx->x_new.p);
+      set_state_from_x(ctx, ctx->x_new.p, true);
+      trial = true;
+    } else {
+      prepare(ctx, with_state(ctx, false));
+    }
+    DeviceProblem P = with_state(ctx, trial);
+    if (r_out && P.N > 0) {
+      DevBuf<double> dr; CK(dr.alloc((size_t)2 * P.N));
+      ViewKernelArgs a{}; a.resid = dr.p;
+      launch_views<MODE_RESID>(ctx, P, a);
+      CK(cudaMemcpyAsync(r_out, dr.p, sizeof(double) * 2 * P.N, cudaMemcpyDeviceToHost, ctx->stream));
+      CK(cudaStreamSynchronize(ctx->stream));
+    }
+    if (cost) {
+      trial_cost(ctx, 0, 1.0, trial);
+      CK(cudaMemcpyAsync(cost, ctx->eval_cost.p, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+      CK(cudaStreamSynchronize(ctx->stream));
+    }
+  });
 }
 
 int mcba_reprojection_error(mcba_ctx* ctx, double* err) {
-  if (!ctx || !err) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
-  CK(cudaSetDevice(ctx->device));
-  DeviceProblem P = with_state(ctx, false);
-  if (P.N == 0) return MCBA_OK;
-  int r = prepare(ctx, P); if (r) return r;
-  DevBuf<double> de; CK(de.alloc((size_t)P.N));
-  ViewKernelArgs a{}; a.err = de.p;
-  r = launch_views<MODE_ERROR>(ctx, P, a); if (r) return r;
-  CK(cudaMemcpyAsync(err, de.p, sizeof(double) * P.N, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  return MCBA_OK;
+  return api(ctx, [&] {
+    REQUIRE(err, MCBA_ERR_ARG, "null argument");
+    REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
+    DeviceProblem P = with_state(ctx, false);
+    if (P.N == 0) return;
+    prepare(ctx, P);
+    DevBuf<double> de; CK(de.alloc((size_t)P.N));
+    ViewKernelArgs a{}; a.err = de.p;
+    launch_views<MODE_ERROR>(ctx, P, a);
+    CK(cudaMemcpyAsync(err, de.p, sizeof(double) * P.N, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+  });
 }
 
 int mcba_linearize(mcba_ctx* ctx, const double* x, double* JtJ, double* Jtr, double* cost) {
-  if (!ctx) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
-  CK(cudaSetDevice(ctx->device));
-  const DeviceProblem& P = ctx->P;
-  if (x) { int r = mcba_set_param_vec(ctx, x); if (r) return r; }
-  else { int r = prepare(ctx, with_state(ctx, false)); if (r) return r; }
-  int r = linearize(ctx, 0, 1.0); if (r) return r;
-  const int n = P.n, n_s = P.n_s, F = P.motion_on ? P.F : 0;
-  const int fb = P.fb;
-  std::vector<double> hHss((size_t)n_s * n_s), hg((size_t)n), hHff((size_t)F * fb * fb), hW((size_t)F * n_s * fb);
-  if (n_s) CK(cudaMemcpyAsync(hHss.data(), ctx->Hss.p, sizeof(double) * hHss.size(), cudaMemcpyDeviceToHost, ctx->stream));
-  if (n) CK(cudaMemcpyAsync(hg.data(), ctx->g.p, sizeof(double) * n, cudaMemcpyDeviceToHost, ctx->stream));
-  if (F) CK(cudaMemcpyAsync(hHff.data(), ctx->Hff.p, sizeof(double) * hHff.size(), cudaMemcpyDeviceToHost, ctx->stream));
-  if (F && n_s) CK(cudaMemcpyAsync(hW.data(), ctx->W.p, sizeof(double) * hW.size(), cudaMemcpyDeviceToHost, ctx->stream));
-  double hcost = 0;
-  CK(cudaMemcpyAsync(&hcost, ctx->lin_cost.p, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  const std::vector<int>& pm = ctx->perm;
-  if (JtJ) {
-    std::fill(JtJ, JtJ + (size_t)n * n, 0.0);
-    for (int i = 0; i < n_s; i++) for (int j = 0; j < n_s; j++) JtJ[(size_t)pm[i] * n + pm[j]] = hHss[(size_t)i * n_s + j];
-    for (int f = 0; f < F; f++) {
-      for (int i = 0; i < fb; i++) for (int j = 0; j < fb; j++) JtJ[(size_t)pm[n_s + fb * f + i] * n + pm[n_s + fb * f + j]] = hHff[((size_t)f * fb + i) * fb + j];
-      for (int s = 0; s < n_s; s++) for (int j = 0; j < fb; j++) {
-        const double w = hW[((size_t)f * n_s + s) * fb + j];
-        JtJ[(size_t)pm[s] * n + pm[n_s + fb * f + j]] = w;
-        JtJ[(size_t)pm[n_s + fb * f + j] * n + pm[s]] = w;
+  return api(ctx, [&] {
+    REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
+    const DeviceProblem& P = ctx->P;
+    if (x) set_param_vec(ctx, x);
+    else prepare(ctx, with_state(ctx, false));
+    linearize(ctx, 0, 1.0);
+    const int n = P.n, n_s = P.n_s, F = P.motion_on ? P.F : 0;
+    const int fb = P.fb;
+    std::vector<double> hHss((size_t)n_s * n_s), hg((size_t)n), hHff((size_t)F * fb * fb), hW((size_t)F * n_s * fb);
+    if (n_s) CK(cudaMemcpyAsync(hHss.data(), ctx->Hss.p, sizeof(double) * hHss.size(), cudaMemcpyDeviceToHost, ctx->stream));
+    if (n) CK(cudaMemcpyAsync(hg.data(), ctx->g.p, sizeof(double) * n, cudaMemcpyDeviceToHost, ctx->stream));
+    if (F) CK(cudaMemcpyAsync(hHff.data(), ctx->Hff.p, sizeof(double) * hHff.size(), cudaMemcpyDeviceToHost, ctx->stream));
+    if (F && n_s) CK(cudaMemcpyAsync(hW.data(), ctx->W.p, sizeof(double) * hW.size(), cudaMemcpyDeviceToHost, ctx->stream));
+    double hcost = 0;
+    CK(cudaMemcpyAsync(&hcost, ctx->lin_cost.p, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    const std::vector<int>& pm = ctx->perm;
+    if (JtJ) {
+      std::fill(JtJ, JtJ + (size_t)n * n, 0.0);
+      for (int i = 0; i < n_s; i++) for (int j = 0; j < n_s; j++) JtJ[(size_t)pm[i] * n + pm[j]] = hHss[(size_t)i * n_s + j];
+      for (int f = 0; f < F; f++) {
+        for (int i = 0; i < fb; i++) for (int j = 0; j < fb; j++) JtJ[(size_t)pm[n_s + fb * f + i] * n + pm[n_s + fb * f + j]] = hHff[((size_t)f * fb + i) * fb + j];
+        for (int s = 0; s < n_s; s++) for (int j = 0; j < fb; j++) {
+          const double w = hW[((size_t)f * n_s + s) * fb + j];
+          JtJ[(size_t)pm[s] * n + pm[n_s + fb * f + j]] = w;
+          JtJ[(size_t)pm[n_s + fb * f + j] * n + pm[s]] = w;
+        }
       }
     }
-  }
-  if (Jtr) for (int i = 0; i < n; i++) Jtr[pm[i]] = hg[(size_t)i];
-  if (cost) *cost = hcost;
-  return MCBA_OK;
+    if (Jtr) for (int i = 0; i < n; i++) Jtr[pm[i]] = hg[(size_t)i];
+    if (cost) *cost = hcost;
+  });
 }
 
 int mcba_solve(mcba_ctx* ctx, const mcba_solve_opts* opts, mcba_solve_result* result, mcba_log_row* log, int32_t log_capacity) {
-  if (!ctx || !opts || !result) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
-  REQUIRE(opts->loss >= 0 && opts->loss <= 4, MCBA_ERR_ARG, "unknown loss");
-  REQUIRE(opts->max_nfev > 0, MCBA_ERR_ARG, "max_nfev must be positive");
-  REQUIRE(opts->f_scale > 0, MCBA_ERR_ARG, "f_scale must be positive");
-  REQUIRE(ctx->world == 1 || !ctx->P.tr_exact, MCBA_ERR_UNSUPPORTED,
-          "tr_solver='exact' on several ranks: the alpha search would exchange the reduced system once per alpha");
-  REQUIRE(ctx->world == 1 || ctx->peer_ready, MCBA_ERR_STATE, "several ranks: the exchanges run over NVLink peer memory (mcba_peer_export / mcba_peer_import first)");
-  CK(cudaSetDevice(ctx->device));
-  const DeviceProblem& P = ctx->P;
-  REQUIRE(ctx->world == 1 || (size_t)P.n_s * P.n_s + 2 * (size_t)P.n_s + 16 <= (size_t)ctx->peer_cap, MCBA_ERR_STATE,
-          "the reduced normal equations do not fit the NVLink exchange slots: export larger peer buffers (mcba_peer_export cap >= n_s^2 + 2 n_s + 16)");
-  cudaStream_t s = ctx->stream;
-  const int n = P.n;
-  memset(result, 0, sizeof(*result));
-  ctx->launches = 0;
-  ctx->last_alpha_iters = 0;
-  ctx->errors_current = false;
-  struct EventPair {       // destroyed on every return path
-    cudaEvent_t a = nullptr, b = nullptr;
-    ~EventPair() { if (a) cudaEventDestroy(a); if (b) cudaEventDestroy(b); }
-  } ev;
-  CK(cudaEventCreate(&ev.a)); CK(cudaEventCreate(&ev.b));
-  CK(cudaEventRecord(ev.a, s));
+  return api(ctx, [&] {
+    REQUIRE(opts && result, MCBA_ERR_ARG, "null options or result");
+    REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
+    REQUIRE(opts->loss >= 0 && opts->loss <= 4, MCBA_ERR_ARG, "unknown loss");
+    REQUIRE(opts->max_nfev > 0, MCBA_ERR_ARG, "max_nfev must be positive");
+    REQUIRE(opts->f_scale > 0, MCBA_ERR_ARG, "f_scale must be positive");
+    REQUIRE(ctx->world == 1 || !ctx->P.tr_exact, MCBA_ERR_UNSUPPORTED,
+            "tr_solver='exact' on several ranks: the alpha search would exchange the reduced system once per alpha");
+    REQUIRE(ctx->world == 1 || ctx->peer_ready, MCBA_ERR_STATE, "several ranks: the exchanges run over NVLink peer memory (mcba_peer_export / mcba_peer_import first)");
+    const DeviceProblem& P = ctx->P;
+    REQUIRE(ctx->world == 1 || (size_t)P.n_s * P.n_s + 2 * (size_t)P.n_s + 16 <= (size_t)ctx->peer_cap, MCBA_ERR_STATE,
+            "the reduced normal equations do not fit the NVLink exchange slots: export larger peer buffers (mcba_peer_export cap >= n_s^2 + 2 n_s + 16)");
+    cudaStream_t s = ctx->stream;
+    const int n = P.n;
+    memset(result, 0, sizeof(*result));
+    ctx->launches = 0;
+    ctx->last_alpha_iters = 0;
+    ctx->errors_current = false;
+    struct EventPair {       // destroyed on every return path
+      cudaEvent_t a = nullptr, b = nullptr;
+      ~EventPair() { if (a) cudaEventDestroy(a); if (b) cudaEventDestroy(b); }
+    } ev;
+    CK(cudaEventCreate(&ev.a)); CK(cudaEventCreate(&ev.b));
+    CK(cudaEventRecord(ev.a, s));
 
-  SolverState h{};
-  h.ftol = opts->ftol; h.xtol = opts->xtol; h.gtol = opts->gtol; h.reg_floor = 1e-12; h.max_nfev = opts->max_nfev;
-  h.nfev = 1; h.njev = 1; h.iteration = 0; h.status = -99; h.first_scale = 1;
-  int r;
-  if (n == 0) {      // nothing to optimise: report the cost and leave
-    r = prepare(ctx, with_state(ctx, false)); if (r) return r;
-    r = linearize(ctx, opts->loss, opts->f_scale); if (r) return r;
-    if (ctx->world > 1) {       // one number: the host's collective is the simplest exchange (no solver state involved)
-      ctx->err = "nothing to optimise on several ranks: sum mcba_residuals' cost on the host"; return MCBA_ERR_UNSUPPORTED;
+    SolverState h{};
+    h.ftol = opts->ftol; h.xtol = opts->xtol; h.gtol = opts->gtol; h.reg_floor = 1e-12; h.max_nfev = opts->max_nfev;
+    h.nfev = 1; h.njev = 1; h.iteration = 0; h.status = -99; h.first_scale = 1;
+    if (n == 0) {      // nothing to optimise: report the cost and leave
+      prepare(ctx, with_state(ctx, false));
+      linearize(ctx, opts->loss, opts->f_scale);
+      // one number: the host's collective is the simplest exchange (no solver state involved)
+      REQUIRE(ctx->world == 1, MCBA_ERR_UNSUPPORTED, "nothing to optimise on several ranks: sum mcba_residuals' cost on the host");
+      CK(cudaMemcpyAsync(&h.cost, ctx->lin_cost.p, sizeof(double), cudaMemcpyDeviceToHost, s));
+      CK(cudaStreamSynchronize(s));
+      result->initial_cost = h.cost; result->cost = h.cost; result->nfev = 1; result->njev = 1; result->status = 1;
+      if (log && log_capacity > 0) { log[0] = mcba_log_row{0, 1, h.cost, NAN, NAN, 0.0}; result->n_log = 1; }
+      CK(cudaEventRecord(ev.b, s)); CK(cudaEventSynchronize(ev.b));
+      float ms0 = 0; cudaEventElapsedTime(&ms0, ev.a, ev.b);
+      result->device_ms = ms0; result->kernel_launches = ctx->launches;
+      return;
     }
-    CK(cudaMemcpyAsync(&h.cost, ctx->lin_cost.p, sizeof(double), cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(ctx->state.p, &h, sizeof(h), cudaMemcpyHostToDevice, s));
+    // x0 and the trial state := the current state; its pose tables
+    k_gather_params<<<(n + 255) / 256, 256, 0, s>>>(P, ctx->x.p, P.cam_rt, P.board_rt, P.frame_rt, P.intr); CKL();
+    CK(cudaMemcpyAsync(ctx->x_new.p, ctx->x.p, sizeof(double) * n, cudaMemcpyDeviceToDevice, s));
+    copy_state_to_trial(ctx);
+    prepare(ctx, with_state(ctx, true));
+    const int cap = std::max(8, opts->max_nfev + 4);
+    CK(ctx->dev_log.alloc((size_t)cap));
+
+    run_lm_loop(ctx, opts->loss, opts->f_scale, cap);
+
+    CK(cudaMemcpyAsync(&h, ctx->state.p, sizeof(h), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
-    result->initial_cost = h.cost; result->cost = h.cost; result->nfev = 1; result->njev = 1; result->status = 1;
-    if (log && log_capacity > 0) { log[0] = mcba_log_row{0, 1, h.cost, NAN, NAN, 0.0}; result->n_log = 1; }
-    CK(cudaEventRecord(ev.b, s)); CK(cudaEventSynchronize(ev.b));
-    float ms0 = 0; cudaEventElapsedTime(&ms0, ev.a, ev.b);
-    result->device_ms = ms0; result->kernel_launches = ctx->launches;
-    return MCBA_OK;
-  }
-  CK(cudaMemcpyAsync(ctx->state.p, &h, sizeof(h), cudaMemcpyHostToDevice, s));
-  // x0 and the trial state := the current state; its pose tables
-  k_gather_params<<<(n + 255) / 256, 256, 0, s>>>(P, ctx->x.p, P.cam_rt, P.board_rt, P.frame_rt, P.intr); CKL();
-  CK(cudaMemcpyAsync(ctx->x_new.p, ctx->x.p, sizeof(double) * n, cudaMemcpyDeviceToDevice, s));
-  r = copy_state_to_trial(ctx); if (r) return r;
-  r = prepare(ctx, with_state(ctx, true)); if (r) return r;
-  const int cap = std::max(8, opts->max_nfev + 4);
-  CK(ctx->dev_log.alloc((size_t)cap));
-
-  r = run_lm_loop(ctx, opts->loss, opts->f_scale, cap); if (r) return r;
-
-  CK(cudaMemcpyAsync(&h, ctx->state.p, sizeof(h), cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  if (h.status == -2) { ctx->err = "Residuals are not finite in the initial point."; return MCBA_ERR_NONFINITE; }
-  if (h.status == -3) { ctx->err = "a peer rank did not answer an in-kernel exchange (timeout): the ranks left mcba_solve out of step"; return MCBA_ERR_NCCL; }
-  const int nlog = std::min(h.nlog, cap);
-  std::vector<mcba_log_row> rows((size_t)std::max(nlog, 1));
-  if (nlog > 0) CK(cudaMemcpyAsync(rows.data(), ctx->dev_log.p, sizeof(mcba_log_row) * nlog, cudaMemcpyDeviceToHost, s));
-  // leave the context consistent: pose tables of the final (current) state
-  r = prepare(ctx, with_state(ctx, false)); if (r) return r;
-  CK(cudaEventRecord(ev.b, s));
-  CK(cudaEventSynchronize(ev.b));
-  float ms = 0; cudaEventElapsedTime(&ms, ev.a, ev.b);
-  if (nlog > 0) result->initial_cost = rows[0].cost;
-  if (log) for (int i = 0; i < nlog && i < log_capacity; i++) log[i] = rows[(size_t)i];
-  result->cost = h.cost; result->optimality = h.g_norm; result->nfev = h.nfev; result->njev = h.njev;
-  result->status = h.status == -99 ? 0 : h.status; result->n_log = std::min(nlog, (int)log_capacity); result->device_ms = ms;
-  if (ctx->graph_launched) ctx->launches += ctx->sg.body_launches * (h.nfev + h.relins);      // the WHILE node ran the body once per evaluation and relinearisation
-  ctx->last_alpha_iters = h.alpha_iters;
-  result->kernel_launches = ctx->launches; result->chol_retries = h.chol_fail;
-  return MCBA_OK;
+    REQUIRE(h.status != -2, MCBA_ERR_NONFINITE, "Residuals are not finite in the initial point.");
+    REQUIRE(h.status != -3, MCBA_ERR_NCCL, "a peer rank did not answer an in-kernel exchange (timeout): the ranks left mcba_solve out of step");
+    const int nlog = std::min(h.nlog, cap);
+    std::vector<mcba_log_row> rows((size_t)std::max(nlog, 1));
+    if (nlog > 0) CK(cudaMemcpyAsync(rows.data(), ctx->dev_log.p, sizeof(mcba_log_row) * nlog, cudaMemcpyDeviceToHost, s));
+    // leave the context consistent: pose tables of the final (current) state
+    prepare(ctx, with_state(ctx, false));
+    CK(cudaEventRecord(ev.b, s));
+    CK(cudaEventSynchronize(ev.b));
+    float ms = 0; cudaEventElapsedTime(&ms, ev.a, ev.b);
+    if (nlog > 0) result->initial_cost = rows[0].cost;
+    if (log) for (int i = 0; i < nlog && i < log_capacity; i++) log[i] = rows[(size_t)i];
+    result->cost = h.cost; result->optimality = h.g_norm; result->nfev = h.nfev; result->njev = h.njev;
+    result->status = h.status == -99 ? 0 : h.status; result->n_log = std::min(nlog, (int)log_capacity); result->device_ms = ms;
+    if (ctx->graph_launched) ctx->launches += ctx->sg.body_launches * (h.nfev + h.relins);      // the WHILE node ran the body once per evaluation and relinearisation
+    ctx->last_alpha_iters = h.alpha_iters;
+    result->kernel_launches = ctx->launches; result->chol_retries = h.chol_fail;
+  });
 }
 
 int mcba_bench_info(mcba_ctx* ctx, int which, int64_t* corners, int64_t* bytes, int32_t* launches) {
-  if (!ctx) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
-  const DeviceProblem& P = ctx->P;
-  int64_t per_corner = 18, per_view = 16, l = 1;
-  if (which == MCBA_BENCH_RESIDUAL) per_corner = 18 + 4 + 16;
-  if (corners) *corners = P.N;
-  if (bytes) *bytes = per_corner * P.N + per_view * P.V;      // per launch
-  if (launches) *launches = (int32_t)l;
-  return MCBA_OK;
+  return api(ctx, [&] {
+    REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
+    const DeviceProblem& P = ctx->P;
+    int64_t per_corner = 18, per_view = 16, l = 1;
+    if (which == MCBA_BENCH_RESIDUAL) per_corner = 18 + 4 + 16;
+    if (corners) *corners = P.N;
+    if (bytes) *bytes = per_corner * P.N + per_view * P.V;      // per launch
+    if (launches) *launches = (int32_t)l;
+  });
 }
 
 int mcba_bench_launch(mcba_ctx* ctx, int which, int repeats) {
-  if (!ctx) return MCBA_ERR_ARG;
-  REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
-  CK(cudaSetDevice(ctx->device));
-  DeviceProblem P = with_state(ctx, false);
-  int r;
-  if (!(which & MCBA_BENCH_NO_PREPARE)) { r = prepare(ctx, P); if (r) return r; }
-  which &= ~MCBA_BENCH_NO_PREPARE;
-  for (int i = 0; i < repeats; i++) {
-    ViewKernelArgs a{}; a.loss = 0; a.f_scale = 1.0;
-    if (which == MCBA_BENCH_LINEARIZE) r = launch_linearize(ctx, P, 0, 1.0);
-    else if (which == MCBA_BENCH_COST) { a.view_cost = ctx->view_cost.p; r = launch_views<MODE_COST>(ctx, P, a); }
-    else { ctx->err = "unsupported bench kernel"; return MCBA_ERR_ARG; }
-    if (r) return r;
-  }
-  return MCBA_OK;
+  return api(ctx, [&] {
+    REQUIRE(ctx->uploaded, MCBA_ERR_STATE, "no problem uploaded");
+    DeviceProblem P = with_state(ctx, false);
+    if (!(which & MCBA_BENCH_NO_PREPARE)) prepare(ctx, P);
+    which &= ~MCBA_BENCH_NO_PREPARE;
+    for (int i = 0; i < repeats; i++) {
+      ViewKernelArgs a{}; a.loss = 0; a.f_scale = 1.0;
+      if (which == MCBA_BENCH_LINEARIZE) launch_linearize(ctx, P, 0, 1.0);
+      else if (which == MCBA_BENCH_COST) { a.view_cost = ctx->view_cost.p; launch_views<MODE_COST>(ctx, P, a); }
+      else throw Failure{MCBA_ERR_ARG, "unsupported bench kernel"};
+    }
+  });
 }
 
 }  // extern "C"
