@@ -316,29 +316,15 @@ int  mcba_hand_eye_vote(mcba_ctx* ctx, int32_t n_sets, const int64_t* set_start,
 
 /* -- applying a finished calibration (Camera.undistort_map / undistort_points / project, camera.py:113-128; undistort_images,
  * camera.py:244-258; the CameraFisheye twins, camera_fisheye.py:102-117) -----------------------------------------------------------
- * camera f64[5+nd] = [fx fy cx cy skew dist...] of `model` (Camera.params order); K = [[fx skew cx] [0 fy cy] [0 0 1]].
- * mcba_undistort_map: cv2.initUndistortRectifyMap(K, dist, None, K, (width, height), CV_32FC2) (cv2.fisheye.initUndistortRectifyMap for
- *   MCBA_MODEL_FISHEYE): the normalised point of pixel (u, v) is K^-1 (u, v, 1) with the skew, the forward projection uses fx, fy, cx,
- *   cy only, as OpenCV's does.  fp64, stored as float32.  The camera's map stays resident on the context in its fixed-point form (the
- *   most recently used 64 maps are kept); map f32[height][width][2] receives the float map when not NULL.
- * mcba_undistort_images: cv2.remap(src[i], map, None, INTER_CUBIC) with the constant-zero border for n images of one camera, host memory
- *   to host memory: src[i] uint8[src_height][src_width][channels], dst[i] uint8[height][width][channels] (the map's size).  Uses the
- *   camera's resident map (computed first if it is not resident).  Chunks of images are staged through pinned buffers on several
- *   streams so that the copies in, the remap and the copies out overlap.  dtype must be MCBA_IMAGE_UINT8 and channels 1 or 3, else
- *   MCBA_ERR_ARG.
+ * camera f64[5+nd] = [fx fy cx cy skew dist...] of `model` (Camera.params order); K = [[fx skew cx] [0 fy cy] [0 0 1]].  Undistortion is
+ * the rectification below with R = I and P = K.
  * mcba_project_points: cv2.projectPoints(points, rvec = 0, tvec = 0, K, dist) (cv2.fisheye.projectPoints): camera-frame points
  *   f64[n][3] -> pixels f64[n][2].
- * mcba_undistort_points: cv2.undistortPoints(pixels, K, dist, P = K) (cv2.fisheye.undistortPoints): f64[n][2] -> f64[n][2].
  * mcba_remap_cubic_table: the fixed-point bicubic weights the remap uses, int32[1024][16]: entry (Y & 31) * 32 + (X & 31) for the map
  *   position (X, Y) = rint(32 (x, y)), 4x4 taps row-major from ((X >> 5) - 1, (Y >> 5) - 1).
  * Non-finite camera parameters fail with MCBA_ERR_NONFINITE.  None of these touches the uploaded problem. */
 enum { MCBA_IMAGE_UINT8 = 0 };
-int  mcba_undistort_map(mcba_ctx* ctx, int32_t model, const double* camera, int32_t width, int32_t height, float* map);
-int  mcba_undistort_images(mcba_ctx* ctx, int32_t model, const double* camera, int32_t width, int32_t height, int32_t n,
-                           int32_t src_width, int32_t src_height, int32_t channels, int32_t dtype, const uint8_t* const* src,
-                           uint8_t* const* dst);
 int  mcba_project_points(mcba_ctx* ctx, int32_t model, const double* camera, int64_t n, const double* points, double* pixels);
-int  mcba_undistort_points(mcba_ctx* ctx, int32_t model, const double* camera, int64_t n, const double* pixels, double* undistorted);
 int  mcba_remap_cubic_table(mcba_ctx* ctx, int32_t* table);
 
 /* -- rectifying a calibrated pair (cv2.initUndistortRectifyMap / cv2.undistortPoints with R and P, after cv2.stereoRectify) ---------------
@@ -346,10 +332,15 @@ int  mcba_remap_cubic_table(mcba_ctx* ctx, int32_t* table);
  * mcba_rectify_map: cv2.initUndistortRectifyMap(K, dist, R, P, (width, height), CV_32FC2) (cv2.fisheye.initUndistortRectifyMap for
  *   MCBA_MODEL_FISHEYE; its two CV_32F maps interleaved).  The normalised point of pixel (u, v) of row v is OpenCV's walk along the row
  *   from (P R)^-1 (0, v, 1) in steps of (P R)^-1 (1, 0, 0): blocks of 8 pixels for the pinhole models, one pixel at a time for the
- *   fisheye, as OpenCV's own loops round it.  (width, height) is the rectified image's size, which need not be the camera's.  The map
- *   stays resident like an undistortion map, keyed by the camera, R, P and the size; map receives the float map when not NULL.  Fisheye
- *   maps may be at most 8533 pixels wide, pinhole maps about 68000.
- * mcba_rectify_images: mcba_undistort_images through the rectification map of (R, P, width, height).
+ *   fisheye, as OpenCV's own loops round it; the forward projection uses fx, fy, cx, cy only, as OpenCV's does.  fp64, stored as
+ *   float32.  (width, height) is the rectified image's size, which need not be the camera's.  The map stays resident on the context in
+ *   its fixed-point form, keyed by the camera, R, P and the size (the most recently used 64 maps are kept); map f32[height][width][2]
+ *   receives the float map when not NULL.
+ * mcba_rectify_images: cv2.remap(src[i], map, None, INTER_CUBIC) with the constant-zero border for n images of one camera through its
+ *   rectification map of (R, P, width, height), host memory to host memory: src[i] uint8[src_height][src_width][channels], dst[i]
+ *   uint8[height][width][channels] (the map's size).  Uses the resident map (computed first if it is not resident).  Chunks of images
+ *   are staged through pinned buffers on several streams so that the copies in, the remap and the copies out overlap.  dtype must be
+ *   MCBA_IMAGE_UINT8 and channels 1 or 3, else MCBA_ERR_ARG.
  * mcba_rectify_points: cv2.undistortPoints(pixels, K, dist, R = R, P = P) (cv2.fisheye.undistortPoints(pixels, K, dist, R, P)):
  *   f64[n][2] -> f64[n][2].  P = I gives normalised coordinates in the rectified frame.
  * (P R)^-1 comes from 3x3 Gaussian elimination with partial pivoting on the host: a singular P R fails with MCBA_ERR_ARG.  Non-finite

@@ -31,9 +31,8 @@ EXPORTS = ["mcba_create", "mcba_destroy", "mcba_last_error", "mcba_set_stream", 
            "mcba_table_upload", "mcba_table_from_detections", "mcba_table_download", "mcba_table_set_inliers",
            "mcba_table_get_inliers", "mcba_table_select", "mcba_pnp_views", "mcba_table_errors", "mcba_table_error_ranks", "mcba_table_count_below", "mcba_table_reject",
            "mcba_intrinsic_init", "mcba_view_errors", "mcba_pose_pairs", "mcba_pose_times", "mcba_pose_cluster",
-           "mcba_hand_eye_quads", "mcba_hand_eye_vote", "mcba_undistort_map", "mcba_undistort_images", "mcba_project_points",
-           "mcba_undistort_points", "mcba_remap_cubic_table", "mcba_stereo_init", "mcba_rectify_map", "mcba_rectify_images",
-           "mcba_rectify_points", "mcba_triangulate", "mcba_triangulate_linear"]
+           "mcba_hand_eye_quads", "mcba_hand_eye_vote", "mcba_project_points", "mcba_remap_cubic_table", "mcba_stereo_init",
+           "mcba_rectify_map", "mcba_rectify_images", "mcba_rectify_points", "mcba_triangulate", "mcba_triangulate_linear"]
 IMAGE_UINT8 = 0          # include/mcba.h MCBA_IMAGE_UINT8
 POINTS_F64, POINTS_F32 = 0, 1          # include/mcba.h MCBA_POINTS_*
 TABLE_VALID, TABLE_INLIERS = 0, 1
@@ -138,10 +137,7 @@ def load():
   lib.mcba_hand_eye_quads.argtypes = [P, i32, i32, i32, D, U8, i32, I32, D, D, I32, U8]
   lib.mcba_hand_eye_vote.argtypes = [P, i32, I64, D, D, I32]
   U8P = C.POINTER(U8)
-  lib.mcba_undistort_map.argtypes = [P, i32, D, i32, i32, C.POINTER(C.c_float)]
-  lib.mcba_undistort_images.argtypes = [P, i32, D, i32, i32, i32, i32, i32, i32, i32, U8P, U8P]
   lib.mcba_project_points.argtypes = [P, i32, D, C.c_int64, D, D]
-  lib.mcba_undistort_points.argtypes = [P, i32, D, C.c_int64, D, D]
   lib.mcba_remap_cubic_table.argtypes = [P, I32]
   lib.mcba_rectify_map.argtypes = [P, i32, D, D, D, i32, i32, C.POINTER(C.c_float)]
   lib.mcba_rectify_images.argtypes = [P, i32, D, D, D, i32, i32, i32, i32, i32, i32, i32, U8P, U8P]

@@ -195,7 +195,7 @@ struct mcba_ctx {
   struct HandEyeInitBuffers {
     DevBuf<double> poses, X, Z, points, density; DevBuf<uint8_t> valid, ok; DevBuf<int32_t> quads, n_images, best; DevBuf<int64_t> start;
   } heinit;
-  // applying a calibration (mcba_undistort_* / mcba_project_points): the cubic weight table, the resident maps of recent cameras
+  // applying a calibration (mcba_rectify_* / mcba_project_points): the cubic weight table, the resident maps of recent cameras
   // (fixed-point form, least recently used dropped first), the optional float map, points, and per-stream pinned staging for images
   struct UndistortMap {
     int model = -1, w = 0, h = 0; std::vector<double> cam; DevBuf<uint32_t> org; DevBuf<uint16_t> idx; uint64_t used = 0;
@@ -712,7 +712,7 @@ int64_t pack_dense(mcba_ctx* ctx, const mcba_problem_desc* desc, const uint8_t* 
 // =====================================================================================================
 extern "C" {
 
-int mcba_version(void) { return 100; }
+int mcba_version(void) { return 101; }
 
 const char* mcba_last_error(const mcba_ctx* ctx) { return ctx ? ctx->err.c_str() : g_create_error.c_str(); }
 
@@ -751,7 +751,6 @@ int mcba_create(int device, mcba_ctx** out) {
     cudaFuncSetAttribute(k_pose_align<PI_SMALL_THREADS, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, PI_SMALL_MAX * PI_ROW_BYTES);
     for (int model = MODEL_STANDARD; model <= MODEL_TILTED; model++)
       with_model(model, false, [](auto M, auto) {
-        cudaFuncSetAttribute(k_rectify_map<decltype(M)::value>, cudaFuncAttributeMaxDynamicSharedMemorySize, RECT_SMEM_MAX);
         cudaFuncSetAttribute(k_triangulate<decltype(M)::value, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                              (int)tri_smem((MCBA_TRI_MAX_CAMERAS + 31) / 32));
       });
@@ -1444,7 +1443,7 @@ int mcba_hand_eye_vote(mcba_ctx* ctx, int32_t n_sets, const int64_t* set_start, 
 
 namespace {
 
-// the camera of the undistortion entries: [fx fy cx cy skew dist...] with 5 + nd values of `model`
+// the camera of the map and point entries: [fx fy cx cy skew dist...] with 5 + nd values of `model`
 void check_camera(int32_t model, const double* camera) {
   REQUIRE(model >= MODEL_STANDARD && model <= MODEL_TILTED, MCBA_ERR_ARG, "unknown camera model");
   REQUIRE(camera, MCBA_ERR_ARG, "null camera");
@@ -1471,8 +1470,7 @@ void ensure_cubic_table(mcba_ctx* ctx) {
 }
 
 // the resident fixed-point map of a key, computed on ctx->stream by launch(float map or null, org, idx) when it is not resident yet (or
-// when the float map is asked for).  The key is the camera vector for an undistortion map, the camera vector followed by R and P for a
-// rectification map: its length tells the two apart.
+// when the float map is asked for)
 mcba_ctx::UndistortMap* resident_map(mcba_ctx* ctx, int model, const double* key, size_t nk, int w, int h, float* map_out,
                                      const std::function<void(float2*, uint32_t*, uint16_t*)>& launch) {
   auto& U = ctx->und;
@@ -1509,16 +1507,6 @@ mcba_ctx::UndistortMap* resident_map(mcba_ctx* ctx, int model, const double* key
   return m;
 }
 
-// the resident undistortion map of a camera (k_undistort_map)
-mcba_ctx::UndistortMap* undistortion_map(mcba_ctx* ctx, int model, const double* camera, int w, int h, float* map_out) {
-  const UndistortCamera c = make_camera(model, camera, w, h);
-  const dim3 grid((w + UND_THREADS - 1) / UND_THREADS, h);
-  cudaStream_t s = ctx->stream;
-  return resident_map(ctx, model, camera, 5 + (size_t)model_nd(model), w, h, map_out, [&](float2* f, uint32_t* org, uint16_t* idx) {
-    with_model(model, false, [&](auto M, auto) { k_undistort_map<decltype(M)::value><<<grid, UND_THREADS, 0, s>>>(c, f, org, idx); });
-  });
-}
-
 // rr = P R and ir = rr^-1 (row-major 3x3) for the rectification entries; a singular or non-finite P R fails with MCBA_ERR_ARG
 RectifyCamera make_rectify_camera(int model, const double* camera, const double* R, const double* P, int w, int h) {
   REQUIRE(R && P, MCBA_ERR_ARG, "null R or P");
@@ -1548,21 +1536,16 @@ RectifyCamera make_rectify_camera(int model, const double* camera, const double*
   return rc;
 }
 
-// shared memory of a k_rectify_map CTA
-size_t rectify_smem(int model, int w) { return 3 * sizeof(double) * (size_t)rectify_walk_len(model, w); }
-
 // the resident rectification map of a camera under (R, P) (k_rectify_map)
 mcba_ctx::UndistortMap* rectification_map(mcba_ctx* ctx, int model, const double* camera, const double* R, const double* P, int w, int h,
                                           float* map_out) {
   const RectifyCamera rc = make_rectify_camera(model, camera, R, P, w, h);
-  const size_t smem = rectify_smem(model, w);
-  REQUIRE(smem <= (size_t)RECT_SMEM_MAX, MCBA_ERR_ARG, "map too wide for one row's walk in shared memory");
   const size_t nk = 5 + (size_t)model_nd(model);
   std::vector<double> key(camera, camera + nk);
   key.insert(key.end(), R, R + 9); key.insert(key.end(), P, P + 9);
   cudaStream_t s = ctx->stream;
   return resident_map(ctx, model, key.data(), key.size(), w, h, map_out, [&](float2* f, uint32_t* org, uint16_t* idx) {
-    with_model(model, false, [&](auto M, auto) { k_rectify_map<decltype(M)::value><<<h, UND_THREADS, smem, s>>>(rc, f, org, idx); });
+    with_model(model, false, [&](auto M, auto) { k_rectify_map<decltype(M)::value><<<h, UND_THREADS, 0, s>>>(rc, f, org, idx); });
   });
 }
 
@@ -1638,13 +1621,13 @@ void check_images(int32_t width, int32_t height, int32_t n, int32_t src_width, i
   for (int i = 0; i < n; i++) REQUIRE(src[i] && dst[i], MCBA_ERR_ARG, "null image " + std::to_string(i));
 }
 
-// point entries: copy in, one thread per point, copy out.  R and P (both or neither) make it the rectification of the points.
+// point entries: copy in, one thread per point, copy out.  The projection of camera-frame points, or the rectification of pixels under
+// R and P.
 void run_points(mcba_ctx* ctx, bool project, int32_t model, const double* camera, int64_t n, const double* in, double* out,
                 const double* R = nullptr, const double* P = nullptr) {
   check_camera(model, camera);
-  const bool rectify = R || P;
   RectifyCamera rc;
-  if (rectify) rc = make_rectify_camera(model, camera, R, P, 0, 0);
+  if (!project) rc = make_rectify_camera(model, camera, R, P, 0, 0);
   REQUIRE(n >= 0, MCBA_ERR_ARG, "negative point count");
   if (n == 0) return;
   REQUIRE(in && out, MCBA_ERR_ARG, "null argument");
@@ -1658,8 +1641,7 @@ void run_points(mcba_ctx* ctx, bool project, int32_t model, const double* camera
   with_model(model, false, [&](auto M, auto) {
     constexpr int MODEL = decltype(M)::value;
     if (project) k_project_points<MODEL><<<blocks, UND_THREADS, 0, s>>>(c, n, U.pin.p, U.pout.p);
-    else if (rectify) k_rectify_points<MODEL><<<blocks, UND_THREADS, 0, s>>>(rc, n, U.pin.p, U.pout.p);
-    else k_undistort_points<MODEL><<<blocks, UND_THREADS, 0, s>>>(c, n, U.pin.p, U.pout.p);
+    else k_rectify_points<MODEL><<<blocks, UND_THREADS, 0, s>>>(rc, n, U.pin.p, U.pout.p);
   });
   CKL();
   CK(cudaMemcpyAsync(out, U.pout.p, sizeof(double) * 2 * n, cudaMemcpyDeviceToHost, s));
@@ -1667,29 +1649,6 @@ void run_points(mcba_ctx* ctx, bool project, int32_t model, const double* camera
 }
 
 }  // namespace
-
-// initUndistortRectifyMap(K, dist, None, K, (width, height)) of one camera, kept resident for mcba_undistort_images
-int mcba_undistort_map(mcba_ctx* ctx, int32_t model, const double* camera, int32_t width, int32_t height, float* map) {
-  return api(ctx, [&] {
-    check_camera(model, camera);
-    REQUIRE(width > 0 && height > 0 && height <= 65535, MCBA_ERR_ARG, "map size out of range");
-    undistortion_map(ctx, model, camera, width, height, map);
-    CK(cudaStreamSynchronize(ctx->stream));
-  });
-}
-
-// cv2.remap(src[i], map, None, INTER_CUBIC) for n images of one camera through its undistortion map, host to host (remap_images)
-int mcba_undistort_images(mcba_ctx* ctx, int32_t model, const double* camera, int32_t width, int32_t height, int32_t n,
-                          int32_t src_width, int32_t src_height, int32_t channels, int32_t dtype, const uint8_t* const* src,
-                          uint8_t* const* dst) {
-  return api(ctx, [&] {
-    check_camera(model, camera);
-    check_images(width, height, n, src_width, src_height, channels, dtype, src, dst);
-    if (n == 0) return;
-    const mcba_ctx::UndistortMap* m = undistortion_map(ctx, model, camera, width, height, nullptr);
-    remap_images(ctx, m, width, height, n, src_width, src_height, channels, src, dst);
-  });
-}
 
 // initUndistortRectifyMap(K, dist, R, P, (width, height)) of one camera, kept resident for mcba_rectify_images
 int mcba_rectify_map(mcba_ctx* ctx, int32_t model, const double* camera, const double* R, const double* P, int32_t width, int32_t height,
@@ -1725,10 +1684,6 @@ int mcba_rectify_points(mcba_ctx* ctx, int32_t model, const double* camera, cons
 
 int mcba_project_points(mcba_ctx* ctx, int32_t model, const double* camera, int64_t n, const double* points, double* pixels) {
   return api(ctx, [&] { run_points(ctx, true, model, camera, n, points, pixels); });
-}
-
-int mcba_undistort_points(mcba_ctx* ctx, int32_t model, const double* camera, int64_t n, const double* pixels, double* undistorted) {
-  return api(ctx, [&] { run_points(ctx, false, model, camera, n, pixels, undistorted); });
 }
 
 // the fixed-point bicubic weights k_remap_cubic reads, int32[1024][16]

@@ -5,9 +5,9 @@
 //   Camera.undistort_points camera.py:119-122, camera_fisheye.py:108-111   cv2.undistortPoints(pts, K, dist, P=K)
 //   Camera.project          camera.py:124-128, camera_fisheye.py:113-117   cv2.projectPoints(pts, 0, 0, K, dist)
 //
-// Map (k_undistort_map): R = I and newK = K.  The normalised coordinates come from K^-1 with the skew, y = (v - cy) / fy,
-// x = (u - cx - s y) / fx; the forward projection uses fx, fy, cx, cy only (OpenCV ignores K[0][1] there).  fp64 in a fixed order with
-// no fused multiply-adds (dmul/dadd below), cast to float32 at the end.  The same kernel writes the resident fixed-point form remap reads.
+// The undistortion map and points are the rectification ones below at R = I, P = K (k_rectify_map, k_rectify_points).  Map entries are
+// fp64 in a fixed order with no fused multiply-adds (dmul/dadd below), cast to float32 at the end; the map kernel also writes the
+// resident fixed-point form remap reads.
 //
 // Remap (k_remap_cubic): cv2.remap's fixed-point bicubic for uint8 with the constant-zero border.  X = rint(32 x), Y = rint(32 y) (ties
 // to even); the 4x4 taps start at (X >> 5) - 1, (Y >> 5) - 1 and their weights are entry (Y & 31) * 32 + (X & 31) of a 32 x 32 table of
@@ -112,18 +112,6 @@ struct UndistortCamera {
   int w, h;
 };
 
-template <int MODEL>
-__host__ __device__ inline void distorted_pixel(const UndistortCamera& c, double x, double y, float& mx, float& my);
-
-// initUndistortRectifyMap (R = I, newK = K) at pixel (u, v) -> float32 (mx, my)
-template <int MODEL>
-__host__ __device__ inline void undistort_map_pixel(const UndistortCamera& c, int u, int v, float& mx, float& my) {
-  const double fx = c.k[0], fy = c.k[1], cx = c.k[2], cy = c.k[3], s = c.k[4];
-  const double y = dadd((double)v, -cy) / fy;
-  const double x = dadd(dadd((double)u, -cx), -dmul(s, y)) / fx;
-  distorted_pixel<MODEL>(c, x, y, mx, my);
-}
-
 // the map entry of the normalised point (x, y): OpenCV's distortion and projection (fx, fy, cx, cy; K[0][1] unused), cast to float32
 template <int MODEL>
 __host__ __device__ inline void distorted_pixel(const UndistortCamera& c, double x, double y, float& mx, float& my) {
@@ -168,18 +156,6 @@ __host__ __device__ __forceinline__ void fixed_point_entry(float mx, float my, u
   const int sx = min(max(X >> 5, -32768), 32767), sy = min(max(Y >> 5, -32768), 32767);
   org = (uint32_t)(uint16_t)(int16_t)sx | ((uint32_t)(uint16_t)(int16_t)sy << 16);
   idx = (uint16_t)((Y & (UND_TAB - 1)) * UND_TAB + (X & (UND_TAB - 1)));
-}
-
-// one thread per pixel; grid (ceil(w / UND_THREADS), h).  fmap (float2 [h][w]) may be null.
-template <int MODEL>
-__global__ void __launch_bounds__(UND_THREADS) k_undistort_map(UndistortCamera c, float2* fmap, uint32_t* org, uint16_t* idx) {
-  const int u = blockIdx.x * blockDim.x + threadIdx.x, v = blockIdx.y;
-  if (u >= c.w) return;
-  float mx, my;
-  undistort_map_pixel<MODEL>(c, u, v, mx, my);
-  const size_t p = (size_t)v * c.w + u;
-  if (fmap) { float2 f; f.x = mx; f.y = my; fmap[p] = f; }
-  fixed_point_entry(mx, my, org[p], idx[p]);
 }
 
 struct RemapArgs {
@@ -247,78 +223,72 @@ __global__ void __launch_bounds__(UND_THREADS) k_project_points(UndistortCamera 
   uv[2 * i] = u; uv[2 * i + 1] = v;
 }
 
-// cv2.undistortPoints(pts, K, dist, P = K) / cv2.fisheye.undistortPoints: undistort_pixel<MODEL>, one thread each
-template <int MODEL>
-__global__ void __launch_bounds__(UND_THREADS) k_undistort_points(UndistortCamera c, int64_t n, const double* in, double* out) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  double u, v;
-  undistort_pixel<MODEL>(c.k, in[2 * i], in[2 * i + 1], u, v);
-  out[2 * i] = u; out[2 * i + 1] = v;
-}
-
 // ---- rectification: initUndistortRectifyMap(K, dist, R, P) and undistortPoints(pts, K, dist, R, P) --------------------------------------
 // ir = (P[:, :3] R)^-1 and rr = P[:, :3] R, both row-major fp64 from the host (its 3x3 Gaussian elimination); cam.w, cam.h are the map size.
+// Undistortion (initUndistortRectifyMap(K, dist, None, K), undistortPoints(P = K)) is this at R = I, P = K.
 //
 // Map (k_rectify_map): OpenCV walks each row i from (x, y, w) = i * ir[1, 4, 7] + ir[2, 5, 8] in steps of ir[0, 3, 6], and the
 // walk's rounding reaches the float32 map.  Pinhole (undistort.simd.hpp, 2 vectors of 4 doubles): blocks of RECT_BLOCK = 8 pixels
 // start at `cur`, pixel k of a block is cur + k * step, then cur += 8 * step while a whole block is left; the last W mod 8 pixels take
 // cur, then cur += step, one at a time.  x = _x * (1 / _w).  Fisheye (fisheye.cpp): one pixel at a time, cur += step, x = _x / _w, and
-// _w <= 0 gives an infinite map entry.  Three threads of the row's CTA write the walk's values (block starts, then the tail) into shared
-// memory, the CTA synchronises, and every thread finishes its pixels with distorted_pixel<MODEL>.
+// _w <= 0 gives an infinite map entry.  The walk of a row is a list of entries (block starts, then tail pixels; every pixel for the
+// fisheye), taken RECT_SEG at a time: three threads of the row's CTA write a segment's entries into shared memory, carrying `cur` over
+// from the segment before, the CTA synchronises, every thread finishes the segment's pixels with distorted_pixel<MODEL>, and the CTA
+// synchronises again before the next segment.  So a map has no width limit.
 constexpr int RECT_BLOCK = 8;
-constexpr int RECT_SMEM_MAX = 200 * 1024;          // the walk of one row: fisheye maps up to 8533 pixels wide
+constexpr int RECT_SEG = 512;                      // walk entries per segment: 12 KB of shared memory for x, y and w
 
 struct RectifyCamera {
   UndistortCamera cam;
   double ir[9], rr[9];
 };
 
-// entries of the walk one row keeps in shared memory: block starts and tail pixels (pinhole), every pixel (fisheye)
-__host__ __device__ __forceinline__ int rectify_walk_len(int model, int w) {
-  return model == MODEL_FISHEYE ? w : w / RECT_BLOCK + w % RECT_BLOCK;
-}
-
-// one CTA of UND_THREADS per map row; dynamic shared memory 3 * rectify_walk_len doubles.  fmap (float2 [h][w]) may be null.
+// one CTA of UND_THREADS per map row.  fmap (float2 [h][w]) may be null.
 template <int MODEL>
 __global__ void __launch_bounds__(UND_THREADS) k_rectify_map(RectifyCamera c, float2* fmap, uint32_t* org, uint16_t* idx) {
-  extern __shared__ double walk[];
-  const int w = c.cam.w, i = blockIdx.x, n = rectify_walk_len(MODEL, w);
+  __shared__ double walk[3][RECT_SEG];
   constexpr int B = MODEL == MODEL_FISHEYE ? 1 : RECT_BLOCK;
-  const int nb = w / B;                                  // whole blocks
-  if (threadIdx.x < 3) {
-    const int r = threadIdx.x;                           // 0: x, 1: y, 2: w
-    const double step = c.ir[3 * r], bstep = dmul((double)B, step);
-    double cur = dadd(dmul((double)i, c.ir[3 * r + 1]), c.ir[3 * r + 2]);
-    double* out = walk + r * n;
-    for (int b = 0; b < nb; b++) { out[b] = cur; cur = dadd(cur, bstep); }
-    for (int t = nb; t < n; t++) { out[t] = cur; cur = dadd(cur, step); }
-  }
-  __syncthreads();
-  for (int j = threadIdx.x; j < w; j += blockDim.x) {
-    double v[3];
-    const int b = j / B, k = j - b * B;
+  const int w = c.cam.w, i = blockIdx.x;
+  const int nb = w / B, n = nb + (w - nb * B);           // whole blocks; walk entries
+  const int r = threadIdx.x;                             // walker r < 3: 0 x, 1 y, 2 w
+  double cur = r < 3 ? dadd(dmul((double)i, c.ir[3 * r + 1]), c.ir[3 * r + 2]) : 0.0;
+  for (int e0 = 0; e0 < n; e0 += RECT_SEG) {
+    const int e1 = min(n, e0 + RECT_SEG);
+    if (r < 3) {
+      const double step = c.ir[3 * r], bstep = dmul((double)B, step);
+      int e = e0;
+      for (; e < min(e1, nb); e++) { walk[r][e - e0] = cur; cur = dadd(cur, bstep); }
+      for (; e < e1; e++) { walk[r][e - e0] = cur; cur = dadd(cur, step); }
+    }
+    __syncthreads();
+    // entry e < nb starts the pixels e B .. e B + B - 1, entry e >= nb is the pixel nb B + e - nb
+    const int j0 = min(e0, nb) * B + max(e0 - nb, 0), j1 = min(e1, nb) * B + max(e1 - nb, 0);
+    for (int j = j0 + threadIdx.x; j < j1; j += blockDim.x) {
+      double v[3];
+      const int b = j / B, k = j - b * B;
+      const int e = (b < nb ? b : nb + (j - nb * B)) - e0;
 #pragma unroll
-    for (int r = 0; r < 3; r++) {
-      const double* in = walk + r * n;
-      if (MODEL == MODEL_FISHEYE) v[r] = in[j];
-      else v[r] = b < nb ? dadd(in[b], dmul((double)k, c.ir[3 * r])) : in[nb + (j - nb * B)];
-    }
-    float mx, my;
-    if constexpr (MODEL == MODEL_FISHEYE) {
-      if (v[2] <= 0.0) {
-        mx = v[0] > 0.0 ? -INFINITY : INFINITY;
-        my = v[1] > 0.0 ? -INFINITY : INFINITY;
-      } else {
-        distorted_pixel<MODEL>(c.cam, v[0] / v[2], v[1] / v[2], mx, my);
+      for (int q = 0; q < 3; q++) {
+        if (MODEL == MODEL_FISHEYE) v[q] = walk[q][e];
+        else v[q] = b < nb ? dadd(walk[q][e], dmul((double)k, c.ir[3 * q])) : walk[q][e];
       }
-    } else {
-      const double iw = 1.0 / v[2];
-      distorted_pixel<MODEL>(c.cam, dmul(v[0], iw), dmul(v[1], iw), mx, my);
+      float mx, my;
+      if constexpr (MODEL == MODEL_FISHEYE) {
+        if (v[2] <= 0.0) {
+          mx = v[0] > 0.0 ? -INFINITY : INFINITY;
+          my = v[1] > 0.0 ? -INFINITY : INFINITY;
+        } else {
+          distorted_pixel<MODEL>(c.cam, v[0] / v[2], v[1] / v[2], mx, my);
+        }
+      } else {
+        const double iw = 1.0 / v[2];
+        distorted_pixel<MODEL>(c.cam, dmul(v[0], iw), dmul(v[1], iw), mx, my);
+      }
+      const size_t p = (size_t)i * w + j;
+      if (fmap) { float2 f; f.x = mx; f.y = my; fmap[p] = f; }
+      fixed_point_entry(mx, my, org[p], idx[p]);
     }
-    const size_t p = (size_t)i * w + j;
-    if (fmap) { float2 f; f.x = mx; f.y = my; fmap[p] = f; }
-    fixed_point_entry(mx, my, org[p], idx[p]);
+    __syncthreads();
   }
 }
 

@@ -1,10 +1,10 @@
 """Applying a finished calibration on the GPU: the reference's Camera.undistort_map, undistort_points and project (camera.py:113-128,
 camera_fisheye.py:102-117) and undistort_images (camera.py:244-258), which run OpenCV on the host there.
 
-The kernels are in csrc/undistort_kernels.cuh.  Maps are OpenCV's to the bit (R = I, newK = K), except rare 1-ulp fisheye values
-(DESIGN.md §3g); the remap is cv2.remap's fixed-point
-bicubic with the constant-zero border for uint8 images of 1 or 3 channels.  Everything runs on an engine of its own, so the bundle
-adjustment engine's uploaded problem survives it."""
+The kernels are in csrc/undistort_kernels.cuh.  Undistortion is the rectification of multical_b200/rectify.py at R = I, P = K, as it
+is in OpenCV: maps follow OpenCV's row walk (DESIGN.md §3g); the remap is cv2.remap's fixed-point bicubic with the constant-zero border
+for uint8 images of 1 or 3 channels.  Everything runs on an engine of its own, so the bundle adjustment engine's uploaded problem
+survives it."""
 import numpy as np
 
 from .camera import engine_model_of
@@ -30,10 +30,16 @@ def camera_vector(camera):
   return model, np.concatenate([[K[0, 0], K[1, 1], K[0, 2], K[1, 2], K[0, 1]], np.asarray(camera.dist, np.float64).reshape(-1)])
 
 
+def identity_rectification(cam):
+  """(R, P) = (I, K) of a camera vector: K with the skew, as OpenCV reads newCameraMatrix."""
+  fx, fy, cx, cy, s = cam[:5]
+  return np.eye(3), np.array([[fx, s, cx], [0, fy, cy], [0, 0, 1]])
+
+
 def undistort_map(camera):
   """float32 [h, w, 2]: cv2.initUndistortRectifyMap(K, dist, None, K, image_size, CV_32FC2), or the fisheye variant."""
   model, cam = camera_vector(camera)
-  return undistort_engine().undistort_map(model, cam, camera.image_size)
+  return undistort_engine().rectify_map(model, cam, *identity_rectification(cam), camera.image_size)
 
 
 def _out_dtype(points):
@@ -45,7 +51,7 @@ def undistort_points(camera, points):
   out, anything else float64, as OpenCV does."""
   points = np.asarray(points)
   model, cam = camera_vector(camera)
-  out = undistort_engine().undistort_points(model, cam, points.reshape(-1, 2))
+  out = undistort_engine().rectify_points(model, cam, *identity_rectification(cam), points.reshape(-1, 2))
   return out.astype(_out_dtype(points)).reshape(*points.shape[:-1], 2)
 
 
@@ -79,5 +85,5 @@ def undistort_images(images, cameras, j=None, chunksize=4):
     shapes = {np.shape(im) for im in cam_images}
     assert len(shapes) <= 1, f"camera {k}: images of one camera must share one shape, got {sorted(shapes)}"
     model, cam = camera_vector(camera)
-    out.append(eng.undistort_images(model, cam, camera.image_size, cam_images))
+    out.append(eng.rectify_images(model, cam, *identity_rectification(cam), camera.image_size, cam_images))
   return out

@@ -1,6 +1,6 @@
 """numpy restatement of OpenCV's rectification map, cv2.initUndistortRectifyMap(K, dist, R, P, size) and
-cv2.fisheye.initUndistortRectifyMap(K, D, R, P, size): the row walk whose rounding reaches the float32 map, then the distortion of
-oracle/undistort_oracle.py.  This is the arithmetic k_rectify_map (multical_b200/csrc/undistort_kernels.cuh) follows.
+cv2.fisheye.initUndistortRectifyMap(K, D, R, P, size): the row walk whose rounding reaches the float32 map, then the distortion.  At
+R = I, P = K it is the undistortion map.  This is the arithmetic k_rectify_map (multical_b200/csrc/undistort_kernels.cuh) follows.
 
 Row i starts at (x, y, w) = i * ir[:, 1] + ir[:, 2], ir = (P[:, :3] R)^-1, and steps by ir[:, 0]:
   pinhole  blocks of 8 pixels (OpenCV's SIMD loop, 2 vectors of 4 doubles): pixel k of a block is cur + k * step, then cur += 8 * step;

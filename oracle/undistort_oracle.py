@@ -1,7 +1,6 @@
-"""numpy restatement of what the reference does with OpenCV to apply a finished calibration (camera.py:113-128, 244-258;
-camera_fisheye.py:102-117): the undistortion map with R = I and newK = K (cv2.initUndistortRectifyMap,
-cv2.fisheye.initUndistortRectifyMap) and cv2.remap(image, map, None, INTER_CUBIC) with the default constant-zero border, for
-uint8 images.
+"""numpy restatement of what the reference does with OpenCV to remap an image through a finished calibration's map (camera.py:244-258):
+cv2.remap(image, map, None, INTER_CUBIC) with the default constant-zero border, for uint8 images, and OpenCV's sensor tilt matrix.  The
+map itself (R = I and newK = K for the undistortion) is restated in oracle/rectify_oracle.py.
 
 This is the arithmetic the device kernels in multical_b200/csrc/undistort_kernels.cuh follow; the tests compare both this and the
 device against live cv2.
@@ -90,41 +89,3 @@ def _tilt(tx, ty):
   R = Ry @ Rx
   Pz = np.array([[R[2, 2], 0, -R[0, 2]], [0, R[2, 2], -R[1, 2]], [0, 0, 1]])
   return Pz @ R
-
-
-def undistort_map(K, dist, size, fisheye=False):
-  """float32 [h][w][2] map of initUndistortRectifyMap(K, dist, None, K, size) (or the fisheye variant), in fp64.  The normalised
-  coordinates come from K^-1 (skew included); the forward projection uses fx, fy, cx, cy only, as OpenCV's does."""
-  w, h = size
-  K = np.asarray(K, np.float64)
-  fx, fy, cx, cy, s = K[0, 0], K[1, 1], K[0, 2], K[1, 2], K[0, 1]
-  v, u = np.mgrid[0:h, 0:w].astype(np.float64)
-  y = (v - cy) / fy
-  x = (u - cx - s * y) / fx
-  d = np.zeros(14)
-  dd = np.asarray(dist, np.float64).reshape(-1)
-  d[:dd.size] = dd
-  if fisheye:
-    r = np.sqrt(x * x + y * y)
-    th = np.arctan(r)
-    t2 = th * th
-    t4 = t2 * t2
-    thd = th * (1 + d[0] * t2 + d[1] * t4 + d[2] * (t4 * t2) + d[3] * (t4 * t4))
-    with np.errstate(invalid="ignore", divide="ignore"):
-      scale = np.where(r == 0, 1.0, thd / r)
-    mu, mv = fx * x * scale + cx, fy * y * scale + cy
-  else:
-    k1, k2, p1, p2, k3, k4, k5, k6, s1, s2, s3, s4, tx, ty = d
-    x2, y2 = x * x, y * y
-    r2 = x2 + y2
-    _2xy = 2 * x * y
-    kr = (1 + ((k3 * r2 + k2) * r2 + k1) * r2) / (1 + ((k6 * r2 + k5) * r2 + k4) * r2)
-    xd = x * kr + p1 * _2xy + p2 * (r2 + 2 * x2) + s1 * r2 + s2 * r2 * r2
-    yd = y * kr + p1 * (r2 + 2 * y2) + p2 * _2xy + s3 * r2 + s4 * r2 * r2
-    M = _tilt(tx, ty)
-    t0 = M[0, 0] * xd + M[0, 1] * yd + M[0, 2]
-    t1 = M[1, 0] * xd + M[1, 1] * yd + M[1, 2]
-    t2 = M[2, 0] * xd + M[2, 1] * yd + M[2, 2]
-    ip = np.where(t2 != 0, 1.0 / np.where(t2 != 0, t2, 1.0), 1.0)
-    mu, mv = fx * ip * t0 + cx, fy * ip * t1 + cy
-  return np.stack([mu, mv], -1).astype(np.float32)

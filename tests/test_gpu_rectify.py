@@ -7,7 +7,8 @@ Bars:
                           without CALIB_ZERO_DISPARITY
   stereo_rectify_fisheye  the same bars against cv2.fisheye.stereoRectify over balance and fov_scale
   maps                    bit-identical to cv2.initUndistortRectifyMap(K, d, R, P, size, CV_32FC2) for the five models (the fisheye twin's
-                          CV_32F pair stacked), with and without skew, at odd widths and a size unlike the image's
+                          CV_32F pair stacked), with and without skew, at odd widths and a size unlike the image's; rows longer than one
+                          segment of the kernel's row walk, for the rectification and the undistortion (R = I, P = K)
   images                  bit-identical to cv2.remap(image, OpenCV's map, None, INTER_CUBIC), 1 and 3 channels
   points                  within 1e-9 px of cv2.undistortPoints(R=R, P=P) and cv2.fisheye.undistortPoints(R, P)
   end to end              a pair calibrated by stereo_calibrate, rectified: noise-free detections land on equal rows (1e-6 px) and Q
@@ -21,7 +22,8 @@ import pytest
 
 from multical_b200 import rectify, undistort
 from multical_b200.camera import Camera, CameraFisheye, rectify_images, stereo_calibrate, stereo_rectify, stereo_rectify_fisheye
-from test_gpu_undistort import DIST, MODELS, images
+from test_gpu_undistort import DIST, MODELS, images, make_camera
+from test_gpu_undistort import cv_map as cv_undistort_map
 
 pytestmark = pytest.mark.gpu
 
@@ -127,6 +129,25 @@ def run_maps(sizes):
           assert m.shape == (size[1], size[0], 2) and m.dtype == np.float32
           bad = int((m.view(np.int32) != ref.view(np.int32)).sum())
           assert bad == 0, f"{model} {w}x{h} -> {size} skew {skew}: {bad} map values differ from OpenCV's"
+
+
+def run_wide_maps():
+  """k_rectify_map walks a row 512 entries (block starts, then tail pixels) at a time: a fisheye row of 9001 pixels takes 18 segments,
+  a pinhole row of 4109 (513 blocks of 8 and a tail of 5) has its last block and its tail in the second segment, and one of 4087 (510
+  blocks and a tail of 7) crosses into the second segment inside its tail."""
+  import cv2
+  rng = np.random.default_rng(9)
+  for model, w in (("fisheye", 9001), ("standard", 4109), ("thin_prism", 4087)):
+    h = 3
+    cam = make_camera(model, w, h, skew=1.5)
+    K = cam.intrinsic
+    R = cv2.Rodrigues(rng.normal(0, 0.05, 3))[0]
+    P = np.array([[K[0, 0] * 0.9, 0, w / 2 + 1.7, 0], [0, K[1, 1] * 0.9, h / 2 - 0.6, 0], [0, 0, 1, 0]])
+    for what, m, ref in (("undistort_map", cam.undistort_map, cv_undistort_map(cam)),
+                         ("rectify_map", cam.rectify_map(R, P), cv_map(cam, R, P, (w, h)))):
+      assert m.shape == (h, w, 2) and m.dtype == np.float32
+      bad = int((m.view(np.int32) != ref.view(np.int32)).sum())
+      assert bad == 0, f"{what} {model} {w}x{h}: {bad} map values differ from OpenCV's"
 
 
 def run_images(w, h):
@@ -276,6 +297,10 @@ def test_stereo_rectify_fisheye_matches_opencv():
 
 def test_maps_are_opencvs_bit_for_bit():
   run_maps([(1920, 1200), (641, 479), (97, 61)])
+
+
+def test_wide_maps_are_opencvs_bit_for_bit():
+  run_wide_maps()
 
 
 def test_rectify_images_are_cv2_remap_bit_for_bit():

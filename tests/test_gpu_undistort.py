@@ -1,11 +1,10 @@
-"""GPU (-m gpu): applying a finished calibration (multical_b200/undistort.py; include/mcba.h mcba_undistort_*, mcba_project_points;
-csrc/undistort_kernels.cuh) against OpenCV, called live.
+"""GPU (-m gpu): applying a finished calibration (multical_b200/undistort.py; include/mcba.h mcba_rectify_* at R = I, P = K,
+mcba_project_points; csrc/undistort_kernels.cuh) against OpenCV, called live.
 
 Bars:
   maps             bit-identical to cv2.initUndistortRectifyMap(K, dist, None, K, size, CV_32FC2) for the standard, rational, thin
-                   prism and tilted models, with and without skew, at odd sizes; the fisheye map against
-                   cv2.fisheye.initUndistortRectifyMap(..., CV_32F) stacked to [h, w, 2] (OpenCV 4.13 refuses CV_32FC2 there) within
-                   1 float32 ulp on at most 4 values (OpenCV's row accumulation, DESIGN.md §3g), bit-identical everywhere else
+                   prism and tilted models, and to cv2.fisheye.initUndistortRectifyMap(..., CV_32F) stacked to [h, w, 2] (OpenCV 4.13
+                   refuses CV_32FC2 there) for the fisheye, with and without skew, at odd sizes
   remap            bit-identical to cv2.remap(image, OpenCV's map, None, INTER_CUBIC): 1 and 3 channels, maps that leave the image,
                    source images larger and smaller than the map
   undistort_images bit-identical to the reference's per-image cv2.remap(image, camera.undistort_map, None, INTER_CUBIC) over a batch of
@@ -73,12 +72,8 @@ def run_maps(sizes):
         cam = make_camera(model, w, h, skew)
         m, ref = cam.undistort_map, cv_map(cam)
         assert m.shape == (h, w, 2) and m.dtype == np.float32
-        ulps = np.abs(m.view(np.int32).astype(np.int64) - ref.view(np.int32))
-        bad = int((ulps != 0).sum())
-        if model == "fisheye":                     # OpenCV accumulates x along each row there: DESIGN.md §3g
-          assert ulps.max() <= 1 and bad <= 4, f"fisheye {w}x{h} skew {skew}: {bad} map values differ, up to {ulps.max()} ulp"
-        else:
-          assert bad == 0, f"{model} {w}x{h} skew {skew}: {bad} map values differ from OpenCV's"
+        bad = int((m.view(np.int32) != ref.view(np.int32)).sum())
+        assert bad == 0, f"{model} {w}x{h} skew {skew}: {bad} map values differ from OpenCV's"
 
 
 def run_remap(w, h):
@@ -89,7 +84,7 @@ def run_remap(w, h):
     assert (ref_map[..., 0] < -1).any() or (ref_map[..., 0] > w).any(), "the map should leave the image"
     for shape in [(h, w), (h, w, 3), (h + 7, w + 13), (h - 9, w - 5, 3), (h // 2 + 1, w // 3 + 2)]:
       src = images(rng, 2, shape)
-      out = undistort.undistort_engine().undistort_images(*undistort.camera_vector(cam), cam.image_size, src)
+      out = undistort_images([src], [cam])[0]
       for i, (a, b) in enumerate(zip(out, (cv_remap(s, ref_map) for s in src))):
         assert a.shape == b.shape and a.dtype == np.uint8, (a.shape, b.shape)
         bad = int((a != b).sum())
@@ -145,14 +140,12 @@ def run_points(w, h, n):
 
 def run_reproducible(w, h):
   rng = np.random.default_rng(3)
-  eng = undistort.undistort_engine()
   for model in MODELS:
     cam = make_camera(model, w, h, skew=0.5)
-    mv = undistort.camera_vector(cam)
-    a, b = eng.undistort_map(*mv, cam.image_size), eng.undistort_map(*mv, cam.image_size)
+    a, b = undistort.undistort_map(cam), undistort.undistort_map(cam)
     assert np.array_equal(a.view(np.int32), b.view(np.int32))
     src = images(rng, 3, (h, w, 3))
-    x, y = eng.undistort_images(*mv, cam.image_size, src), eng.undistort_images(*mv, cam.image_size, src)
+    x, y = undistort_images([src], [cam])[0], undistort_images([src], [cam])[0]
     assert all(np.array_equal(p, q) for p, q in zip(x, y))
     X = rng.uniform(0.5, 2.0, (64, 3))
     assert np.array_equal(cam.project(X), cam.project(X))
@@ -176,17 +169,18 @@ def run_errors(w, h):
   # the C ABI: unsupported dtype or channel count -> MCBA_ERR_ARG (1)
   eng = undistort.undistort_engine()
   model, vec = undistort.camera_vector(cam)
-  U8 = C.POINTER(C.c_uint8)
+  R, P = (np.ascontiguousarray(a).ravel() for a in undistort.identity_rectification(vec))
+  U8, D = C.POINTER(C.c_uint8), C.POINTER(C.c_double)
   src, dst = ok.copy(), np.zeros_like(ok)
   sp, dp = (U8 * 1)(src.ctypes.data_as(U8)), (U8 * 1)(dst.ctypes.data_as(U8))
-  vp = vec.ctypes.data_as(C.POINTER(C.c_double))
+  vp, rp, pp = vec.ctypes.data_as(D), R.ctypes.data_as(D), P.ctypes.data_as(D)
   for dtype, channels in [(1, 1), (0, 2), (0, 4), (-1, 3)]:
-    rc = eng.lib.mcba_undistort_images(eng.h, 0, vp, w, h, 1, w, h, channels, dtype, sp, dp)
+    rc = eng.lib.mcba_rectify_images(eng.h, 0, vp, rp, pp, w, h, 1, w, h, channels, dtype, sp, dp)
     assert rc == 1, (dtype, channels, rc)
-  assert eng.lib.mcba_undistort_images(eng.h, 0, vp, w, h, 1, w, h, 1, 0, sp, dp) == 0
+  assert eng.lib.mcba_rectify_images(eng.h, 0, vp, rp, pp, w, h, 1, w, h, 1, 0, sp, dp) == 0
   bad = vec.copy(); bad[5] = np.nan
   with pytest.raises(ValueError, match="non-finite"):
-    eng.undistort_points(model, bad, np.zeros((1, 2)))
+    eng.rectify_points(model, bad, *undistort.identity_rectification(bad), np.zeros((1, 2)))
 
 
 def test_maps_are_opencvs_bit_for_bit():

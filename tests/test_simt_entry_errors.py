@@ -115,13 +115,14 @@ ROWS = [
   ("mcba_hand_eye_vote", None, lambda L, h: L.mcba_hand_eye_vote(h, 1, p(np.array([0, 3], np.int64)), p(z(3, 3)), p(z(3)), p(z(1, dtype=np.int32))),
    DEGENERATE, "set 0 has 3 points"),
   # ---- applying a calibration
-  ("mcba_undistort_map", None, lambda L, h: L.mcba_undistort_map(h, 0, p(np.r_[0.0, CAM[1:]]), 8, 8, None), ARG, "zero focal length"),
-  ("mcba_undistort_map", None, lambda L, h: L.mcba_undistort_map(h, 0, p(CAM), 0, 8, None), ARG, "map size out of range"),
-  ("mcba_undistort_images", None, lambda L, h: L.mcba_undistort_images(h, 0, p(CAM), 8, 8, 1, 8, 8, 1, 1, u8pp(1), u8pp(1)),
+  ("mcba_rectify_map", None, lambda L, h: L.mcba_rectify_map(h, 0, p(np.r_[0.0, CAM[1:]]), p(R3), p(R3), 8, 8, None), ARG, "zero focal length"),
+  ("mcba_rectify_map", None, lambda L, h: L.mcba_rectify_map(h, 0, p(CAM), p(R3), p(R3), 0, 8, None), ARG, "map size out of range"),
+  ("mcba_rectify_images", None, lambda L, h: L.mcba_rectify_images(h, 0, p(CAM), p(R3), p(R3), 8, 8, 1, 8, 8, 1, 1, u8pp(1), u8pp(1)),
    ARG, "unsupported image dtype"),
   ("mcba_project_points", None, lambda L, h: L.mcba_project_points(h, 9, p(CAM), 1, p(z(3)), p(z(2))), ARG, "unknown camera model"),
-  ("mcba_undistort_points", None, lambda L, h: L.mcba_undistort_points(h, 0, None, 1, p(z(2)), p(z(2))), ARG, "null camera"),
-  ("mcba_undistort_points", None, lambda L, h: L.mcba_undistort_points(h, 0, p(CAM), -1, p(z(2)), p(z(2))), ARG, "negative point count"),
+  ("mcba_rectify_points", None, lambda L, h: L.mcba_rectify_points(h, 0, None, p(R3), p(R3), 1, p(z(2)), p(z(2))), ARG, "null camera"),
+  ("mcba_rectify_points", None, lambda L, h: L.mcba_rectify_points(h, 0, p(CAM), p(R3), p(R3), -1, p(z(2)), p(z(2))), ARG,
+   "negative point count"),
   ("mcba_remap_cubic_table", None, lambda L, h: L.mcba_remap_cubic_table(h, None), ARG, "null table"),
   ("mcba_rectify_map", None, lambda L, h: L.mcba_rectify_map(h, 0, p(CAM), None, p(R3), 8, 8, None), ARG, "null R or P"),
   ("mcba_rectify_map", None, lambda L, h: L.mcba_rectify_map(h, 0, p(CAM), p(R3), p(z(3, 3)), 8, 8, None), ARG, "P R is singular"),

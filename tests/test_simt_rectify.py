@@ -1,9 +1,11 @@
 """CPU (-m "not gpu"): the checks of tests/test_gpu_rectify.py on the SIMT interpreter (tests/simt) at small sizes, and the numpy
-restatement of OpenCV's row walk (oracle/rectify_oracle.py) against live cv2 on random R and P, at widths that are not multiples of 8."""
+restatement of OpenCV's row walk (oracle/rectify_oracle.py) against live cv2 on random R and P, at widths that are not multiples of 8,
+and at R = I, P = K (the undistortion map)."""
 import numpy as np
 import pytest
 
 import test_gpu_rectify as gr
+import test_gpu_undistort as gu
 from multical_b200 import undistort
 from oracle import rectify_oracle as ro
 from test_simt_kernels import on_the_interpreter, simt_library  # noqa: F401  (fixtures)
@@ -30,6 +32,11 @@ def test_oracle_walk_is_opencvs():
       ref = gr.cv_map(cams[0], R, P, size)
       ours = ro.rectify_map(K, d, R, P, size, fisheye=model == "fisheye")
       assert np.array_equal(ours.view(np.int32), ref.view(np.int32)), (model, w, h)
+  for model in gr.MODELS:
+    for skew in (0.0, 2.5):
+      cam = gu.make_camera(model, 97, 61, skew=skew)
+      ours = ro.rectify_map(cam.intrinsic, cam.dist, np.eye(3), cam.intrinsic, cam.image_size, fisheye=model == "fisheye")
+      assert np.array_equal(ours.view(np.int32), gu.cv_map(cam).view(np.int32)), (model, skew)
 
 
 def test_stereo_rectify_matches_opencv():
@@ -42,6 +49,10 @@ def test_stereo_rectify_fisheye_matches_opencv():
 
 def test_maps_are_opencvs_bit_for_bit():
   gr.run_maps([(64, 48), (37, 23)])
+
+
+def test_wide_maps_are_opencvs_bit_for_bit():
+  gr.run_wide_maps()
 
 
 def test_rectify_images_are_cv2_remap_bit_for_bit():

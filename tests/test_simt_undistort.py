@@ -34,14 +34,6 @@ def test_oracle_remap_is_cv2_remap():
     assert np.array_equal(uo.remap_cubic(src, m), cv2.remap(src, m, None, cv2.INTER_CUBIC)), shape
 
 
-def test_oracle_map_is_opencvs():
-  for model in gu.MODELS:
-    cam = gu.make_camera(model, 97, 61, skew=2.5)
-    ref = gu.cv_map(cam)
-    assert np.array_equal(uo.undistort_map(cam.intrinsic, cam.dist, cam.image_size, fisheye=model == "fisheye").view(np.int32),
-                          ref.view(np.int32)), model
-
-
 def test_maps_are_opencvs_bit_for_bit():
   gu.run_maps([(64, 48), (37, 23)])
 
