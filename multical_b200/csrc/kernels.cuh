@@ -396,11 +396,45 @@ k_views(DeviceProblem p, ViewKernelArgs a) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// One fp64 tensor-core step (mma.sync m8n8k4 "DMMA"; wgmma has no fp64 kind): the 8x8 C fragment, two doubles per lane, += A (8x4) B (4x8).
-// k_linearize accumulates its per-view moment SYRKs with it, k_lm the Schur complement.
+// fp64 tensor-core steps (mma.sync "DMMA"; wgmma has no fp64 kind): the 16x8 C fragment += A (16xK) B (Kx8), K = 8 or 4.
+// k_linearize accumulates its per-view moment SYRKs and the view epilogue's products with them, k_lm the Schur complement.  Fragments
+// (PTX ISA "Matrix fragments for mma.m16n8k*", .f64), lane = 4 grp + tig:
+//   a[i] = A[grp + 8 (i & 1)][tig + 4 (i >> 1)]     b[i] = B[tig + 4 i][grp]     c[i] = C[grp + 8 (i >> 1)][2 tig + (i & 1)]
+// On an H100 (SXM, 700 W) the m16n8k* shapes run at 128 MAC/clk/SM, twice the rate of m8n8k4 (scripts/dmma_shapes.cu).  A host build
+// of the sources (no __CUDA_ARCH__) composes each shape from m8n8k4 steps: rows grp and grp + 8 are two m8n8k4 with the same B.
 __device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double b) {
   asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
                : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
+}
+__device__ __forceinline__ void dmma1688(double (&c)[4], const double (&a)[4], const double (&b)[2]) {
+#ifdef __CUDA_ARCH__
+  asm __volatile__("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                   : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3]) : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(b[0]), "d"(b[1]));
+#else
+  dmma884(c[0], c[1], a[0], b[0]); dmma884(c[2], c[3], a[1], b[0]);      // k = tig
+  dmma884(c[0], c[1], a[2], b[1]); dmma884(c[2], c[3], a[3], b[1]);      // k = tig + 4
+#endif
+}
+__device__ __forceinline__ void dmma1684(double (&c)[4], const double (&a)[2], const double (&b)[1]) {
+#ifdef __CUDA_ARCH__
+  asm __volatile__("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
+                   : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3]) : "d"(a[0]), "d"(a[1]), "d"(b[0]));
+#else
+  dmma884(c[0], c[1], a[0], b[0]); dmma884(c[2], c[3], a[1], b[0]);
+#endif
+}
+// C += A B over K = 4 NQ: m16n8k8 steps, and m16n8k4 for an odd last quad.  a[q][h] = A[grp + 8 h][4 q + tig], b[q] = B[4 q + tig][grp].
+template <int NQ>
+__device__ __forceinline__ void dmma_quads(double (&c)[4], const double (&a)[NQ][2], const double (&b)[NQ]) {
+#pragma unroll
+  for (int q = 0; q + 1 < NQ; q += 2) {
+    const double a8[4] = {a[q][0], a[q][1], a[q + 1][0], a[q + 1][1]}, b8[2] = {b[q], b[q + 1]};
+    dmma1688(c, a8, b8);
+  }
+  if constexpr (NQ % 2 == 1) {
+    const double a4[2] = {a[NQ - 1][0], a[NQ - 1][1]}, b4[1] = {b[NQ - 1]};
+    dmma1684(c, a4, b4);
+  }
 }
 // columns of a staged residual row [G | r]: the local Jacobian (D, plus 6 for the second twist block of rolling frames) and r, padded to 8
 __host__ __device__ constexpr int mma_nc(int model, bool roll = false) { return ((model_D(model) + (roll ? 6 : 0) + 1 + 7) / 8) * 8; }

@@ -2,7 +2,7 @@
 // expansion into the block-arrow normal equations, in ONE kernel that reads every corner once and writes nothing per corner or per view.
 //
 //   k_linearize<MODEL, ROLL>   one CTA per frame (persistent, static frame -> CTA map), warps own the frame's views by camera:
-//                              per view   M = sum [G r]^T [G r]  (mma.sync.m8n8k4.f64, view_chunk below)
+//                              per view   M = sum [G r]^T [G r]  (mma.sync.m16n8k4.f64, view_chunk below)
 //                              epilogue   the view's 6x6 twist maps (camera / frame / board pose -> camera-frame twist) applied to M:
 //                                         H_ff, g_f, W_f (this frame's block row of the arrow) are COMPLETE when the CTA leaves the frame and
 //                                         are stored once; the shared-parameter blocks are accumulated per (CTA, camera) in a record that
@@ -40,21 +40,23 @@ struct LinShape {
   static constexpr int E = D * (D + 1) / 2;
   static constexpr int T = E + D + 1;               // moment record: upper triangle | G^T r | cost
   static constexpr int NC = mma_nc(MODEL, ROLL);    // staged columns (D + 1 padded to 8)
-  static constexpr int NT = NC / 8;
-  static constexpr int NPAIR = NT * (NT + 1) / 2;
+  static constexpr int NT = NC / 8;                 // 8-column tiles of M
+  static constexpr int NMB = (NC + 15) / 16;        // 16-row blocks of M
+  static constexpr int NBLK = NMB * NT - NMB * (NMB - 1);   // 16 x 8 C blocks on or above the diagonal: (mb, J) with J >= 2 mb
   static constexpr int KINT = 5 + ND;
   static constexpr int FB = KO;                     // parameters of one eliminated frame block
   static constexpr int UB = D * 6 + 42;             // per (camera, board): M[:,xi] Ab (D x 6) | Ab^T M Ab (36) | Ab^T g (6)
 };
 
 // One 32-corner chunk of a view: every lane computes its corner's residual pair and 2 x D Jacobian rows (fp64), the warp stages
-// [G | r] (64 rows x NC columns) in shared memory and accumulates M += [G r]^T [G r] into the DMMA C fragments `acc`.
+// [G | r] (64 rows x NC columns) in shared memory and accumulates M += [G r]^T [G r] into the DMMA C fragments `acc`: block t = (mb, J)
+// of the enumeration mb = 0.., J = 2 mb .. NT-1 holds M[16 mb .. 16 mb + 15][8 J .. 8 J + 7].
 template <int MODEL, bool ROLL>
 __device__ __forceinline__ void view_chunk(const DeviceProblem& p, int loss, double f_scale, const ViewPose& vp, const ViewPose& vpe, const double* k,
                                            const double* bp, double inv_h, int base, int end, int lane, double* stage,
-                                           double (&acc)[LinShape<MODEL, ROLL>::NPAIR][2], double& cost_acc, double2 ob, int pi) {
+                                           double (&acc)[LinShape<MODEL, ROLL>::NBLK][4], double& cost_acc, double2 ob, int pi) {
   using S = LinShape<MODEL, ROLL>;
-  constexpr int ND = S::ND, D = S::D, NC = S::NC, NT = S::NT;
+  constexpr int ND = S::ND, D = S::D, NC = S::NC, NT = S::NT, NMB = S::NMB;
   const int grp = lane >> 2, tig = lane & 3;
   const int idx = base + lane;
   double gu[NC], gv[NC];
@@ -84,19 +86,25 @@ __device__ __forceinline__ void view_chunk(const DeviceProblem& p, int loss, dou
         *reinterpret_cast<double2*>(stage + j * LIN_KPAD + 2 * (lane & 15)) = make_double2(gu[j], gv[j]);
     }
     __syncwarp();
-    // k-steps of 4 residual rows; fragment of column tile I = Gt[k0 + tig][8 I + grp] serves as A (row tile) and B (col tile)
+    // m16n8k4 steps of 4 residual rows; fr[I] = Gt[k0 + tig][8 I + grp] of column tile I: tiles 2 mb, 2 mb + 1 are the A fragment of row
+    // block mb (a tile past NC reads as zero), tile J is the B fragment of block (mb, J)
     const int rows = 2 * max(0, min(16, cnt - 16 * half));
     const int ksteps = (rows + 3) >> 2;                          // ragged last chunk: skip all-zero row groups
-#pragma unroll 4
-    for (int ks = 0; ks < ksteps; ks++) {
-      double fr[NT];
 #pragma unroll
-      for (int I = 0; I < NT; I++) fr[I] = stage[(8 * I + grp) * LIN_KPAD + 4 * ks + tig];
+    for (int ks = 0; ks < 8; ks++) {
+      if (ks >= ksteps) break;
+      double fr[2 * NMB];
+#pragma unroll
+      for (int I = 0; I < 2 * NMB; I++) fr[I] = I < NT ? stage[(8 * I + grp) * LIN_KPAD + 4 * ks + tig] : 0.0;
       int t = 0;
 #pragma unroll
-      for (int I = 0; I < NT; I++)
+      for (int mb = 0; mb < NMB; mb++)
 #pragma unroll
-        for (int J = I; J < NT; J++) { dmma884(acc[t][0], acc[t][1], fr[I], fr[J]); t++; }
+        for (int J = 2 * mb; J < NT; J++) {
+          const double a[2] = {fr[2 * mb], fr[2 * mb + 1]}, b[1] = {fr[J]};
+          dmma1684(acc[t], a, b);
+          t++;
+        }
     }
     __syncwarp();
   }
@@ -148,8 +156,9 @@ template <int MODEL, bool ROLL>
 struct LinLayout {
   using S = LinShape<MODEL, ROLL>;
   static constexpr int PC = 6 * (S::NP + 1);                    // columns of the map matrix E: frame-pose block(s) | board-pose block
-  static constexpr int PT = (PC + 7) / 8;                       // 8-row tiles of T^t = E^T M[xi, :]
-  static constexpr int KS = (S::KO + 3) / 4;                    // k-steps over the twist components
+  static constexpr int PT = (PC + 7) / 8;                       // 8-row tiles of T^t = E^T M[xi, :] (rows of T^t held, columns of E)
+  static constexpr int PM = (PC + 15) / 16;                     // 16-row blocks of the products: rows past 8 PT are zero, never loaded or stored
+  static constexpr int KS = (S::KO + 3) / 4;                    // quads of twist components: m16n8k8 steps, m16n8k4 for an odd last quad
   static constexpr int EK = 4 * KS;                             // rows of E (twist components), zero padded to the k-steps
   static constexpr int EP = 8 * PT + 4;                         // row stride of E; strides mod 16 == 4 or 12: the mma fragment loads
   static constexpr int MSTR = S::NC + 4;                        //   (address = 4-lane group x stride + lane in group) hit 16 different banks
@@ -158,12 +167,12 @@ struct LinLayout {
   static constexpr int Tt = Ms + MR * MSTR;                     // [8 PT][LIN_TSTR]   T^t[:, xi]
   static constexpr int stage_need = Tt + 8 * PT * LIN_TSTR;     // what the epilogue needs
   static constexpr int stage_end = ((S::NC * LIN_KPAD > stage_need ? S::NC * LIN_KPAD : stage_need) + 1) & ~1;
-  static_assert((2 * S::NPAIR + 1) * 32 <= stage_end, "the fragments of a view part must fit the warp's stage buffer");
+  static_assert((4 * S::NBLK + 1) * 32 <= stage_end, "the fragments of a view part must fit the warp's stage buffer");
   static_assert(EK <= LIN_TSTR && (MSTR % 16 == 4 || MSTR % 16 == 12) && (EP % 16 == 4 || EP % 16 == 12), "fragment strides");
   static constexpr int NHF = S::FB * S::FB + S::FB;             // H_ff | g_f
   static constexpr int NWC = S::D * S::FB;                      // sum over the camera's boards of Tf = M[:, xi] Af (D x FB)
   // scatter tables (per CTA, one entry per lane): where the C fragments of the epilogue's products and of the moment tiles are added
-  static constexpr int NTT = PT * S::NT * 2, NTP = PT * PT * 2, NTM = S::NPAIR * 2;
+  static constexpr int NTT = PM * S::NT * 4, NTP = PM * PT * 4, NTM = S::NBLK * 4;
   // after the stage buffer: E [EK][EP] | chain (R_cf 9, t_cf 3) x NP | Wb [B][6][FB] | hacc [NHF] | wacc [NWC] | macc [T] | ub [UB] | tail [6]
   static constexpr int E = stage_end;
   static constexpr int chain = E + EK * EP;
@@ -282,7 +291,8 @@ __device__ __noinline__ void lin_flush(const DeviceProblem* p, const LinArgs* a,
 // (rows = twist components):
 //     T^t = E^T M[xi, :]      rows f: Tf^t (-> W_f camera / intrinsics rows, g_f)      rows b: Tb^t (-> camera x board blocks, board gradient)
 //     P   = T^t[:, xi] E      (f,f) -> H_ff      (b,f) -> W_f board rows      (b,b) -> board x board block
-// both products on the fp64 tensor path (mma.m8n8k4, 8 + 8 instructions for the 5-coefficient model); every lane adds its C fragments
+// both products on the fp64 tensor path (m16n8k8, 2 + 2 instructions for static frames; rolling frames' 12 twist components add an
+// m16n8k4 per C block); every lane adds its C fragments
 // to the warp's running sums at offsets it reads from the CTA's scatter tables (no index arithmetic, no branches on the element's role).
 // A call, not inlined: the chunk loop of the kernel keeps its registers.
 template <int MODEL, bool ROLL>
@@ -290,7 +300,7 @@ __device__ __noinline__ void lin_view_epilogue(int B, bool frames_on, bool board
                                                const short (*tabT)[32], const short (*tabP)[32], int b, double cost_acc, bool new_chain) {
   using S = LinShape<MODEL, ROLL>; using L = LinLayout<MODEL, ROLL>;
   constexpr int NP = S::NP, T = S::T, NT = S::NT, FB = S::FB;
-  constexpr int PT = L::PT, KS = L::KS, EP = L::EP, MSTR = L::MSTR, EK = L::EK;
+  constexpr int PT = L::PT, PM = L::PM, KS = L::KS, EP = L::EP, MSTR = L::MSTR, EK = L::EK;
   const int lane = threadIdx.x & 31, grp = lane >> 2, tig = lane & 3;
   double* Ms = w + L::Ms; double* Tt = w + L::Tt;
   double* Em = w + L::E; const double* chain = w + L::chain;
@@ -321,37 +331,47 @@ __device__ __noinline__ void lin_view_epilogue(int B, bool frames_on, bool board
   __syncwarp();
   // ---- T^t = E^T M[xi, :]
 #pragma unroll
-  for (int I = 0; I < PT; I++) {
-    double fa[KS];
+  for (int I = 0; I < PM; I++) {
+    double fa[KS][2];
 #pragma unroll
-    for (int ks = 0; ks < KS; ks++) fa[ks] = Em[(4 * ks + tig) * EP + 8 * I + grp];
+    for (int ks = 0; ks < KS; ks++)
+#pragma unroll
+      for (int h = 0; h < 2; h++) fa[ks][h] = 16 * I + 8 * h < 8 * PT ? Em[(4 * ks + tig) * EP + 16 * I + 8 * h + grp] : 0.0;
 #pragma unroll
     for (int J = 0; J < NT; J++) {
-      double c0 = 0.0, c1 = 0.0;
+      double fb[KS], c[4] = {0.0, 0.0, 0.0, 0.0};
 #pragma unroll
-      for (int ks = 0; ks < KS; ks++) dmma884(c0, c1, fa[ks], Ms[(4 * ks + tig) * MSTR + 8 * J + grp]);
-      if (8 * J < EK) { if (8 * J + 2 * tig < EK) *reinterpret_cast<double2*>(Tt + (8 * I + grp) * LIN_TSTR + 8 * J + 2 * tig) = make_double2(c0, c1); }
-      const int o0 = tabT[(I * NT + J) * 2][lane], o1 = tabT[(I * NT + J) * 2 + 1][lane];
-      if (o0 >= 0) w[o0] += c0;
-      if (o1 >= 0) w[o1] += c1;
+      for (int ks = 0; ks < KS; ks++) fb[ks] = Ms[(4 * ks + tig) * MSTR + 8 * J + grp];
+      dmma_quads<KS>(c, fa, fb);
+#pragma unroll
+      for (int h = 0; h < 2; h++)
+        if (16 * I + 8 * h < 8 * PT && 8 * J < EK && 8 * J + 2 * tig < EK)
+          *reinterpret_cast<double2*>(Tt + (16 * I + 8 * h + grp) * LIN_TSTR + 8 * J + 2 * tig) = make_double2(c[2 * h], c[2 * h + 1]);
+#pragma unroll
+      for (int i = 0; i < 4; i++) { const int o = tabT[(I * NT + J) * 4 + i][lane]; if (o >= 0) w[o] += c[i]; }
     }
   }
   __syncwarp();
   // ---- P = T^t[:, xi] E
   const int wb = b * 6 * FB;
 #pragma unroll
-  for (int I = 0; I < PT; I++) {
-    double fa[KS];
+  for (int I = 0; I < PM; I++) {
+    double fa[KS][2];
 #pragma unroll
-    for (int ks = 0; ks < KS; ks++) fa[ks] = Tt[(8 * I + grp) * LIN_TSTR + 4 * ks + tig];
+    for (int ks = 0; ks < KS; ks++)
+#pragma unroll
+      for (int h = 0; h < 2; h++) fa[ks][h] = 16 * I + 8 * h < 8 * PT ? Tt[(16 * I + 8 * h + grp) * LIN_TSTR + 4 * ks + tig] : 0.0;
 #pragma unroll
     for (int J = 0; J < PT; J++) {
-      double c0 = 0.0, c1 = 0.0;
+      double fb[KS], c[4] = {0.0, 0.0, 0.0, 0.0};
 #pragma unroll
-      for (int ks = 0; ks < KS; ks++) dmma884(c0, c1, fa[ks], Em[(4 * ks + tig) * EP + 8 * J + grp]);
-      const int o0 = tabP[(I * PT + J) * 2][lane], o1 = tabP[(I * PT + J) * 2 + 1][lane];
-      if (o0 >= 0) w[(o0 & (LIN_WB_FLAG - 1)) + ((o0 & LIN_WB_FLAG) ? wb : 0)] += c0;
-      if (o1 >= 0) w[(o1 & (LIN_WB_FLAG - 1)) + ((o1 & LIN_WB_FLAG) ? wb : 0)] += c1;
+      for (int ks = 0; ks < KS; ks++) fb[ks] = Em[(4 * ks + tig) * EP + 8 * J + grp];
+      dmma_quads<KS>(c, fa, fb);
+#pragma unroll
+      for (int i = 0; i < 4; i++) {
+        const int o = tabP[(I * PT + J) * 4 + i][lane];
+        if (o >= 0) w[(o & (LIN_WB_FLAG - 1)) + ((o & LIN_WB_FLAG) ? wb : 0)] += c[i];
+      }
     }
   }
   __syncwarp();
@@ -362,7 +382,7 @@ template <int MODEL, bool ROLL>
 __global__ void __launch_bounds__(LIN_THREADS, 2)
 k_linearize(DeviceProblem p, LinArgs a) {
   using S = LinShape<MODEL, ROLL>; using L = LinLayout<MODEL, ROLL>;
-  constexpr int NIN = S::NIN, D = S::D, T = S::T, NC = S::NC, NT = S::NT, NPAIR = S::NPAIR, KINT = S::KINT, FB = S::FB, NP = S::NP;
+  constexpr int NIN = S::NIN, D = S::D, T = S::T, NC = S::NC, NT = S::NT, NBLK = S::NBLK, KINT = S::KINT, FB = S::FB, NP = S::NP;
   extern __shared__ double lsm[];
   __shared__ int fv_cam[LIN_MAXV], fv_board[LIN_MAXV], fv_start[LIN_MAXV + 1];
   __shared__ int any_view;
@@ -392,17 +412,18 @@ k_linearize(DeviceProblem p, LinArgs a) {
   {
     constexpr int PC = L::PC, PT = L::PT, E_ = S::E;
     const bool boards_on = p.off_bp >= 0;
+    // C fragment slot i of a 16 x 8 block: row grp + 8 (i >> 1), column 2 tig + (i & 1)
     for (int o = tid; o < L::NTT * 32; o += nthreads) {
-      const int e = o >> 5, l = o & 31, I = e / (NT * 2), J = (e >> 1) % NT, h = e & 1;
-      const int pp = 8 * I + (l >> 2), j = 8 * J + 2 * (l & 3) + h;
+      const int e = o >> 5, l = o & 31, I = (e >> 2) / NT, J = (e >> 2) % NT, i = e & 3;
+      const int pp = 16 * I + (l >> 2) + 8 * (i >> 1), j = 8 * J + 2 * (l & 3) + (i & 1);
       int off = -1;
       if (pp < 6 * NP) { if (frames_on) { if (j < D) off = L::wacc(B) + j * FB + pp; else if (j == D) off = L::hacc(B) + FB * FB + pp; } }
       else if (pp < PC && boards_on) { const int r = pp - 6 * NP; if (j < D) off = L::ub(B) + j * 6 + r; else if (j == D) off = L::ub(B) + D * 6 + 36 + r; }
       tabT[e][l] = (short)off;
     }
     for (int o = tid; o < L::NTP * 32; o += nthreads) {
-      const int e = o >> 5, l = o & 31, I = e / (PT * 2), J = (e >> 1) % PT, h = e & 1;
-      const int pp = 8 * I + (l >> 2), q = 8 * J + 2 * (l & 3) + h;
+      const int e = o >> 5, l = o & 31, I = (e >> 2) / PT, J = (e >> 2) % PT, i = e & 3;
+      const int pp = 16 * I + (l >> 2) + 8 * (i >> 1), q = 8 * J + 2 * (l & 3) + (i & 1);
       int off = -1;
       if (pp < FB) { if (frames_on && q < FB) off = L::hacc(B) + pp * FB + q; }
       else if (pp < PC && boards_on) {
@@ -413,10 +434,10 @@ k_linearize(DeviceProblem p, LinArgs a) {
       tabP[e][l] = (short)off;
     }
     for (int o = tid; o < L::NTM * 32; o += nthreads) {
-      const int e = o >> 5, l = o & 31, h = e & 1;
-      int t = e >> 1, I = 0;
-      while (t >= NT - I) { t -= NT - I; I++; }
-      const int J = I + t, i = 8 * I + (l >> 2), j = 8 * J + 2 * (l & 3) + h;
+      const int e = o >> 5, l = o & 31, s = e & 3;
+      int t = e >> 2, mb = 0;
+      while (t >= NT - 2 * mb) { t -= NT - 2 * mb; mb++; }
+      const int J = 2 * mb + t, i = 16 * mb + (l >> 2) + 8 * (s >> 1), j = 8 * J + 2 * (l & 3) + (s & 1);      // i > j below the diagonal
       int off = -1;
       if (i < D && j < D && i <= j) off = L::macc(B) + tri_index(D, i, j);
       else if (i < D && j == D) off = L::macc(B) + E_ + i;
@@ -501,9 +522,11 @@ k_linearize(DeviceProblem p, LinArgs a) {
         __syncthreads();
         if (!any_view) break;
       }
-      double acc[NPAIR][2];
+      double acc[NBLK][4];
 #pragma unroll
-      for (int i = 0; i < NPAIR; i++) { acc[i][0] = 0.0; acc[i][1] = 0.0; }
+      for (int t = 0; t < NBLK; t++)
+#pragma unroll
+        for (int i = 0; i < 4; i++) acc[t][i] = 0.0;
       double cost_acc = 0.0;
       int c = 0, b = 0;
       bool new_chain = false;
@@ -562,16 +585,20 @@ k_linearize(DeviceProblem p, LinArgs a) {
         if (have && !leader) {
           double* xr = w;                      // this warp's stage buffer is free between two views
 #pragma unroll
-          for (int t = 0; t < NPAIR; t++) { xr[(2 * t) * 32 + lane] = acc[t][0]; xr[(2 * t + 1) * 32 + lane] = acc[t][1]; }
-          if (lane == 0) xr[2 * NPAIR * 32] = cost_acc;
+          for (int t = 0; t < NBLK; t++)
+#pragma unroll
+            for (int i = 0; i < 4; i++) xr[(4 * t + i) * 32 + lane] = acc[t][i];
+          if (lane == 0) xr[4 * NBLK * 32] = cost_acc;
         }
         __syncthreads();
         if (have && leader) {
           for (int q = 1; q < split; q++) {
             const double* xr = lsm + (size_t)(warp + q) * wd;
 #pragma unroll
-            for (int t = 0; t < NPAIR; t++) { acc[t][0] += xr[(2 * t) * 32 + lane]; acc[t][1] += xr[(2 * t + 1) * 32 + lane]; }
-            cost_acc += xr[2 * NPAIR * 32];
+            for (int t = 0; t < NBLK; t++)
+#pragma unroll
+              for (int i = 0; i < 4; i++) acc[t][i] += xr[(4 * t + i) * 32 + lane];
+            cost_acc += xr[4 * NBLK * 32];
           }
         }
       }
@@ -590,18 +617,19 @@ k_linearize(DeviceProblem p, LinArgs a) {
         }
         // the camera's raw moment sum (upper triangle | G^T r) straight from the fragments; rows xi of M -> Ms for the epilogue's products
         double* Ms = w + L::Ms;
+        // (the 8 x 8 tile of a diagonal block below the diagonal, I > J, is the mirror of a tile above it: neither summed nor stored)
         int t = 0;
 #pragma unroll
-        for (int I = 0; I < NT; I++)
+        for (int mb = 0; mb < S::NMB; mb++)
 #pragma unroll
-          for (int J = I; J < NT; J++) {
+          for (int J = 2 * mb; J < NT; J++) {
 #pragma unroll
-            for (int h = 0; h < 2; h++) {
-              const int o = tabM[2 * t + h][lane];
-              if (o >= 0) w[o] += acc[t][h];
-              const int i = 8 * I + grp, j = 8 * J + 2 * tig + h;
-              if (8 * I < L::EK) Ms[i * L::MSTR + j] = acc[t][h];
-              if (I != J && 8 * J < L::EK) Ms[j * L::MSTR + i] = acc[t][h];
+            for (int s = 0; s < 4; s++) {
+              const int o = tabM[4 * t + s][lane];
+              if (o >= 0) w[o] += acc[t][s];
+              const int I = 2 * mb + (s >> 1), i = 8 * I + grp, j = 8 * J + 2 * tig + (s & 1);
+              if (I <= J && 8 * I < L::EK) Ms[i * L::MSTR + j] = acc[t][s];
+              if (I < J && 8 * J < L::EK) Ms[j * L::MSTR + i] = acc[t][s];
             }
             t++;
           }

@@ -278,9 +278,9 @@ __device__ __forceinline__ void syrk_tile(const LmArgs& a, int ti, int tj, int c
   const int qd = warp & 3, I2 = qd >> 1, J2 = qd & 1, kh = warp >> 2;
   const int pg = 2 * (grp & 3) + (grp >> 2);                 // row of the 8-row fragment this lane group reads
   const int nsteps = (f1 - f0 + SYRK_FR - 1) / SYRK_FR;
-  double c[8];
+  double c[2][4];                                             // C blocks of column halves 0 | 1 of the warp's 16 x 16 block
 #pragma unroll
-  for (int q = 0; q < 8; q++) c[q] = 0.0;
+  for (int q = 0; q < 8; q++) c[q >> 2][q & 3] = 0.0;
   double racc = 0.0;
   __syncthreads();                                            // every warp has left the previous tile's stages
   fence_proxy_async();                                        // (also orders the previous phase's plain stores to this buffer before the copies)
@@ -303,18 +303,21 @@ __device__ __forceinline__ void syrk_tile(const LmArgs& a, int ti, int tj, int c
     const double* Yi = sh + (size_t)st * STAGE; const double* Yj = Yi + SYRK_K * SYRK_TILE;
     const int fbase = f0 + step * SYRK_FR, nf = min(SYRK_FR, f1 - fbase);
 #pragma unroll
-    for (int ks2 = 0; ks2 < SYRK_K / 8; ks2++) {
-      const int ks = 2 * ks2 + kh;
-      const int kidx = 4 * ks + tig, ff = kidx / FB, k = kidx % FB;          // k-column -> (frame of the step, component)
-      const double* yi = Yi + ff * FR_DOUBLES + (16 * I2 + pg) * FB + k;
-      const double* yj = Yj + ff * FR_DOUBLES + (16 * J2 + pg) * FB + k;
-      // a chunk's last step may hold fewer frames than a stage: what lies behind them is a previous step's data, not zeros
-      const bool on = ff < nf;
-      const double fa0 = on ? yi[0] : 0.0, fa1 = on ? yi[8 * FB] : 0.0, fb0 = on ? yj[0] : 0.0, fb1 = on ? yj[8 * FB] : 0.0;
-      dmma884(c[0], c[1], fa0, fb0);
-      dmma884(c[2], c[3], fa0, fb1);
-      dmma884(c[4], c[5], fa1, fb0);
-      dmma884(c[6], c[7], fa1, fb1);
+    for (int ks2 = 0; ks2 < SYRK_K / 16; ks2++) {
+      const int ks = 2 * ks2 + kh;                            // m16n8k8 step: k-columns 8 ks + tig (+ 4)
+      double fa[4], fb[2][2];
+#pragma unroll
+      for (int q = 0; q < 2; q++) {
+        const int kidx = 8 * ks + 4 * q + tig, ff = kidx / FB, k = kidx % FB;          // k-column -> (frame of the step, component)
+        const double* yi = Yi + ff * FR_DOUBLES + (16 * I2 + pg) * FB + k;
+        const double* yj = Yj + ff * FR_DOUBLES + (16 * J2 + pg) * FB + k;
+        // a chunk's last step may hold fewer frames than a stage: what lies behind them is a previous step's data, not zeros
+        const bool on = ff < nf;
+        fa[2 * q] = on ? yi[0] : 0.0; fa[2 * q + 1] = on ? yi[8 * FB] : 0.0;
+        fb[0][q] = on ? yj[0] : 0.0; fb[1][q] = on ? yj[8 * FB] : 0.0;
+      }
+      dmma1688(c[0], fa, fb[0]);
+      dmma1688(c[1], fa, fb[1]);
     }
     if (ti == tj) {                                           // rhs: thread (row = tid % 32, frame slot = tid / 32 (+ 8 for 4-frame steps: none))
       const int r = tid & 31, ff = tid >> 5;
@@ -342,12 +345,12 @@ __device__ __forceinline__ void syrk_tile(const LmArgs& a, int ti, int tj, int c
   // the second k-half's fragments go through shared memory to the warp that owns the same block and are added there
   if (kh == 1) {
 #pragma unroll
-    for (int q = 0; q < 8; q++) sh[(qd * 8 + q) * 32 + lane] = c[q];
+    for (int q = 0; q < 8; q++) sh[(qd * 8 + q) * 32 + lane] = c[q >> 2][q & 3];
   }
   __syncthreads();
   if (kh == 0) {
 #pragma unroll
-    for (int q = 0; q < 8; q++) c[q] += sh[(qd * 8 + q) * 32 + lane];
+    for (int q = 0; q < 8; q++) c[q >> 2][q & 3] += sh[(qd * 8 + q) * 32 + lane];
     const int p0 = 2 * ((2 * tig) & 3) + ((2 * tig) >> 2), p1 = 2 * ((2 * tig + 1) & 3) + ((2 * tig + 1) >> 2);      // columns of the C fragment's two entries
 #pragma unroll
     for (int ra = 0; ra < 2; ra++)
@@ -356,8 +359,8 @@ __device__ __forceinline__ void syrk_tile(const LmArgs& a, int ti, int tj, int c
         const int i = ti * SYRK_TILE + 16 * I2 + 8 * ra + pg;
         const int jb = tj * SYRK_TILE + 16 * J2 + 8 * cb;
         if (i < n_s) {
-          if (jb + p0 < n_s) Sp[(size_t)i * n_s + jb + p0] = c[(2 * ra + cb) * 2];
-          if (jb + p1 < n_s) Sp[(size_t)i * n_s + jb + p1] = c[(2 * ra + cb) * 2 + 1];
+          if (jb + p0 < n_s) Sp[(size_t)i * n_s + jb + p0] = c[cb][2 * ra];
+          if (jb + p1 < n_s) Sp[(size_t)i * n_s + jb + p1] = c[cb][2 * ra + 1];
         }
       }
   }
